@@ -32,6 +32,7 @@ sharded  : beside the headline every line carries `"sharded"`: BASELINE configs 
            over min(16 N, host cores) threads (independent/checker's fan-out).
 """
 import argparse
+import atexit
 import json
 import os
 import subprocess
@@ -68,7 +69,7 @@ def config_block(args, n_gpus):
                         f"tau_op 10 ms, tau_think {args.think_ms} ms, seed 1+key, "
                         f"{'one stale read (invalid)' if args.invalid else 'linearizable (valid)'}",
             "keys": n_gpus, "sharding": "one key (ledger) per GPU" if n_gpus > 1 else "single key",
-            "l2": "level windows up to 16 GiB and level arrays of 2 GB (45 M configurations per level) exceed the 126 MB L2",
+            "l2": "level windows up to 16 GiB and level arrays of 2 GB (45 M configurations per level) exceed the 50 MB L2",
             "model": "bank", "table": "16 B slots, linear probing, per-level window of 16 slots per configuration",
             "engine": "level-synchronous (csrc/jtb_level.cuh)",
             "search_space": "eager-read reduction (product default)" if args.eager_reads else
@@ -151,7 +152,8 @@ def run_sharded_reference(args, world):
 
 
 class ClockSampler:
-    """nvidia-smi clocks during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks during the timed region, with the card's name and power limit (a rate means little without
+    them).  Read-only queries; the sampling process is killed at exit even when the bench fails."""
 
     def __init__(self, index):
         self.rows, self.proc, self.index = [], None, index
@@ -159,11 +161,12 @@ class ClockSampler:
     def start(self):
         q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
              "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
-             "clocks_event_reasons.sw_power_cap")
+             "clocks_event_reasons.sw_power_cap,power.limit,name")
         try:
             self.proc = subprocess.Popen(["nvidia-smi", f"--id={self.index}", f"--query-gpu={q}",
                                           "--format=csv,noheader,nounits", "-lms", "100"],
                                          stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True)
+            atexit.register(self.proc.kill)
             threading.Thread(target=self._read, daemon=True).start()
         except OSError:
             self.proc = None
@@ -177,7 +180,8 @@ class ClockSampler:
             return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"]}
         time.sleep(0.15)
         self.proc.terminate()
-        sm, mx, reasons = [], [], set()
+        self.proc.wait()
+        sm, mx, reasons, limit, name = [], [], set(), None, None
         names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
         for r in self.rows:
             try:
@@ -187,8 +191,10 @@ class ClockSampler:
             for nm, v in zip(names, r[3:7]):
                 if v.lower().startswith("active"):
                     reasons.add(nm)
-        return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": max(mx) if mx else None,
-                "reasons": sorted(reasons), "samples": len(sm)}
+            if len(r) >= 9:
+                limit, name = r[7], r[8]
+        return {"gpu": name, "power_limit_w": limit, "sm_mhz": float(np.median(sm)) if sm else None,
+                "sm_max_mhz": max(mx) if mx else None, "reasons": sorted(reasons), "samples": len(sm)}
 
 
 def peak_hbm():
@@ -198,17 +204,7 @@ def peak_hbm():
             return float(json.load(open(p))["hbm_gbs"]), "of measured (MEASURED_PEAKS.json)"
         except Exception:  # noqa: BLE001
             pass
-    return 6650.0, "of fallback (B200_PROFILING.md)"
-
-
-def traffic_from_profile():
-    p = os.path.join(ROOT, "profiles", "bench_traffic.json")
-    if os.path.exists(p):
-        try:
-            return json.load(open(p))
-        except Exception:  # noqa: BLE001
-            pass
-    return None
+    return 3350.0, "of the H100 SXM data sheet's HBM3 bandwidth (not measured)"
 
 
 def reduced_search_check(h, m, args):
@@ -225,6 +221,24 @@ def reduced_search_check(h, m, args):
         return {"algo": "oracle ALGO_LAZY_BANK", "unavailable": str(e)}
     return {"algo": "oracle ALGO_LAZY_BANK (reduced search, CPU, 1 thread)", "verdict": {0: "valid", 1: "unknown", 2: "invalid"}[r["valid"]],
             "witness_index": r["shards"][0]["witness_index"], "configs": r["configs"], "seconds": time.perf_counter() - t}
+
+
+def dump_outputs(path, merged, res):
+    """What the last timed step returned, as float64 arrays: the merged verdict per key and this rank's result of the
+    C-ABI call.  Timings and probe counts (which depend on the order of concurrent table inserts) are left out, so the
+    same arguments give the same files and two builds can be compared file by file."""
+    os.makedirs(path, exist_ok=True)
+    arrays = {
+        "verdict": [merged["valid"]],
+        "shard_valid": merged["shard_valid"],
+        "shard_witness_index": merged["shard_witness"],
+        "shard_previous_ok_index": [s["previous_ok_index"] for s in res["shards"]],
+        "shard_cause": [s["cause"] for s in res["shards"]],
+        "n_failures": [res["n_failures"]],
+        "configs": [res["configs"]],
+    }
+    for name, a in arrays.items():
+        np.save(os.path.join(path, f"{name}.npy"), np.asarray(a, dtype=np.float64))
 
 
 def run_reference(args, rank, world):
@@ -302,7 +316,11 @@ def main():
     ap.add_argument("--eager-reads", action="store_true",
                     help="time the product default (eager-read reduction: ~18x fewer configs, same verdict) instead of "
                          "the Knossos-exact search space the CPU reference explores")
+    ap.add_argument("--dump-outputs", metavar="DIR",
+                    help="write what the last timed step computed to DIR/<name>.npy (float64)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
@@ -352,6 +370,7 @@ def main():
     verdict = None
     for _ in range(args.steps):
         out = step()
+        res = dict(last)
         verdict = out["valid"]
         kern_s += last["seconds_kernel"]
         configs += last["configs"]; probes += last["probes"]; algo_bytes += last["hbm_bytes_algorithmic"]
@@ -378,13 +397,11 @@ def main():
         with native.Context(device=local_rank) as sctx:      # product defaults (eager reads, scouts)
             sharded = run_sharded_ours(args, sctx, rank, world, reduce_max, dist, dev)
     configs_t, probes_t, bytes_t, launches_t, h2d_t, d2h_t = (float(x) for x in tot.cpu())
+    if rank == 0 and args.dump_outputs:
+        dump_outputs(args.dump_outputs, out, res)
     if rank == 0:
         peak, peak_src = peak_hbm()
         achieved = bytes_t / world / kern_max / 1e9  # per GPU, GB/s (algorithmic bytes / launch time)
-        tr = traffic_from_profile()
-        if tr and not (args.think_ms == tr.get("think_ms", 0.0) and args.ops == 10000 and args.clients == 32
-                       and not args.eager_reads and not args.invalid):
-            tr = None   # the capture is of the default workload only
         line = {
             "metric": METRIC, "value": configs_t / kern_max, "unit": UNIT, "n_gpus": world,
             "steps": args.steps, "warmup": max(args.warmup, 3), "ms_per_step": 1e3 * wall_max / args.steps,
@@ -398,12 +415,10 @@ def main():
                     "h2d_bytes_per_step": h2d_t / args.steps, "d2h_bytes_per_step": d2h_t / args.steps},
             "gpu_launches": int(launches_t),
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                         "frac": achieved / peak, "traffic": tr["dram_bytes_per_launch"] if tr else None,
-                         "traffic_source": tr.get("source") if tr else None,
+                         "frac": achieved / peak,
                          "peak_source": peak_src, "kernel": last["stats"].get("engine_level") and "level_search_kernel<bank,KW=2,exact>"
                          or "wgl_search_kernel<bank,KW=2>",
-                         "algorithmic_bytes": "16 B x (probes + inserts) per launch (SURVEY 8(d))",
-                         "random_probe_ceiling_GBps": tr.get("table_probe_algo_GBps") if tr else None},
+                         "algorithmic_bytes": "16 B x (probes + inserts) per launch (SURVEY 8(d))"},
             "clocks": clocks,
         }
         line["per_rank_kernel_s_per_step"] = [x / args.steps for x in per_rank_kern]

@@ -1,5 +1,5 @@
 (ns jtb.checker
-  "Clojure glue for the B200 history checker: jepsen.checker/Checker implementations that flatten the history, call
+  "Clojure glue for the H100 history checker: jepsen.checker/Checker implementations that flatten the history, call
   libjtb_check.so through jtb.Native (java/jtb/Native.java -> jni/jtb_jni.c) and build the SAME result maps the
   reference's checkers return.
 

@@ -1,5 +1,5 @@
 /*
- * jtb_check.h — C ABI of the B200-native history checker (libjtb_check.so).
+ * jtb_check.h — C ABI of the H100-native history checker (libjtb_check.so).
  *
  * This is the drop-in boundary for the ONE hot path of nurturenature/jepsen-tigerbeetle that this
  * repo accelerates: the history checkers that sit behind the Clojure protocol
@@ -350,7 +350,7 @@ int jtb_table_bench(jtb_ctx* ctx, uint64_t n_keys, int variant, int rounds,
  * Every thread issues `iters` rounds of `in_flight` (1, 2, 4, 8, 16) independent random 16 B loads (the search
  * kernel's ld.global.cg.v2.u64 probe; wide = 2: both halves of the 32 B sector) over a table of table_bytes
  * (rounded down to a power of two), ctas_per_sm x 256 threads per SM.  Returns the best of `rounds` timings and the
- * number of 16 B-slot probes issued.  profiles/ holds the sweep 64 MiB .. 16 GiB (DESIGN.md §4).               */
+ * number of 16 B-slot probes issued.  scripts/probe_sweep.py runs it over table sizes and in-flight depths.     */
 int jtb_gather_bench(jtb_ctx* ctx, uint64_t table_bytes, int in_flight, int wide, uint32_t iters, int ctas_per_sm,
                      int rounds, double* seconds, uint64_t* n_probes);
 

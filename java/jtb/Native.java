@@ -1,7 +1,7 @@
 package jtb;
 
 /**
- * JNI surface of the B200 history checker: one static native method per C-ABI entry point of libjtb_check.so
+ * JNI surface of the H100 history checker: one static native method per C-ABI entry point of libjtb_check.so
  * (include/jtb_check.h), implemented by jni/jtb_jni.c (libjtb_jni.so).  Used by clj/jtb/checker.clj.
  *
  * <p>A flattened history travels as ONE {@code Object[14]} of primitive arrays laid out like {@code struct

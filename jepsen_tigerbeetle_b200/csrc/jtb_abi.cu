@@ -99,7 +99,7 @@ int launch_wgl_b(jtb_ctx* ctx, const WglParams& p, int neg_ok, int grid, size_t 
 }
 
 // two builds of the kernel: Knossos-exact space (no eager-read code, 64 regs, JTB_CTAS_EXACT CTAs/SM) and the
-// eager-read default (78 regs, no spills, JTB_CTAS_EAGER CTAs/SM)
+// eager-read default (up to 80 regs, JTB_CTAS_EAGER CTAs/SM)
 template <int MODEL, int KW>
 int launch_wgl(jtb_ctx* ctx, const WglParams& p, int neg_ok, int grid, size_t smem, int ctas_per_sm) {
     (void)ctas_per_sm;
@@ -410,7 +410,7 @@ struct ScoutGuard {
 };
 
 // CUDA loads kernels lazily, and loading one synchronizes the context: the first launch of a search / compact /
-// re-hash kernel would wait for the running scouts (measured: the search sat behind them for 16 s).  So every kernel
+// re-hash kernel would wait for the running scouts (for seconds).  So every kernel
 // a search can need is loaded before the scouts start.
 template <typename K>
 int preload(jtb_ctx* ctx, K kernel) {
@@ -607,7 +607,7 @@ static int check_lin_impl(jtb_ctx* ctx, const jtb_history* h, const jtb_model* m
             P.n_ranks < LV_MAX_RANKS && !force_engine &&
             !(ctx->opts.flags & (JTB_OPT_NO_BEAM | JTB_OPT_ENGINE_LEVEL | JTB_OPT_ENGINE_WORKLIST)) && !getenv("JTB_NO_BEAM") &&
             !getenv("JTB_SCOUT_ONLY") && !getenv("JTB_ENGINE")) {
-            // A budgeted run of the work list first (16 M configurations, no scouts: ~20 ms): easy histories — most
+            // A budgeted run of the work list first (16 M configurations, no scouts): easy histories — most
             // histories with a few crashed ops — end there, at the work list's latency; only what it leaves open gets
             // the beam ladder.
             if (!ctx->in_probe) {
@@ -667,12 +667,12 @@ static int check_lin_impl(jtb_ctx* ctx, const jtb_history* h, const jtb_model* m
         }
         if (!searchable.empty()) {
         // ---- engine: level-synchronous sweep (jtb_level.cuh) or work list (jtb_wgl.cuh / jtb_search.cuh) ----------
-        // Default choice (measured, profiles/r2_engines.md): histories with crashed ops -> work list (its depth-first
+        // Default choice: histories with crashed ops -> work list (its depth-first
         // order + scouts find the linearization of a valid history long before a breadth-first sweep would);
-        // Knossos-exact space -> level engine (wide levels: 1.2-4 G configs/s against 0.9, bounded memory);
+        // Knossos-exact space -> level engine (higher throughput on wide levels, bounded memory);
         // eager reads (product default) -> the search is narrow unless ~every client always has an op in flight
         // (mean open ops per frontier row >= 26 of 32): narrow searches are a chain of short levels, where the work
-        // list's ~7 us per dependent step beats a grid barrier per level (67 vs 99 ms on the 10k-op bank history).
+        // list's dependent steps are cheaper than a grid barrier per level.
         bool use_level = P.max_nc == 0 && (!eager_mode || P.mean_open >= 26.0);
         if (ctx->opts.flags & JTB_OPT_ENGINE_LEVEL) use_level = true;
         if (ctx->opts.flags & JTB_OPT_ENGINE_WORKLIST) use_level = false;
@@ -761,7 +761,7 @@ static int check_lin_impl(jtb_ctx* ctx, const jtb_history* h, const jtb_model* m
             if (bytes <= b.cap) return 0;
             if (b.p) { if (scouts.active) deferred.push_back(b.p); else cudaFree(b.p); }
             b = DevBuf();
-            // cudaMalloc also synchronizes with running kernels (measured: the search sat behind the scouts for 16 s at
+            // cudaMalloc also synchronizes with running kernels (the search would sit behind the scouts for seconds at
             // its first table growth); the stream-ordered allocator does not
             const cudaError_t e = scouts.active ? cudaMallocAsync(&b.p, bytes, ctx->stream) : cudaMalloc(&b.p, bytes);
             if (e != cudaSuccess) {

@@ -3,15 +3,15 @@
 // Replaces the hot loop of knossos.wgl/analysis (SURVEY.md A.5: `step` over every call entry that may be linearized
 // next, then `cache.add((linearized BitSet, model))`) for exhaustive searches.  Same configurations, same keys, same
 // per-thread expansion core (jtb_expand.h) as the work-list engines (jtb_wgl.cuh / jtb_search.cuh); what differs is the
-// ORDER, and what that order buys on a B200:
+// ORDER, and what that order buys on an H100:
 //
 //   depth(config) = number of linearized ops = frontier rank + popcount(open-slot mask) + crashed-class counts is a
 //   function of the key, and every move adds exactly one.  So two equal configurations always meet IN THE SAME LEVEL:
 //   the visited set only has to live for one level.  The engine keeps two level arrays (ping-pong, coalesced) and ONE
 //   small hash window sized to the level (16 slots per configuration, 6-bit epoch tag in every slot, stale entries are
 //   simply overwritten: no clearing, no growth, no re-hash, no pause/resume).  At the bench sizes the window is a few
-//   MB — the probe stream runs out of the 126 MB L2 (measured 287 G random 16 B probes/s, profiles/r2_probe_sweep.json)
-//   instead of HBM (36.6 G/s) — and memory no longer bounds the search: 10^10-configuration spaces fit.
+//   MB — the probe stream runs out of the 50 MB L2 instead of HBM — and memory no longer bounds the search:
+//   10^10-configuration spaces fit in 80 GB.
 //
 //   Inside a level, a warp takes 32 configurations: phase 1, one lane per configuration, finds the candidate ops
 //   (bit masks from the frontier row); phase 2 hands EVERY child of the 32 configurations to its own lane (prefix sum

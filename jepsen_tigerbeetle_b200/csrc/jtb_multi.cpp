@@ -1,6 +1,6 @@
 // jtb_multi.cpp — multi-GPU fan-out inside the library (include/jtb_check.h, "jtb_multi_*").
 //
-// The B200 shape of `independent/checker` (src/tigerbeetle/workloads/set_full.clj:155) for a single-process host
+// The multi-GPU shape of `independent/checker` (src/tigerbeetle/workloads/set_full.clj:155) for a single-process host
 // (a JVM through JNI): shards = independent keys, partitioned over the devices of the box by LPT on events^2, one
 // host thread and one jtb_ctx per device, no configuration ever crosses GPUs.  The only collective is ONE
 // ncclAllReduce(ncclMax) over int32[3 * n_shards] — (verdict, witness :index, previous-ok :index) per shard, verdict

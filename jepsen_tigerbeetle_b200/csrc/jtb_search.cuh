@@ -6,7 +6,7 @@
 //   jtb_wgl.cuh   a WARP expands one configuration, lane t evaluates open slot t.  Every child of a configuration is
 //                 probed in the same round trip, which is what a latency-bound search wants (eager reads: ~1 new
 //                 config per rank, 10k dependent ranks), but it costs ~550 warp instructions per configuration with
-//                 half the lanes idle (ncu, profiles/r1_wgl_search_ncu.md) — instruction-bound at 0.9 G configs/s.
+//                 half the lanes idle — instruction-bound.
 //   this file     a THREAD expands one configuration (jtb_expand.h): candidate slots come from two bit masks in the
 //                 frontier row, a bank read is rejected by one 32-bit hash compare, a transfer child needs no balance
 //                 arithmetic until it turns out to be NEW (its balances are then patched in the queue entry), the

@@ -1,6 +1,6 @@
 // jtb_table_bench.cuh — the visited-config table (K2) in isolation: insert + probe micro-benchmark used
-// for the roofline evidence in DESIGN.md / profiles/.  Keys are pseudo-random 128-bit values; the
-// table is sized >> L2 (126 MB) so probes are honest HBM traffic.
+// for the roofline evidence in DESIGN.md.  Keys are pseudo-random 128-bit values; the
+// table is sized >> L2 (50 MB) so probes are honest HBM traffic.
 //
 // Probe variants:
 //   0  slot probing     one lane per key, ld.global.cg.v2.u64 of the 16 B home slot, linear probing
@@ -205,7 +205,7 @@ __global__ void __launch_bounds__(128) tb_probe_buckets_tma(const uint64_t* tabl
 // Every thread walks its own pseudo-random slot sequence (xorshift32 + one multiply: the address generation costs a
 // handful of instructions, so the ALUs are not what is measured) with U independent 16 B loads (ld.global.cg.v2.u64,
 // exactly the search kernel's probe) in flight; WIDE = 2 also loads the other half of the 32 B sector.  The loaded
-// words are folded into a checksum so nothing is optimised away.  Footprints from 64 MiB (L2-resident: 126 MB L2) to
+// words are folded into a checksum so nothing is optimised away.  Footprints from a few MiB (inside the 50 MB L2) to
 // 16 GiB show where random 16 B probes stop being served by L2 and what DRAM / the TLBs sustain beyond it.
 template <int U, int WIDE>
 __global__ void __launch_bounds__(256) tb_gather(const uint64_t* __restrict__ table, uint64_t slot_mask, uint32_t iters,

@@ -1,7 +1,7 @@
-// jtb_wgl.cuh — Wing–Gong/Lowe linearizability search as a persistent sm_100a kernel.
+// jtb_wgl.cuh — Wing–Gong/Lowe linearizability search as a persistent sm_90a kernel.
 //
 // Replaces the hot loop of knossos.wgl/analysis behind jepsen.checker/linearizable (SURVEY.md §3.3,
-// A.5): `cache.add((linearized BitSet, model))` + `model.step`.  B200-first formulation:
+// A.5): `cache.add((linearized BitSet, model))` + `model.step`.  GPU-first formulation:
 //
 //  * A configuration is keyed EXACTLY by its window form
 //        word0 = valid | global return rank of the first un-linearized :ok op | register state
@@ -17,8 +17,8 @@
 //  * Work distribution: depth-first locally, breadth-first globally, no locks.
 //      - each CTA keeps a LIFO deque in shared memory shared by its 8 warps (deep dives find the
 //        linearization of a valid history quickly).  A barrier-free variant with one private deque per
-//        warp was also measured: correct, but 1.5x slower (private stacks fragment the work: 100 M idle
-//        polls vs 6 M) even though bar.sync is the top stall reason of this version (ncu, profiles/);
+//        warp was also measured: correct, but slower (private stacks fragment the work: many more idle
+//        polls) even though bar.sync is the top stall reason of this version;
 //      - an idle warp takes a read TICKET (ring position from atomicAdd(head)) on a global FIFO ring in HBM
 //        and polls that slot; head - tail > 0 is therefore the number of hungry warps;
 //      - a CTA whose deque is nearly full, or that sees hungry warps, donates its OLDEST entries with one
@@ -472,8 +472,8 @@ struct CtaShared {
 
 __device__ __forceinline__ uint64_t ld_volatile64(const uint64_t* p) { return *(const volatile uint64_t*)p; }
 
-// MINB = resident CTAs per SM the register budget is cut for: 4 (64 regs, 32 warps/SM) is best for large,
-// throughput-bound searches; 3 (78 regs, no spills) is 11-17 % faster on small latency-bound ones (measured A/B).
+// MINB = resident CTAs per SM the register budget is cut for: 4 (64 regs, 32 warps/SM) for large,
+// throughput-bound searches; 3 (up to 80 regs, fewer spills) for small latency-bound ones.
 template <int MODEL, int KW, int MINB, bool EAGER>
 __global__ void __launch_bounds__(WGL_THREADS, MINB) wgl_search_kernel(const WglParams p, const int neg_ok) {
     using L = EntryLayout<MODEL, KW>;

@@ -1,7 +1,7 @@
 """Multi-GPU fan-out of a keyed history: one process per GPU, shards (independent keys) partitioned
 across ranks, ONE tiny collective to merge the verdicts.
 
-This is the B200 shape of `jepsen.independent/checker` (workloads/set_full.clj:155): linearizability is
+This is the multi-GPU shape of `jepsen.independent/checker` (workloads/set_full.clj:155): linearizability is
 local (Herlihy–Wing), so per-key verdicts compose with no cross-shard state; ranks never exchange
 configurations.  The only exchange is `all_reduce(MAX)` over int32 verdict codes (true 0 < :unknown 1 <
 false 2 == checker/merge-valid) and witness indices — bytes over NVLink/NVSwitch through NCCL

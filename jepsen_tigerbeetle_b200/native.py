@@ -19,7 +19,7 @@ CSRC = os.path.join(_HERE, "csrc")
 _SOURCES = ["jtb_abi.cu", "jtb_prep.cpp", "jtb_multi.cpp"]
 _DEPS = _SOURCES + ["jtb_prep.h", "jtb_expand.h", "jtb_wgl.cuh", "jtb_search.cuh", "jtb_scout.cuh", "jtb_scans.cuh",
                     "jtb_table_bench.cuh", "jtb_level.cuh", "jtb_partition.cuh"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared", "-ldl"]
 
 EXPORTS = ["jtb_abi_version", "jtb_device_count", "jtb_create", "jtb_destroy", "jtb_last_error",
@@ -37,7 +37,7 @@ class NativeError(RuntimeError):
 
 
 def build(force: bool = False) -> str:
-    """Compile the CUDA library in-tree for sm_100a (nvcc cross-compiles without a GPU)."""
+    """Compile the CUDA library in-tree for sm_90a (nvcc cross-compiles without a GPU)."""
     deps = [os.path.join(CSRC, f) for f in _DEPS]
     deps.append(os.path.join(_HERE, "..", "include", "jtb_check.h"))
     stale = (not os.path.exists(LIB_PATH)

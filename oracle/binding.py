@@ -4,6 +4,7 @@ from __future__ import annotations
 import ctypes as C
 import os
 import subprocess
+import tempfile
 
 from jepsen_tigerbeetle_b200 import abi
 from jepsen_tigerbeetle_b200.history import CModel, FlatHistory, as_c_history
@@ -32,6 +33,8 @@ def _cpu_stamp() -> str:
 
 
 def build(force: bool = False) -> str:
+    """The library in oracle/, (re)built when stale or built on another CPU; when oracle/ is read-only, a rebuild goes
+    to a fresh temporary directory instead."""
     so = os.path.join(_HERE, "libjtb_oracle.so")
     stamp_file = os.path.join(_HERE, ".build_cpu")
     srcs = [os.path.join(_HERE, f) for f in ("lin_oracle.cpp", "scan_oracle.cpp", "oracle_common.h", "Makefile")]
@@ -43,6 +46,10 @@ def build(force: bool = False) -> str:
     except OSError:
         other_cpu = True
     if force or stale or other_cpu:
+        if not os.access(_HERE, os.W_OK):
+            so = os.path.join(tempfile.mkdtemp(prefix="jtb_oracle_"), "libjtb_oracle.so")
+            subprocess.check_call(["make", "-C", _HERE, "-B", "-s", f"LIB={so}"], stdout=subprocess.DEVNULL)
+            return so
         subprocess.check_call(["make", "-C", _HERE, "-B", "-s"], stdout=subprocess.DEVNULL)
         with open(stamp_file, "w") as f:
             f.write(stamp)

@@ -3,7 +3,7 @@
 //       jepsen_tigerbeetle_b200/csrc/jtb_prep.cpp ;  python scripts/experiments/beam_emulation.py
 // policy 0 = (rank desc, crashed asc) exact top-W, 1 = (crashed asc, rank desc) exact top-W, 2 = the device's binned keys
 // relative to the previous level's best + pseudo-random share of the boundary bin.  BEAM_LAZY=1 (bank): crashed
-// transfers only when they move the balances towards a pending read.  Results: profiles/r2_beam.md.
+// transfers only when they move the balances towards a pending read.
 // experiment: level-synchronous BEAM (keep the W best configurations of every level: furthest rank first, then fewest
 // crashed ops consumed; no backlog) — does it find the linearization of crash-heavy VALID histories, at which W?
 #include <algorithm>

@@ -1,4 +1,4 @@
-"""CPU tier: the C-ABI library builds for sm_100a, loads without a GPU and exports every symbol that
+"""CPU tier: the C-ABI library builds for sm_90a, loads without a GPU and exports every symbol that
 include/jtb_check.h declares; the ctypes struct images match the header's layout."""
 import ctypes
 import os
