@@ -8,10 +8,10 @@
 #include <mutex>
 #include <string>
 #include <thread>
+#include <type_traits>
 #include <vector>
 
 #include "jtb_wgl.cuh"
-#include "jtb_search.cuh"
 #include "jtb_level.cuh"
 #include "jtb_scout.cuh"
 #include "jtb_scans.cuh"
@@ -41,7 +41,6 @@ struct jtb_ctx {
     DevBuf lv_ctrl, lv_buf[2];          // level engine: control block, the two level arrays
     DevBuf lv_aux[2], lv_beam;          // beam mode: per-entry priority words, histogram + trackers
     size_t table_dirty = ~(size_t)0;    // bytes at the start of `table` that may hold old slots (level engine clears only these)
-    bool in_probe = false;              // inside the budgeted work-list probe that precedes a beam
     int last_engine = 0;                // 0 work-list (visited table complete), 1 level (visited set is ephemeral)
     unsigned long long stats[24] = {0};
     unsigned long long last_configs = 0;  // configs of the previous search (sizes the next table)
@@ -89,60 +88,35 @@ int upload(jtb_ctx* ctx, DevBuf& b, const std::vector<T>& v) {
     return 0;
 }
 
-template <int MODEL, int KW, int MINB, bool EAGER>
-int launch_wgl_b(jtb_ctx* ctx, const WglParams& p, int neg_ok, int grid, size_t smem) {
-    auto k = wgl_search_kernel<MODEL, KW, MINB, EAGER>;
+// The one list of the (model, key width) combinations the search kernels are built for: bank and cas-register at 2, 4
+// and 8 key words, set at 2 (register histories run the cas-register kernels).  Calls
+// f(std::integral_constant<int, MODEL>, std::integral_constant<int, KW>).
+template <typename F>
+int dispatch_model_kw(jtb_ctx* ctx, int kind, int kw, F&& f) {
+    using std::integral_constant;
+    if (kind == JTB_MODEL_SET) return f(integral_constant<int, JTB_MODEL_SET>(), integral_constant<int, 2>());
+    auto by_kw = [&](auto model) -> int {
+        switch (kw) {
+        case 2: return f(model, integral_constant<int, 2>());
+        case 4: return f(model, integral_constant<int, 4>());
+        case 8: return f(model, integral_constant<int, 8>());
+        }
+        ctx->err = "unsupported key width";
+        return -1;
+    };
+    return kind == JTB_MODEL_BANK ? by_kw(integral_constant<int, JTB_MODEL_BANK>())
+                                  : by_kw(integral_constant<int, JTB_MODEL_CAS_REGISTER>());
+}
+
+// two builds of the work-list kernel: Knossos-exact space (no eager-read code, 64 regs, JTB_CTAS_EXACT CTAs/SM) and the
+// eager-read default (up to 80 regs, JTB_CTAS_EAGER CTAs/SM)
+template <int MODEL, int KW>
+int launch_wgl(jtb_ctx* ctx, const WglParams& p, int neg_ok, int grid, size_t smem) {
+    auto k = p.eager_reads ? wgl_search_kernel<MODEL, KW, JTB_CTAS_EAGER, true> : wgl_search_kernel<MODEL, KW, JTB_CTAS_EXACT, false>;
     CK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     k<<<grid, WGL_THREADS, smem, ctx->stream>>>(p, neg_ok);
     CK(cudaGetLastError());
     return 0;
-}
-
-// two builds of the kernel: Knossos-exact space (no eager-read code, 64 regs, JTB_CTAS_EXACT CTAs/SM) and the
-// eager-read default (up to 80 regs, JTB_CTAS_EAGER CTAs/SM)
-template <int MODEL, int KW>
-int launch_wgl(jtb_ctx* ctx, const WglParams& p, int neg_ok, int grid, size_t smem, int ctas_per_sm) {
-    (void)ctas_per_sm;
-    return p.eager_reads ? launch_wgl_b<MODEL, KW, JTB_CTAS_EAGER, true>(ctx, p, neg_ok, grid, smem)
-                         : launch_wgl_b<MODEL, KW, JTB_CTAS_EXACT, false>(ctx, p, neg_ok, grid, smem);
-}
-
-// the thread-per-configuration kernel (jtb_search.cuh)
-template <int MODEL, int KW>
-int launch_tpc(jtb_ctx* ctx, const WglParams& p, int neg_ok, int grid, size_t smem) {
-    if (p.eager_reads) {
-        auto k = wgl_tpc_kernel<MODEL, KW, true>;
-        CK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        k<<<grid, TPC_THREADS, smem, ctx->stream>>>(p, neg_ok);
-    } else {
-        auto k = wgl_tpc_kernel<MODEL, KW, false>;
-        CK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        k<<<grid, TPC_THREADS, smem, ctx->stream>>>(p, neg_ok);
-    }
-    CK(cudaGetLastError());
-    return 0;
-}
-
-template <int MODEL>
-int launch_tpc_kw(jtb_ctx* ctx, int kw, const WglParams& p, int neg_ok, int grid, size_t smem) {
-    switch (kw) {
-    case 2: return launch_tpc<MODEL, 2>(ctx, p, neg_ok, grid, smem);
-    case 4: return launch_tpc<MODEL, 4>(ctx, p, neg_ok, grid, smem);
-    case 8: return launch_tpc<MODEL, 8>(ctx, p, neg_ok, grid, smem);
-    }
-    ctx->err = "unsupported key width";
-    return -1;
-}
-
-template <int MODEL>
-int launch_wgl_kw(jtb_ctx* ctx, int kw, const WglParams& p, int neg_ok, int grid, size_t smem, int ctas_per_sm) {
-    switch (kw) {
-    case 2: return launch_wgl<MODEL, 2>(ctx, p, neg_ok, grid, smem, ctas_per_sm);
-    case 4: return launch_wgl<MODEL, 4>(ctx, p, neg_ok, grid, smem, ctas_per_sm);
-    case 8: return launch_wgl<MODEL, 8>(ctx, p, neg_ok, grid, smem, ctas_per_sm);
-    }
-    ctx->err = "unsupported key width";
-    return -1;
 }
 
 // the level engine (jtb_level.cuh): cooperative launch, every CTA resident (the levels are separated by grid barriers)
@@ -163,7 +137,6 @@ int launch_level(jtb_ctx* ctx, const LvParams& p, int neg_ok, bool eager, int* g
     CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k, LV_THREADS, smem));
     if (per_sm < 1) { ctx->err = "level engine: the kernel does not fit on an SM"; return -1; }
     per_sm = std::min(per_sm, JTB_LV_CTAS);
-    if (getenv("JTB_LV_CTAS_PER_SM")) per_sm = std::max(1, std::min(per_sm, atoi(getenv("JTB_LV_CTAS_PER_SM"))));
     const int grid = ctx->opts.search_ctas ? std::min<int>((int)ctx->opts.search_ctas, ctx->n_sms * per_sm) : ctx->n_sms * per_sm;
     if (grid > 1024) { ctx->err = "level engine: more CTAs than barrier release words"; return -1; }
     *grid_out = grid;
@@ -171,17 +144,6 @@ int launch_level(jtb_ctx* ctx, const LvParams& p, int neg_ok, bool eager, int* g
     void* args[] = {&pp};
     CK(cudaLaunchCooperativeKernel(k, dim3(grid), dim3(LV_THREADS), args, smem, ctx->stream));
     return 0;
-}
-
-template <int MODEL>
-int launch_level_kw(jtb_ctx* ctx, int kw, const LvParams& p, int neg_ok, bool eager, int* grid_out) {
-    switch (kw) {
-    case 2: return launch_level<MODEL, 2>(ctx, p, neg_ok, eager, grid_out);
-    case 4: return launch_level<MODEL, 4>(ctx, p, neg_ok, eager, grid_out);
-    case 8: return launch_level<MODEL, 8>(ctx, p, neg_ok, eager, grid_out);
-    }
-    ctx->err = "unsupported key width";
-    return -1;
 }
 
 // ---- level engine, host side: buffers, (re)launch, growth ------------------------------------------------------
@@ -285,11 +247,9 @@ int search_level(jtb_ctx* ctx, const jtb_model* m, const Prepared& P, int n_shar
             const double left = ctx->opts.time_budget_ms * 1e-3 - (now_s() - t_begin);
             p.time_budget_ns = (unsigned long long)(std::max(left, 1e-3) * 1e9);
         }
-        int rc;
-        if (bank) rc = launch_level_kw<JTB_MODEL_BANK>(ctx, KW, p, m->negative_balances_ok, eager, &grid);
-        else if (m->kind == JTB_MODEL_SET) rc = launch_level<JTB_MODEL_SET, 2>(ctx, p, 0, eager, &grid);
-        else rc = launch_level_kw<JTB_MODEL_CAS_REGISTER>(ctx, KW, p, 0, eager, &grid);
-        if (rc) return rc;
+        const int neg_ok = bank ? m->negative_balances_ok : 0;
+        if (int rc = dispatch_model_kw(ctx, m->kind, KW, [&](auto M, auto K) { return launch_level<M(), K()>(ctx, p, neg_ok, eager, &grid); }))
+            return rc;
         CK(cudaMemcpyAsync(&lc, ctx->lv_ctrl.p, sizeof lc, cudaMemcpyDeviceToHost, ctx->stream));
         CK(cudaStreamSynchronize(ctx->stream));
         if (lc.abort) { ctx->err = "level engine: a grid barrier timed out (internal error)"; return -1; }
@@ -422,22 +382,10 @@ int preload(jtb_ctx* ctx, K kernel) {
 template <int MODEL, int KW>
 int preload_search(jtb_ctx* ctx, bool eager) {
     constexpr int EW = KW + (MODEL == JTB_MODEL_BANK ? 4 : 0);
-    int rc = eager ? (preload(ctx, wgl_search_kernel<MODEL, KW, JTB_CTAS_EAGER, true>) | preload(ctx, wgl_tpc_kernel<MODEL, KW, true>) |
-                      preload(ctx, wgl_scout_kernel<MODEL, KW, true>))
-                   : (preload(ctx, wgl_search_kernel<MODEL, KW, JTB_CTAS_EXACT, false>) | preload(ctx, wgl_tpc_kernel<MODEL, KW, false>) |
-                      preload(ctx, wgl_scout_kernel<MODEL, KW, false>));
+    int rc = eager ? (preload(ctx, wgl_search_kernel<MODEL, KW, JTB_CTAS_EAGER, true>) | preload(ctx, wgl_scout_kernel<MODEL, KW, true>))
+                   : (preload(ctx, wgl_search_kernel<MODEL, KW, JTB_CTAS_EXACT, false>) | preload(ctx, wgl_scout_kernel<MODEL, KW, false>));
     rc |= preload(ctx, table_rehash_kernel<KW>) | preload(ctx, ring_compact_kernel<EW>) | preload(ctx, wgl_resume_ctrl_kernel);
     return rc ? -1 : 0;
-}
-
-template <int MODEL>
-int preload_search_kw(jtb_ctx* ctx, int kw, bool eager) {
-    switch (kw) {
-    case 2: return preload_search<MODEL, 2>(ctx, eager);
-    case 4: return preload_search<MODEL, 4>(ctx, eager);
-    case 8: return preload_search<MODEL, 8>(ctx, eager);
-    }
-    return -1;
 }
 
 template <int MODEL, int KW>
@@ -448,15 +396,311 @@ int launch_scout(jtb_ctx* ctx, const WglParams& p, const ScoutParams& sp, int ne
     return 0;
 }
 
-template <int MODEL>
-int launch_scout_kw(jtb_ctx* ctx, int kw, const WglParams& p, const ScoutParams& sp, int neg_ok, int n_scouts) {
-    switch (kw) {
-    case 2: return launch_scout<MODEL, 2>(ctx, p, sp, neg_ok, n_scouts);
-    case 4: return launch_scout<MODEL, 4>(ctx, p, sp, neg_ok, n_scouts);
-    case 8: return launch_scout<MODEL, 8>(ctx, p, sp, neg_ok, n_scouts);
+// What one search leaves for the verdicts.
+struct Search {
+    Ctrl hc;                            // stop / cause / overflow
+    std::vector<int> found, max_rank;   // per shard: found VALID, furthest frontier rank reached
+    double kernel_s = 0;
+    uint64_t configs = 0, probes = 0;
+    uint64_t n_slots = 0;               // work list: slots of the visited table (jtb_final_configs reads it)
+    explicit Search(int n_shards) : found(n_shards, 0), max_rank(n_shards, 0) { std::memset(&hc, 0, sizeof hc); }
+};
+
+// Per-shard results on the device before a search: nothing found, furthest rank = the shard's first rank.
+int arm_shards(jtb_ctx* ctx, const Prepared& P, int n_shards, std::vector<int>& max_rank) {
+    CK(cudaMemsetAsync(ctx->found.p, 0, n_shards * sizeof(int), ctx->stream));
+    for (int s = 0; s < n_shards; ++s) max_rank[s] = (int)P.rank_base[s];
+    CK(cudaMemcpyAsync(ctx->maxrank.p, max_rank.data(), n_shards * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
+    return 0;
+}
+
+// ---- work-list engine, host side: ring and visited table, scouts, pause / grow / resume ------------------------
+// The persistent kernel pauses when its ring or its table is nearly full; the host then compacts the live ring entries
+// into a 4x larger ring and/or re-hashes the table into a 4x larger one and relaunches, so no work is lost.
+// max_configs: stop (UNKNOWN) after this many configurations, 0 = no budget; scouts: run the depth-first scouts beside
+// the search on histories with crashed ops.  t_start: start of the call (the scouts' grace period ends with its time budget).
+int search_worklist(jtb_ctx* ctx, const jtb_history* h, const jtb_model* m, const Prepared& P,
+                    const std::vector<int>& searchable, const std::vector<uint64_t>& init_entries, uint64_t max_configs,
+                    bool scouts_on, double t_start, Search& r) {
+    const int n_shards = h->n_shards;
+    const int KW = P.key_words;
+    const int EW = KW + (m->kind == JTB_MODEL_BANK ? 4 : 0);
+    const int neg_ok = m->kind == JTB_MODEL_BANK ? m->negative_balances_ok : 0;
+    const bool eager_mode = !(ctx->opts.flags & JTB_OPT_NO_EAGER_READS);
+    Ctrl& hc = r.hc;
+    ctx->last_engine = 0;
+    ctx->table_dirty = ~(size_t)0;   // the work-list engine fills the table
+    // CTA deque / grid: one WARP per configuration (jtb_wgl.cuh), every child of a configuration probed in the same
+    // round trip
+    const int cand_rounds = P.S_pad / 32, cls_rounds = (P.max_nc + 31) / 32;
+    // worst case of children one CTA step can push (overflow -> ring)
+    const uint32_t worst_push = (WGL_BATCH + WGL_WARPS) * 32 * (cand_rounds + cls_rounds);
+    uint32_t deque_cap = 1024;                       // fixed: a full deque overflows to the ring
+    while ((size_t)deque_cap * EW * 8 > 48 * 1024) deque_cap >>= 1;
+    const uint32_t stage_cap = std::max(deque_cap, worst_push);
+    const size_t smem = (size_t)(deque_cap + WGL_BATCH) * EW * 8;
+    // eager-read searches are small and latency-bound: 3 CTAs/SM (no register spills) wins; the Knossos-exact space is
+    // throughput-bound: 4 CTAs/SM (measured A/B, DESIGN.md)
+    const int want_ctas = eager_mode ? JTB_CTAS_EAGER : JTB_CTAS_EXACT;
+    const int ctas_per_sm = std::max(1, (int)std::min<size_t>(want_ctas, (220 * 1024) / (smem + 1024)));
+    const int grid = ctx->opts.search_ctas ? (int)ctx->opts.search_ctas : ctx->n_sms * ctas_per_sm;
+    const uint64_t per_step_push = (uint64_t)grid * stage_cap;  // worst case children of one step of every CTA
+    // work ring
+    uint64_t ring_entries = 1ull << 22;
+    while (ring_entries < 4 * per_step_push + 2 * searchable.size()) ring_entries <<= 1;
+    // test hook: start with a ring that is too small so that the RING_FULL pause/grow/resume path runs
+    const bool tiny_ring = getenv("JTB_TEST_TINY_RING") != nullptr;
+    if (ensure(ctx, ctx->pool, ring_entries * EW * 8)) return -1;
+    CK(cudaMemsetAsync(ctx->pool.p, 0, ring_entries * EW * 8, ctx->stream));
+    CK(cudaMemcpyAsync(ctx->pool.p, init_entries.data(), init_entries.size() * 8, cudaMemcpyHostToDevice, ctx->stream));
+    // visited table: start at 1 GiB (or the caller's size), grow x4 on load > 0.7 without losing work
+    size_t free_b = 0, total_b = 0;
+    CK(cudaMemGetInfo(&free_b, &total_b));
+    const size_t reserve = (size_t)4 << 30;
+    size_t max_table = ctx->opts.table_bytes ? ctx->opts.table_bytes : (size_t)64 << 30;
+    max_table = std::min(max_table, ctx->table.cap + (free_b > reserve ? free_b - reserve : 0));
+    // start at 1 GiB, or at 4x what the previous call on this context ended up needing (warm context)
+    const size_t min_start = getenv("JTB_TABLE_START_MB") ? (size_t)atoll(getenv("JTB_TABLE_START_MB")) << 20 : (size_t)1 << 30;
+    size_t start_bytes = std::max<size_t>(min_start, (size_t)ctx->last_configs * 4 * KW * 8);
+    size_t table_bytes = std::min<size_t>(max_table, ctx->opts.table_bytes ? ctx->opts.table_bytes : start_bytes);
+    uint64_t n_slots = 1;
+    while (n_slots * 2 * KW * 8 <= table_bytes) n_slots <<= 1;
+    if (ensure(ctx, ctx->table, n_slots * KW * 8)) return -1;
+    CK(cudaMemsetAsync(ctx->table.p, 0, n_slots * KW * 8, ctx->stream));
+    hc.tail = searchable.size();
+    hc.created = searchable.size();
+    hc.n_undecided = (int)searchable.size();
+    CK(cudaMemcpyAsync(ctx->ctrl.p, &hc, sizeof hc, cudaMemcpyHostToDevice, ctx->stream));
+    if (arm_shards(ctx, P, n_shards, r.max_rank)) return -1;
+    DevBuf ring2, table2;  // growth targets (freed below)
+    // cudaFree synchronizes the whole device, i.e. it would wait for the scouts: while they run, frees are deferred
+    // (cudaFree is valid for stream-ordered allocations too)
+    ScoutGuard scouts(ctx);
+    std::vector<void*> deferred;
+    auto free_tmp = [&]() {
+        scouts.stop();
+        for (void* q : deferred) cudaFree(q);
+        deferred.clear();
+        if (ring2.p) cudaFree(ring2.p);
+        if (table2.p) cudaFree(table2.p);
+        ring2 = DevBuf(); table2 = DevBuf();
+    };
+    auto grow_buf = [&](DevBuf& b, size_t bytes) -> int {
+        if (bytes <= b.cap) return 0;
+        if (b.p) { if (scouts.active) deferred.push_back(b.p); else cudaFree(b.p); }
+        b = DevBuf();
+        // cudaMalloc also synchronizes with running kernels (the search would sit behind the scouts for seconds at
+        // its first table growth); the stream-ordered allocator does not
+        const cudaError_t e = scouts.active ? cudaMallocAsync(&b.p, bytes, ctx->stream) : cudaMalloc(&b.p, bytes);
+        if (e != cudaSuccess) {
+            (void)cudaGetLastError();
+            b.p = nullptr;
+            if (scouts.stop()) return -1;   // out of memory with frees pending: give the scouts up
+            for (void* q : deferred) cudaFree(q);
+            deferred.clear();
+            CK(cudaMalloc(&b.p, bytes));
+        }
+        b.cap = bytes;
+        return 0;
+    };
+    int attempts = 0;
+    CK(cudaEventRecord(ctx->ev0, ctx->stream));
+    WglParams pb{};   // what the search kernel and the scouts share
+    pb.rows = (const int32_t*)ctx->rows.p;
+    pb.classes = (const ClassRec*)ctx->classes.p;
+    pb.cls_inv_pos = (const int32_t*)ctx->cls_inv.p;
+    pb.ctrl = (Ctrl*)ctx->ctrl.p;
+    pb.shard_found = (int*)ctx->found.p;
+    pb.shard_max_rank = (int*)ctx->maxrank.p;
+    pb.row_words = P.row_words;
+    pb.S_pad = P.S_pad;
+    pb.n_shards = n_shards;
+    pb.max_nc = P.max_nc;
+    pb.eager_reads = eager_mode ? 1 : 0;
+    // ---- depth-first scouts (jtb_scout.cuh): only where the crowd is known to drown — histories with
+    //      crashed ops — and launched FIRST so that they are resident before the persistent CTAs fill the SMs
+    int64_t max_shard_events = 0;
+    for (int s : searchable) max_shard_events = std::max<int64_t>(max_shard_events, h->shard_off[s + 1] - h->shard_off[s]);
+    int n_scouts = 0;
+    const bool scout_only = getenv("JTB_SCOUT_ONLY") != nullptr;   // test hook: no search kernel at all
+    if (scouts_on && (P.max_nc > 0 || scout_only) && max_shard_events < (1ll << 29)) {
+        n_scouts = getenv("JTB_SCOUTS") ? std::max(1, atoi(getenv("JTB_SCOUTS"))) : SCOUT_ORDERS;
+        ScoutParams sp{};
+        sp.n_init = (int)searchable.size();
+        sp.n_orders = getenv("JTB_SCOUT_ORDERS") ? std::min(SCOUT_ORDERS, std::max(1, atoi(getenv("JTB_SCOUT_ORDERS")))) : SCOUT_ORDERS;
+        const uint64_t sc_slots = 1ull << 22;                       // 2 M configs per scout
+        sp.slot_mask = sc_slots - 1;
+        sp.stack_cap = (uint32_t)(max_shard_events + 2);            // a path linearizes each op at most once
+        sp.pair_budget = 8ull << 20;
+        if (upload(ctx, ctx->sc_init, init_entries) ||
+            ensure(ctx, ctx->sc_tables, (size_t)n_scouts * sc_slots * KW * 8) ||
+            ensure(ctx, ctx->sc_stacks, (size_t)n_scouts * sp.stack_cap * (EW + 1) * 8) ||
+            ensure(ctx, ctx->sc_ctl, SCOUT_CTL_WORDS * 8))
+            return -1;
+        CK(cudaMemsetAsync(ctx->sc_tables.p, 0, (size_t)n_scouts * sc_slots * KW * 8, ctx->stream));
+        CK(cudaMemsetAsync(ctx->sc_ctl.p, 0, SCOUT_CTL_WORDS * 8, ctx->stream));
+        sp.init = (const uint64_t*)ctx->sc_init.p;
+        sp.tables = (uint64_t*)ctx->sc_tables.p;
+        sp.stacks = (uint64_t*)ctx->sc_stacks.p;
+        sp.ctl = (unsigned long long*)ctx->sc_ctl.p;
+        CK(cudaEventRecord(ctx->ev_setup, ctx->stream));
+        CK(cudaStreamWaitEvent(ctx->scout_stream, ctx->ev_setup, 0));
+        if (int rc = dispatch_model_kw(ctx, m->kind, KW, [&](auto M, auto K) {
+                return preload_search<M(), K()>(ctx, eager_mode) ? -1 : launch_scout<M(), K()>(ctx, pb, sp, neg_ok, n_scouts);
+            }))
+            return rc;
+        scouts.active = true;
     }
-    ctx->err = "unsupported key width";
-    return -1;
+    for (;;) {
+        ++attempts;
+        if (scout_only) { hc.stop = 2; hc.cause = JTB_CAUSE_BUDGET; break; }
+        WglParams p = pb;
+        p.table = (uint64_t*)ctx->table.p;
+        p.slot_mask = n_slots - 1;
+        p.ring = (uint64_t*)ctx->pool.p;
+        p.ring_mask = ring_entries - 1;
+        p.ring_guard = (tiny_ring && attempts == 1) ? 20000 : ring_entries - 3 * per_step_push;
+        const uint64_t load_guard = (uint64_t)(0.50 * (double)n_slots);  // linear probing: keep chains short
+        p.max_configs = load_guard;
+        p.budget_cause = JTB_CAUSE_TABLE_FULL;
+        if (max_configs && max_configs <= load_guard) {
+            p.max_configs = max_configs;
+            p.budget_cause = JTB_CAUSE_BUDGET;
+        }
+        p.time_budget_ns = (unsigned long long)ctx->opts.time_budget_ms * 1000000ull;
+        p.deque_cap = deque_cap;
+        if (int rc = dispatch_model_kw(ctx, m->kind, KW, [&](auto M, auto K) { return launch_wgl<M(), K()>(ctx, p, neg_ok, grid, smem); })) {
+            free_tmp();
+            return rc;
+        }
+        CK(cudaMemcpyAsync(&hc, ctx->ctrl.p, sizeof hc, cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));
+        const bool grow_table = hc.stop == 2 && hc.cause == JTB_CAUSE_TABLE_FULL && n_slots * KW * 8 * 4 <= max_table;
+        const bool grow_ring = hc.stop == 2 && hc.cause == CAUSE_RING_FULL && ring_entries * EW * 8 * 4 <= ((size_t)16 << 30);
+        if (!grow_table && !grow_ring) break;
+        if (hc.n_undecided <= 0) break;   // the scouts decided every shard while the search was pausing
+        // ---- pause/resume: the live work is exactly the non-zero ring slots ---------------------
+        const uint64_t new_ring_entries = grow_ring ? ring_entries * 4 : ring_entries;
+        if (grow_buf(ring2, new_ring_entries * EW * 8)) {   // no memory for the larger ring: give up like a full table
+            (void)cudaGetLastError();
+            hc.stop = 2; hc.cause = JTB_CAUSE_TABLE_FULL;
+            break;
+        }
+        CK(cudaMemsetAsync(ring2.p, 0, new_ring_entries * EW * 8, ctx->stream));
+        Ctrl* dc = (Ctrl*)ctx->ctrl.p;
+        CK(cudaMemsetAsync(&dc->tail, 0, sizeof(unsigned long long), ctx->stream));
+        dispatch_model_kw(ctx, m->kind, KW, [&](auto M, auto K) {
+            ring_compact_kernel<EntryLayout<M(), K()>::EW><<<ctx->n_sms * 8, 256, 0, ctx->stream>>>(
+                (const uint64_t*)ctx->pool.p, ring_entries - 1, 0, ring_entries, (uint64_t*)ring2.p, new_ring_entries - 1, &dc->tail);
+            return 0;
+        });
+        CK(cudaGetLastError());
+        std::swap(ctx->pool, ring2);
+        ring_entries = new_ring_entries;
+        CK(cudaMemsetAsync(&dc->head, 0, sizeof(unsigned long long), ctx->stream));
+        wgl_resume_ctrl_kernel<<<1, 1, 0, ctx->stream>>>(dc);   // stop, cause := 0 (unless everything is decided)
+        CK(cudaGetLastError());
+        if (grow_table) {
+            const uint64_t new_slots = n_slots * 4;
+            if (grow_buf(table2, new_slots * KW * 8)) {   // old + 4x table do not fit together: UNKNOWN, not an error
+                (void)cudaGetLastError();
+                hc.stop = 2; hc.cause = JTB_CAUSE_TABLE_FULL;
+                break;
+            }
+            CK(cudaMemsetAsync(table2.p, 0, new_slots * KW * 8, ctx->stream));
+            dispatch_model_kw(ctx, m->kind, KW, [&](auto, auto K) {
+                table_rehash_kernel<K()><<<ctx->n_sms * 8, 256, 0, ctx->stream>>>((const uint64_t*)ctx->table.p, n_slots,
+                                                                                  (uint64_t*)table2.p, new_slots - 1, &dc->overflow);
+                return 0;
+            });
+            CK(cudaGetLastError());
+            CK(cudaStreamSynchronize(ctx->stream));
+            std::swap(ctx->table, table2);
+            if (table2.p) {   // release the old table right away (deferred while the scouts run)
+                if (scouts.active) deferred.push_back(table2.p); else cudaFree(table2.p);
+                table2 = DevBuf();
+            }
+            n_slots = new_slots;
+        }
+    }
+    unsigned long long sc_ctl[SCOUT_CTL_WORDS] = {0};
+    if (n_scouts) {
+        // the search gave up (UNKNOWN) while scouts are still walking: give them a grace period
+        if (hc.stop == 2 && hc.n_undecided > 0) {
+            double grace_s = getenv("JTB_SCOUT_GRACE_MS") ? atof(getenv("JTB_SCOUT_GRACE_MS")) * 1e-3 : 20.0;
+            if (ctx->opts.time_budget_ms)
+                grace_s = std::max(0.0, ctx->opts.time_budget_ms * 1e-3 - (now_s() - t_start));
+            const double deadline = now_s() + grace_s;
+            while (now_s() < deadline && cudaStreamQuery(ctx->scout_stream) == cudaErrorNotReady)
+                std::this_thread::sleep_for(std::chrono::microseconds(200));
+        }
+        (void)cudaGetLastError();
+        if (scouts.stop()) { free_tmp(); return -1; }
+        CK(cudaMemcpyAsync(sc_ctl, ctx->sc_ctl.p, sizeof sc_ctl, cudaMemcpyDeviceToHost, ctx->stream));
+    }
+    CK(cudaEventRecord(ctx->ev1, ctx->stream));
+    CK(cudaMemcpyAsync(r.found.data(), ctx->found.p, n_shards * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaMemcpyAsync(r.max_rank.data(), ctx->maxrank.p, n_shards * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    free_tmp();
+    float ms = 0;
+    CK(cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1));
+    r.kernel_s = ms * 1e-3;
+    r.configs = hc.configs;
+    r.probes = hc.probes;
+    r.n_slots = n_slots;
+    ctx->last_configs = hc.configs;
+    unsigned long long* st = ctx->stats;
+    st[0] = hc.configs; st[1] = hc.probes; st[2] = hc.expansions; st[3] = hc.tail;
+    st[4] = hc.head; st[5] = hc.polls; st[6] = hc.max_probe_len; st[7] = n_slots;
+    st[8] = (unsigned long long)grid; st[9] = ring_entries; st[10] = (unsigned long long)attempts;
+    st[11] = (unsigned long long)(ms * 1e3);
+    st[12] += init_entries.size() * 8 + sizeof(Ctrl) + (size_t)n_shards * 4;
+    st[13] = (unsigned long long)attempts * sizeof(Ctrl) + (size_t)n_shards * 8;  // device -> host bytes
+    st[14] = (unsigned long long)((scout_only ? 0 : attempts) + 3 * (attempts - 1) + (n_scouts ? 1 : 0));  // search + compact/rehash/re-arm + scouts
+    st[15] = sc_ctl[2]; st[16] = sc_ctl[3]; st[17] = sc_ctl[4]; st[18] = (unsigned long long)n_scouts;
+    st[19] = 0;   // engine: work list
+    return 0;
+}
+
+// Verdicts of the shards a search ran on, and the record jtb_final_configs reads.  fc_valid = false: the visited
+// table is not complete (scout-only test runs).
+void set_verdicts(jtb_ctx* ctx, const jtb_history* h, const Prepared& P, const std::vector<int>& searchable, Search& r,
+                  bool fc_valid, jtb_lin_shard* shards) {
+    const int n_shards = h->n_shards;
+    Ctrl& hc = r.hc;
+    if (hc.stop == 2 && hc.cause == CAUSE_RING_FULL) hc.cause = JTB_CAUSE_BUDGET;
+    if (hc.overflow) {   // a ring slot was overwritten before it was consumed: no verdict may be derived from this search
+        hc.stop = 2;
+        hc.cause = JTB_CAUSE_BUDGET;
+        std::fill(r.found.begin(), r.found.end(), 0);
+    }
+    for (int s : searchable) {
+        jtb_lin_shard& sh = shards[s];
+        if (r.found[s]) {
+            sh.valid = JTB_VALID;
+        } else if (hc.stop == 2) {
+            sh.valid = JTB_UNKNOWN;
+            sh.cause = hc.cause;
+        } else {
+            sh.valid = JTB_INVALID;
+            const int64_t g = r.max_rank[s];
+            sh.witness_index = P.ret_index[g];
+            if (g > P.rank_base[s]) sh.previous_ok_index = P.ret_index[g - 1];
+        }
+    }
+    if (n_shards == 1) {
+        shards[0].configs_explored = r.configs;
+        shards[0].probes = r.probes;
+    }
+    ctx->fc.valid = fc_valid;
+    ctx->fc.n_events = h->n_events;
+    ctx->fc.n_shards = n_shards;
+    ctx->fc.kw = P.key_words;
+    ctx->fc.n_slots = r.n_slots;
+    ctx->fc.max_rank = r.max_rank;
+    ctx->fc.verdict.assign(n_shards, JTB_UNKNOWN);
+    for (int s = 0; s < n_shards; ++s) ctx->fc.verdict[s] = shards[s].valid;
 }
 
 }  // namespace
@@ -531,9 +775,10 @@ void jtb_destroy(jtb_ctx* ctx) {
 const char* jtb_last_error(const jtb_ctx* ctx) { return ctx ? ctx->err.c_str() : "no context (no CUDA device?)"; }
 
 // -------------------------------------------------------------------------------------------------
-// force_engine: 0 = by options / history, 1 = level, 2 = work list
+// force_worklist: search with the work-list engine whatever the options and the history say (its table then holds
+// every visited configuration, which jtb_final_configs reads)
 static int check_lin_impl(jtb_ctx* ctx, const jtb_history* h, const jtb_model* m, jtb_lin_shard* shards,
-                          jtb_lin_result* out, int force_engine) {
+                          jtb_lin_result* out, bool force_worklist) {
     const double t_start = now_s();
     ctx->fc.valid = false;
     CK(cudaSetDevice(ctx->device));
@@ -577,96 +822,89 @@ static int check_lin_impl(jtb_ctx* ctx, const jtb_history* h, const jtb_model* m
     };
     for (int s = 0; s < n_shards; ++s)
         if (!P.shard_cause[s] && P.rank_base[s + 1] != P.rank_base[s]) add_init(s);
-    double kernel_s = 0;
-    uint64_t configs = 0, probes = 0;
     ctx->stats[10] = 0;
     ctx->stats[12] = ctx->stats[13] = ctx->stats[14] = 0;
     ctx->stats[15] = ctx->stats[16] = ctx->stats[17] = ctx->stats[18] = 0;
-    Ctrl hc;
-    std::memset(&hc, 0, sizeof hc);
-    std::vector<int> h_found(n_shards, 0), h_max(n_shards, 0);
-    uint64_t fc_n_slots = 0;
-    bool scout_only_run = false;
-    if (!searchable.empty()) {
-        if (upload(ctx, ctx->rows, P.rows) || upload(ctx, ctx->classes, P.classes) || upload(ctx, ctx->cls_inv, P.cls_inv_pos))
-            return -1;
-        if (ensure(ctx, ctx->ctrl, sizeof(Ctrl)) || ensure(ctx, ctx->found, n_shards * sizeof(int)) ||
-            ensure(ctx, ctx->maxrank, n_shards * sizeof(int)))
-            return -1;
-        const bool eager_mode = !(ctx->opts.flags & JTB_OPT_NO_EAGER_READS);
-        // ---- beam first (single-key histories with crashed ops; measured on the 8-key C5 "monster": one beam shared by
-        //      several keys starves most of them — 2 of 8 decided after 7.7e8 configurations — so many-key histories keep
-        //      the work list + scouts): finds the linearization of a VALID history in a few
-        //      thousand narrow levels where an exhaustive search visits 10^8..10^10 configurations; keys it decides are
-        //      VALID, the others go on to the exhaustive engine below ------------------------------------------------
-        std::vector<char> beam_found(n_shards, 0);
-        double beam_kernel_s = 0;
-        unsigned long long beam_configs = 0, beam_levels = 0, beam_attempts = 0, beam_decided = 0, beam_probes = 0;
-        ctx->stats[20] = ctx->stats[21] = ctx->stats[22] = ctx->stats[23] = 0;
-        if (P.max_nc > 0 && P.max_nc <= 64 * LV_CLS_WORDS && n_shards <= LV_BEAM_SHARDS && searchable.size() == 1 &&
-            P.n_ranks < LV_MAX_RANKS && !force_engine &&
-            !(ctx->opts.flags & (JTB_OPT_NO_BEAM | JTB_OPT_ENGINE_LEVEL | JTB_OPT_ENGINE_WORKLIST)) && !getenv("JTB_NO_BEAM") &&
-            !getenv("JTB_SCOUT_ONLY") && !getenv("JTB_ENGINE")) {
-            // A budgeted run of the work list first (16 M configurations, no scouts): easy histories — most
-            // histories with a few crashed ops — end there, at the work list's latency; only what it leaves open gets
-            // the beam ladder.
-            if (!ctx->in_probe) {
-                ctx->in_probe = true;
-                const jtb_opts saved = ctx->opts;
-                const uint64_t probe_budget = 16ull << 20;
-                ctx->opts.max_configs = saved.max_configs ? std::min<uint64_t>(saved.max_configs, probe_budget) : probe_budget;
-                ctx->opts.flags |= JTB_OPT_NO_SCOUTS;
-                std::vector<jtb_lin_shard> ps((size_t)n_shards);
-                jtb_lin_result po;
-                const int prc = check_lin_impl(ctx, h, m, ps.data(), &po, 2);
-                ctx->opts = saved;
-                ctx->in_probe = false;
-                if (prc) return prc;
-                bool all = true;
-                for (int s : searchable) all = all && ps[s].valid != JTB_UNKNOWN;
-                if (all) {
-                    for (int s = 0; s < n_shards; ++s) shards[s] = ps[s];
-                    *out = po;
-                    out->seconds_total = now_s() - t_start;
-                    return 0;
-                }
-            }
-            uint32_t widths[3] = {256u, 2048u, 16384u};
-            int n_widths = 3;
-            if (const char* bw = getenv("JTB_BEAM_W")) { widths[0] = (uint32_t)std::max(1, atoi(bw)); n_widths = 1; }   // experiments
-            for (int wi = 0; wi < n_widths && !searchable.empty(); ++wi) {
-                CK(cudaMemsetAsync(ctx->found.p, 0, n_shards * sizeof(int), ctx->stream));
-                for (int s = 0; s < n_shards; ++s) h_max[s] = (int)P.rank_base[s];
-                CK(cudaMemcpyAsync(ctx->maxrank.p, h_max.data(), n_shards * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
-                Ctrl bhc;
-                double ks = 0;
-                uint64_t bc = 0, bp = 0;
-                if (int rc = search_level(ctx, m, P, n_shards, searchable, init_entries, bhc, ks, bc, bp, widths[wi])) return rc;
-                CK(cudaMemcpyAsync(h_found.data(), ctx->found.p, n_shards * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-                CK(cudaStreamSynchronize(ctx->stream));
-                beam_kernel_s += ks; beam_configs += bc; beam_probes += bp; beam_levels += ctx->stats[2]; ++beam_attempts;
-                std::vector<int> left;
-                for (int s : searchable) {
-                    if (h_found[s]) { beam_found[s] = 1; ++beam_decided; }
-                    else left.push_back(s);
-                }
-                searchable.clear();
-                init_entries.clear();
-                for (int s : left) add_init(s);
-            }
-            ctx->stats[20] = beam_levels; ctx->stats[21] = beam_configs; ctx->stats[22] = beam_decided; ctx->stats[23] = beam_attempts;
-            std::fill(h_found.begin(), h_found.end(), 0);
-            for (int s = 0; s < n_shards; ++s) h_max[s] = 0;
-            if (searchable.empty()) {   // every key decided by the beam
-                kernel_s = beam_kernel_s; configs = beam_configs; probes = beam_probes;
-                std::memset(&hc, 0, sizeof hc);
-                hc.stop = 1;
-                ctx->stats[19] = 1;
-                ctx->last_engine = 1;
-            }
+    Search r(n_shards);
+    auto finish = [&](const Search& res) {
+        for (int s = 0; s < n_shards; ++s) {
+            out->valid = std::max(out->valid, shards[s].valid);
+            out->n_failures += shards[s].valid != JTB_VALID;
         }
-        if (!searchable.empty()) {
-        // ---- engine: level-synchronous sweep (jtb_level.cuh) or work list (jtb_wgl.cuh / jtb_search.cuh) ----------
+        out->configs_explored = res.configs;
+        out->probes = res.probes;
+        out->hbm_bytes_algorithmic = (uint64_t)KW * 8 * (res.probes + res.configs);
+        out->seconds_kernel = res.kernel_s;
+        out->seconds_total = now_s() - t_start;
+        return 0;
+    };
+    if (searchable.empty()) return finish(r);
+    if (upload(ctx, ctx->rows, P.rows) || upload(ctx, ctx->classes, P.classes) || upload(ctx, ctx->cls_inv, P.cls_inv_pos))
+        return -1;
+    if (ensure(ctx, ctx->ctrl, sizeof(Ctrl)) || ensure(ctx, ctx->found, n_shards * sizeof(int)) ||
+        ensure(ctx, ctx->maxrank, n_shards * sizeof(int)))
+        return -1;
+    const bool eager_mode = !(ctx->opts.flags & JTB_OPT_NO_EAGER_READS);
+    const bool scout_only = getenv("JTB_SCOUT_ONLY") != nullptr;   // test hook of the work-list engine
+    // ---- beam first (single-key histories with crashed ops; measured on the 8-key C5 "monster": one beam shared by
+    //      several keys starves most of them — 2 of 8 decided after 7.7e8 configurations — so many-key histories keep
+    //      the work list + scouts): finds the linearization of a VALID history in a few
+    //      thousand narrow levels where an exhaustive search visits 10^8..10^10 configurations; keys it decides are
+    //      VALID, the others go on to the exhaustive engine below ------------------------------------------------
+    std::vector<char> beam_found(n_shards, 0);
+    double beam_kernel_s = 0;
+    unsigned long long beam_configs = 0, beam_levels = 0, beam_attempts = 0, beam_decided = 0, beam_probes = 0;
+    ctx->stats[20] = ctx->stats[21] = ctx->stats[22] = ctx->stats[23] = 0;
+    if (P.max_nc > 0 && P.max_nc <= 64 * LV_CLS_WORDS && n_shards <= LV_BEAM_SHARDS && searchable.size() == 1 &&
+        P.n_ranks < LV_MAX_RANKS && !force_worklist && !scout_only &&
+        !(ctx->opts.flags & (JTB_OPT_NO_BEAM | JTB_OPT_ENGINE_LEVEL | JTB_OPT_ENGINE_WORKLIST))) {
+        // A budgeted run of the work list first (16 M configurations, no scouts): easy histories — most
+        // histories with a few crashed ops — end there, at the work list's latency; only what it leaves open gets
+        // the beam ladder.
+        const uint64_t probe_budget = 16ull << 20;
+        Search probe(n_shards);
+        if (int rc = search_worklist(ctx, h, m, P, searchable, init_entries,
+                                     ctx->opts.max_configs ? std::min<uint64_t>(ctx->opts.max_configs, probe_budget) : probe_budget,
+                                     /*scouts_on=*/false, t_start, probe))
+            return rc;
+        std::vector<jtb_lin_shard> ps(shards, shards + n_shards);
+        set_verdicts(ctx, h, P, searchable, probe, true, ps.data());
+        bool all = true;
+        for (int s : searchable) all = all && ps[s].valid != JTB_UNKNOWN;
+        if (all) {
+            std::copy(ps.begin(), ps.end(), shards);
+            return finish(probe);
+        }
+        uint32_t widths[3] = {256u, 2048u, 16384u};
+        int n_widths = 3;
+        if (const char* bw = getenv("JTB_BEAM_W")) { widths[0] = (uint32_t)std::max(1, atoi(bw)); n_widths = 1; }   // experiments
+        for (int wi = 0; wi < n_widths && !searchable.empty(); ++wi) {
+            Search b(n_shards);
+            if (arm_shards(ctx, P, n_shards, b.max_rank)) return -1;
+            if (int rc = search_level(ctx, m, P, n_shards, searchable, init_entries, b.hc, b.kernel_s, b.configs, b.probes, widths[wi]))
+                return rc;
+            CK(cudaMemcpyAsync(b.found.data(), ctx->found.p, n_shards * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+            CK(cudaStreamSynchronize(ctx->stream));
+            beam_kernel_s += b.kernel_s; beam_configs += b.configs; beam_probes += b.probes; beam_levels += ctx->stats[2]; ++beam_attempts;
+            std::vector<int> left;
+            for (int s : searchable) {
+                if (b.found[s]) { beam_found[s] = 1; ++beam_decided; }
+                else left.push_back(s);
+            }
+            searchable.clear();
+            init_entries.clear();
+            for (int s : left) add_init(s);
+        }
+        ctx->stats[20] = beam_levels; ctx->stats[21] = beam_configs; ctx->stats[22] = beam_decided; ctx->stats[23] = beam_attempts;
+        if (searchable.empty()) {   // every key decided by the beam
+            r.kernel_s = beam_kernel_s; r.configs = beam_configs; r.probes = beam_probes;
+            r.hc.stop = 1;
+            ctx->stats[19] = 1;
+            ctx->last_engine = 1;
+        }
+    }
+    if (!searchable.empty()) {
+        // ---- engine: level-synchronous sweep (jtb_level.cuh) or work list (jtb_wgl.cuh) ---------------------------
         // Default choice: histories with crashed ops -> work list (its depth-first
         // order + scouts find the linearization of a valid history long before a breadth-first sweep would);
         // Knossos-exact space -> level engine (higher throughput on wide levels, bounded memory);
@@ -676,345 +914,33 @@ static int check_lin_impl(jtb_ctx* ctx, const jtb_history* h, const jtb_model* m
         bool use_level = P.max_nc == 0 && (!eager_mode || P.mean_open >= 26.0);
         if (ctx->opts.flags & JTB_OPT_ENGINE_LEVEL) use_level = true;
         if (ctx->opts.flags & JTB_OPT_ENGINE_WORKLIST) use_level = false;
-        if (const char* en = getenv("JTB_ENGINE")) use_level = std::strcmp(en, "level") == 0;
-        if (force_engine) use_level = force_engine == 1;
-        if (getenv("JTB_SCOUT_ONLY")) use_level = false;                     // test hook of the work-list engine
+        if (force_worklist || scout_only) use_level = false;
         if (P.n_ranks >= LV_MAX_RANKS || P.max_nc > 64) use_level = false;   // epoch tag bits / class mask width
-        ctx->stats[19] = 0;
         if (use_level) {
-            CK(cudaMemsetAsync(ctx->found.p, 0, n_shards * sizeof(int), ctx->stream));
-            for (int s = 0; s < n_shards; ++s) h_max[s] = (int)P.rank_base[s];
-            CK(cudaMemcpyAsync(ctx->maxrank.p, h_max.data(), n_shards * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
-            if (int rc = search_level(ctx, m, P, n_shards, searchable, init_entries, hc, kernel_s, configs, probes)) return rc;
-            CK(cudaMemcpyAsync(h_found.data(), ctx->found.p, n_shards * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-            CK(cudaMemcpyAsync(h_max.data(), ctx->maxrank.p, n_shards * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+            if (arm_shards(ctx, P, n_shards, r.max_rank)) return -1;
+            if (int rc = search_level(ctx, m, P, n_shards, searchable, init_entries, r.hc, r.kernel_s, r.configs, r.probes)) return rc;
+            CK(cudaMemcpyAsync(r.found.data(), ctx->found.p, n_shards * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+            CK(cudaMemcpyAsync(r.max_rank.data(), ctx->maxrank.p, n_shards * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
             CK(cudaStreamSynchronize(ctx->stream));
-            ctx->last_configs = configs;
+            ctx->last_configs = r.configs;
             ctx->last_engine = 1;
-        } else {
-        ctx->last_engine = 0;
-        ctx->table_dirty = ~(size_t)0;   // the work-list engine fills the table
-        // CTA deque / grid.  Two interchangeable search kernels: "tpc" (one THREAD per configuration, jtb_search.cuh:
-        // throughput) and "warp" (one WARP per configuration, jtb_wgl.cuh: every child of a configuration probed in
-        // the same round trip).  Default tpc; env JTB_KERNEL=warp|tpc overrides (A/B measurements).
-        bool use_tpc = false;
-        if (const char* kk = getenv("JTB_KERNEL")) use_tpc = std::strcmp(kk, "warp") != 0;
-        const int cand_rounds = P.S_pad / 32, cls_rounds = (P.max_nc + 31) / 32;
-        // worst case of children one CTA step can push (overflow -> ring)
-        const uint32_t worst_push = use_tpc ? (uint32_t)TPC_THREADS * (uint32_t)std::min(P.S_pad + P.max_nc, 64)
-                                            : (WGL_BATCH + WGL_WARPS) * 32 * (cand_rounds + cls_rounds);
-        uint32_t deque_cap = 1024;                       // fixed: a full deque overflows to the ring
-        while ((size_t)deque_cap * EW * 8 > 48 * 1024) deque_cap >>= 1;
-        const uint32_t stage_cap = std::max(deque_cap, worst_push);
-        const size_t smem = use_tpc ? (size_t)deque_cap * EW * 8 : (size_t)(deque_cap + WGL_BATCH) * EW * 8;
-        // warp kernel: eager-read searches are small and latency-bound: 3 CTAs/SM (no register spills) wins; the
-        // Knossos-exact space is throughput-bound: 4 CTAs/SM (measured A/B, DESIGN.md)
-        const int want_ctas = use_tpc ? JTB_TPC_CTAS : (eager_mode ? JTB_CTAS_EAGER : JTB_CTAS_EXACT);
-        int ctas_per_sm = (int)std::min<size_t>(want_ctas, (220 * 1024) / (smem + 1024));
-        if (getenv("JTB_CTAS_PER_SM")) ctas_per_sm = std::min(ctas_per_sm, std::max(1, atoi(getenv("JTB_CTAS_PER_SM"))));
-        ctas_per_sm = std::max(1, ctas_per_sm);
-        const int grid = ctx->opts.search_ctas ? (int)ctx->opts.search_ctas : ctx->n_sms * ctas_per_sm;
-        const uint64_t per_step_push = (uint64_t)grid * stage_cap;  // worst case children of one step of every CTA
-        // work ring
-        uint64_t ring_entries = 1ull << 22;
-        while (ring_entries < 4 * per_step_push + 2 * searchable.size()) ring_entries <<= 1;
-        // test hook: start with a ring that is too small so that the RING_FULL pause/grow/resume path runs
-        const bool tiny_ring = getenv("JTB_TEST_TINY_RING") != nullptr;
-        if (ensure(ctx, ctx->pool, ring_entries * EW * 8)) return -1;
-        CK(cudaMemsetAsync(ctx->pool.p, 0, ring_entries * EW * 8, ctx->stream));
-        CK(cudaMemcpyAsync(ctx->pool.p, init_entries.data(), init_entries.size() * 8, cudaMemcpyHostToDevice, ctx->stream));
-        // visited table: start at 1 GiB (or the caller's size), grow x4 on load > 0.7 without losing work
-        size_t free_b = 0, total_b = 0;
-        CK(cudaMemGetInfo(&free_b, &total_b));
-        const size_t reserve = (size_t)4 << 30;
-        size_t max_table = ctx->opts.table_bytes ? ctx->opts.table_bytes : (size_t)64 << 30;
-        max_table = std::min(max_table, ctx->table.cap + (free_b > reserve ? free_b - reserve : 0));
-        // start at 1 GiB, or at 4x what the previous call on this context ended up needing (warm context)
-        const size_t min_start = getenv("JTB_TABLE_START_MB") ? (size_t)atoll(getenv("JTB_TABLE_START_MB")) << 20 : (size_t)1 << 30;
-        size_t start_bytes = std::max<size_t>(min_start, (size_t)ctx->last_configs * 4 * KW * 8);
-        size_t table_bytes = std::min<size_t>(max_table, ctx->opts.table_bytes ? ctx->opts.table_bytes : start_bytes);
-        uint64_t n_slots = 1;
-        while (n_slots * 2 * KW * 8 <= table_bytes) n_slots <<= 1;
-        if (ensure(ctx, ctx->table, n_slots * KW * 8)) return -1;
-        CK(cudaMemsetAsync(ctx->table.p, 0, n_slots * KW * 8, ctx->stream));
-        hc.tail = searchable.size();
-        hc.created = searchable.size();
-        hc.n_undecided = (int)searchable.size();
-        CK(cudaMemcpyAsync(ctx->ctrl.p, &hc, sizeof hc, cudaMemcpyHostToDevice, ctx->stream));
-        CK(cudaMemsetAsync(ctx->found.p, 0, n_shards * sizeof(int), ctx->stream));
-        for (int s = 0; s < n_shards; ++s) h_max[s] = (int)P.rank_base[s];
-        CK(cudaMemcpyAsync(ctx->maxrank.p, h_max.data(), n_shards * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
-        DevBuf ring2, table2;  // growth targets (freed below)
-        // cudaFree synchronizes the whole device, i.e. it would wait for the scouts: while they run, frees are deferred
-        // (cudaFree is valid for stream-ordered allocations too)
-        ScoutGuard scouts(ctx);
-        std::vector<void*> deferred;
-        auto free_tmp = [&]() {
-            scouts.stop();
-            for (void* q : deferred) cudaFree(q);
-            deferred.clear();
-            if (ring2.p) cudaFree(ring2.p);
-            if (table2.p) cudaFree(table2.p);
-            ring2 = DevBuf(); table2 = DevBuf();
-        };
-        auto grow_buf = [&](DevBuf& b, size_t bytes) -> int {
-            if (bytes <= b.cap) return 0;
-            if (b.p) { if (scouts.active) deferred.push_back(b.p); else cudaFree(b.p); }
-            b = DevBuf();
-            // cudaMalloc also synchronizes with running kernels (the search would sit behind the scouts for seconds at
-            // its first table growth); the stream-ordered allocator does not
-            const cudaError_t e = scouts.active ? cudaMallocAsync(&b.p, bytes, ctx->stream) : cudaMalloc(&b.p, bytes);
-            if (e != cudaSuccess) {
-                (void)cudaGetLastError();
-                b.p = nullptr;
-                if (scouts.stop()) return -1;   // out of memory with frees pending: give the scouts up
-                for (void* q : deferred) cudaFree(q);
-                deferred.clear();
-                CK(cudaMalloc(&b.p, bytes));
-            }
-            b.cap = bytes;
-            return 0;
-        };
-        int attempts = 0;
-        // table placement: plain hash, or (experiment switch JTB_WIN_LOG2) rank-windowed: a window of 2^JTB_WIN_LOG2
-        // slots whose origin moves by ~n_slots / n_ranks slots per frontier rank, so that the whole table is used
-        auto geometry = [&](uint64_t slots, uint64_t& win_mask, uint64_t& rank_stride) {
-            win_mask = slots - 1;
-            rank_stride = 0;
-            if (const char* wl = getenv("JTB_WIN_LOG2")) {
-                const int lg = atoi(wl);
-                if (lg > 0 && (1ull << lg) < slots) {
-                    win_mask = (1ull << lg) - 1;
-                    rank_stride = std::max<uint64_t>(1, (slots - (1ull << lg)) / (uint64_t)std::max<int64_t>(1, P.n_ranks));
-                }
-            }
-        };
-        CK(cudaEventRecord(ctx->ev0, ctx->stream));
-        WglParams pb{};   // what the search kernel and the scouts share
-        pb.rows = (const int32_t*)ctx->rows.p;
-        pb.classes = (const ClassRec*)ctx->classes.p;
-        pb.cls_inv_pos = (const int32_t*)ctx->cls_inv.p;
-        pb.ctrl = (Ctrl*)ctx->ctrl.p;
-        pb.shard_found = (int*)ctx->found.p;
-        pb.shard_max_rank = (int*)ctx->maxrank.p;
-        pb.row_words = P.row_words;
-        pb.S_pad = P.S_pad;
-        pb.n_shards = n_shards;
-        pb.max_nc = P.max_nc;
-        pb.eager_reads = (ctx->opts.flags & JTB_OPT_NO_EAGER_READS) ? 0 : 1;
-        // ---- depth-first scouts (jtb_scout.cuh): only where the crowd is known to drown — histories with
-        //      crashed ops — and launched FIRST so that they are resident before the persistent CTAs fill the SMs
-        int64_t max_shard_events = 0;
-        for (int s : searchable) max_shard_events = std::max<int64_t>(max_shard_events, h->shard_off[s + 1] - h->shard_off[s]);
-        int n_scouts = 0;
-        const bool scout_only = getenv("JTB_SCOUT_ONLY") != nullptr;   // test hook: no search kernel at all
-        if (!(ctx->opts.flags & JTB_OPT_NO_SCOUTS) && !getenv("JTB_NO_SCOUTS") && (P.max_nc > 0 || scout_only) &&
-            max_shard_events < (1ll << 29)) {
-            n_scouts = getenv("JTB_SCOUTS") ? std::max(1, atoi(getenv("JTB_SCOUTS"))) : SCOUT_ORDERS;
-            ScoutParams sp{};
-            sp.n_init = (int)searchable.size();
-            sp.n_orders = getenv("JTB_SCOUT_ORDERS") ? std::min(SCOUT_ORDERS, std::max(1, atoi(getenv("JTB_SCOUT_ORDERS")))) : SCOUT_ORDERS;
-            const uint64_t sc_slots = 1ull << 22;                       // 2 M configs per scout
-            sp.slot_mask = sc_slots - 1;
-            sp.stack_cap = (uint32_t)(max_shard_events + 2);            // a path linearizes each op at most once
-            sp.pair_budget = 8ull << 20;
-            if (upload(ctx, ctx->sc_init, init_entries) ||
-                ensure(ctx, ctx->sc_tables, (size_t)n_scouts * sc_slots * KW * 8) ||
-                ensure(ctx, ctx->sc_stacks, (size_t)n_scouts * sp.stack_cap * (EW + 1) * 8) ||
-                ensure(ctx, ctx->sc_ctl, SCOUT_CTL_WORDS * 8))
-                return -1;
-            CK(cudaMemsetAsync(ctx->sc_tables.p, 0, (size_t)n_scouts * sc_slots * KW * 8, ctx->stream));
-            CK(cudaMemsetAsync(ctx->sc_ctl.p, 0, SCOUT_CTL_WORDS * 8, ctx->stream));
-            sp.init = (const uint64_t*)ctx->sc_init.p;
-            sp.tables = (uint64_t*)ctx->sc_tables.p;
-            sp.stacks = (uint64_t*)ctx->sc_stacks.p;
-            sp.ctl = (unsigned long long*)ctx->sc_ctl.p;
-            CK(cudaEventRecord(ctx->ev_setup, ctx->stream));
-            CK(cudaStreamWaitEvent(ctx->scout_stream, ctx->ev_setup, 0));
-            int rc;
-            if (m->kind == JTB_MODEL_BANK) rc = preload_search_kw<JTB_MODEL_BANK>(ctx, KW, pb.eager_reads != 0);
-            else if (m->kind == JTB_MODEL_SET) rc = preload_search<JTB_MODEL_SET, 2>(ctx, pb.eager_reads != 0);
-            else rc = preload_search_kw<JTB_MODEL_CAS_REGISTER>(ctx, KW, pb.eager_reads != 0);
-            if (rc) return rc;
-            if (m->kind == JTB_MODEL_BANK) rc = launch_scout_kw<JTB_MODEL_BANK>(ctx, KW, pb, sp, m->negative_balances_ok, n_scouts);
-            else if (m->kind == JTB_MODEL_SET) rc = launch_scout<JTB_MODEL_SET, 2>(ctx, pb, sp, 0, n_scouts);
-            else rc = launch_scout_kw<JTB_MODEL_CAS_REGISTER>(ctx, KW, pb, sp, 0, n_scouts);
-            if (rc) return rc;
-            scouts.active = true;
+        } else if (int rc = search_worklist(ctx, h, m, P, searchable, init_entries, ctx->opts.max_configs,
+                                            !(ctx->opts.flags & JTB_OPT_NO_SCOUTS), t_start, r)) {
+            return rc;
         }
-        for (;;) {
-            ++attempts;
-            if (scout_only) { hc.stop = 2; hc.cause = JTB_CAUSE_BUDGET; break; }
-            WglParams p = pb;
-            p.table = (uint64_t*)ctx->table.p;
-            p.slot_mask = n_slots - 1;
-            geometry(n_slots, p.win_mask, p.rank_stride);
-            p.ring = (uint64_t*)ctx->pool.p;
-            p.ring_mask = ring_entries - 1;
-            p.ring_guard = (tiny_ring && attempts == 1) ? 20000 : ring_entries - 3 * per_step_push;
-            const uint64_t load_guard = (uint64_t)(0.50 * (double)n_slots);  // linear probing: keep chains short
-            p.max_configs = load_guard;
-            p.budget_cause = JTB_CAUSE_TABLE_FULL;
-            if (ctx->opts.max_configs && ctx->opts.max_configs <= load_guard) {
-                p.max_configs = ctx->opts.max_configs;
-                p.budget_cause = JTB_CAUSE_BUDGET;
-            }
-            p.time_budget_ns = (unsigned long long)ctx->opts.time_budget_ms * 1000000ull;
-            p.deque_cap = deque_cap;
-            p.cas_first = getenv("JTB_CAS_FIRST") ? atoi(getenv("JTB_CAS_FIRST")) : 0;
-            int rc;
-            if (use_tpc) {
-                if (m->kind == JTB_MODEL_BANK) rc = launch_tpc_kw<JTB_MODEL_BANK>(ctx, KW, p, m->negative_balances_ok, grid, smem);
-                else if (m->kind == JTB_MODEL_SET) rc = launch_tpc<JTB_MODEL_SET, 2>(ctx, p, 0, grid, smem);
-                else rc = launch_tpc_kw<JTB_MODEL_CAS_REGISTER>(ctx, KW, p, 0, grid, smem);
-            } else if (m->kind == JTB_MODEL_BANK) rc = launch_wgl_kw<JTB_MODEL_BANK>(ctx, KW, p, m->negative_balances_ok, grid, smem, ctas_per_sm);
-            else if (m->kind == JTB_MODEL_SET) rc = launch_wgl<JTB_MODEL_SET, 2>(ctx, p, 0, grid, smem, ctas_per_sm);
-            else rc = launch_wgl_kw<JTB_MODEL_CAS_REGISTER>(ctx, KW, p, 0, grid, smem, ctas_per_sm);
-            if (rc) { free_tmp(); return rc; }
-            CK(cudaMemcpyAsync(&hc, ctx->ctrl.p, sizeof hc, cudaMemcpyDeviceToHost, ctx->stream));
-            CK(cudaStreamSynchronize(ctx->stream));
-            const bool grow_table = hc.stop == 2 && hc.cause == JTB_CAUSE_TABLE_FULL && n_slots * KW * 8 * 4 <= max_table;
-            const bool grow_ring = hc.stop == 2 && hc.cause == CAUSE_RING_FULL && ring_entries * EW * 8 * 4 <= ((size_t)16 << 30);
-            if (!grow_table && !grow_ring) break;
-            if (hc.n_undecided <= 0) break;   // the scouts decided every shard while the search was pausing
-            // ---- pause/resume: the live work is exactly the non-zero ring slots ---------------------
-            const uint64_t new_ring_entries = grow_ring ? ring_entries * 4 : ring_entries;
-            if (grow_buf(ring2, new_ring_entries * EW * 8)) {   // no memory for the larger ring: give up like a full table
-                (void)cudaGetLastError();
-                hc.stop = 2; hc.cause = JTB_CAUSE_TABLE_FULL;
-                break;
-            }
-            CK(cudaMemsetAsync(ring2.p, 0, new_ring_entries * EW * 8, ctx->stream));
-            Ctrl* dc = (Ctrl*)ctx->ctrl.p;
-            CK(cudaMemsetAsync(&dc->tail, 0, sizeof(unsigned long long), ctx->stream));
-            if (EW == 2) ring_compact_kernel<2><<<ctx->n_sms * 8, 256, 0, ctx->stream>>>((const uint64_t*)ctx->pool.p, ring_entries - 1, 0, ring_entries, (uint64_t*)ring2.p, new_ring_entries - 1, &dc->tail);
-            else if (EW == 4) ring_compact_kernel<4><<<ctx->n_sms * 8, 256, 0, ctx->stream>>>((const uint64_t*)ctx->pool.p, ring_entries - 1, 0, ring_entries, (uint64_t*)ring2.p, new_ring_entries - 1, &dc->tail);
-            else if (EW == 6) ring_compact_kernel<6><<<ctx->n_sms * 8, 256, 0, ctx->stream>>>((const uint64_t*)ctx->pool.p, ring_entries - 1, 0, ring_entries, (uint64_t*)ring2.p, new_ring_entries - 1, &dc->tail);
-            else if (EW == 8) ring_compact_kernel<8><<<ctx->n_sms * 8, 256, 0, ctx->stream>>>((const uint64_t*)ctx->pool.p, ring_entries - 1, 0, ring_entries, (uint64_t*)ring2.p, new_ring_entries - 1, &dc->tail);
-            else ring_compact_kernel<12><<<ctx->n_sms * 8, 256, 0, ctx->stream>>>((const uint64_t*)ctx->pool.p, ring_entries - 1, 0, ring_entries, (uint64_t*)ring2.p, new_ring_entries - 1, &dc->tail);
-            CK(cudaGetLastError());
-            std::swap(ctx->pool, ring2);
-            ring_entries = new_ring_entries;
-            CK(cudaMemsetAsync(&dc->head, 0, sizeof(unsigned long long), ctx->stream));
-            wgl_resume_ctrl_kernel<<<1, 1, 0, ctx->stream>>>(dc);   // stop, cause := 0 (unless everything is decided)
-            CK(cudaGetLastError());
-            if (grow_table) {
-                const uint64_t new_slots = n_slots * 4;
-                if (grow_buf(table2, new_slots * KW * 8)) {   // old + 4x table do not fit together: UNKNOWN, not an error
-                    (void)cudaGetLastError();
-                    hc.stop = 2; hc.cause = JTB_CAUSE_TABLE_FULL;
-                    break;
-                }
-                CK(cudaMemsetAsync(table2.p, 0, new_slots * KW * 8, ctx->stream));
-                uint64_t g_win, g_stride;
-                geometry(new_slots, g_win, g_stride);
-                if (KW == 2) table_rehash_kernel<2><<<ctx->n_sms * 8, 256, 0, ctx->stream>>>((const uint64_t*)ctx->table.p, n_slots, (uint64_t*)table2.p, new_slots - 1, g_win, g_stride, &dc->overflow);
-                else if (KW == 4) table_rehash_kernel<4><<<ctx->n_sms * 8, 256, 0, ctx->stream>>>((const uint64_t*)ctx->table.p, n_slots, (uint64_t*)table2.p, new_slots - 1, g_win, g_stride, &dc->overflow);
-                else table_rehash_kernel<8><<<ctx->n_sms * 8, 256, 0, ctx->stream>>>((const uint64_t*)ctx->table.p, n_slots, (uint64_t*)table2.p, new_slots - 1, g_win, g_stride, &dc->overflow);
-                CK(cudaGetLastError());
-                CK(cudaStreamSynchronize(ctx->stream));
-                std::swap(ctx->table, table2);
-                if (table2.p) {   // release the old table right away (deferred while the scouts run)
-                    if (scouts.active) deferred.push_back(table2.p); else cudaFree(table2.p);
-                    table2 = DevBuf();
-                }
-                n_slots = new_slots;
-            }
-        }
-        unsigned long long sc_ctl[SCOUT_CTL_WORDS] = {0};
-        if (n_scouts) {
-            // the search gave up (UNKNOWN) while scouts are still walking: give them a grace period
-            if (hc.stop == 2 && hc.n_undecided > 0) {
-                double grace_s = getenv("JTB_SCOUT_GRACE_MS") ? atof(getenv("JTB_SCOUT_GRACE_MS")) * 1e-3 : 20.0;
-                if (ctx->opts.time_budget_ms)
-                    grace_s = std::max(0.0, ctx->opts.time_budget_ms * 1e-3 - (now_s() - t_start));
-                const double deadline = now_s() + grace_s;
-                while (now_s() < deadline && cudaStreamQuery(ctx->scout_stream) == cudaErrorNotReady)
-                    std::this_thread::sleep_for(std::chrono::microseconds(200));
-            }
-            (void)cudaGetLastError();
-            if (scouts.stop()) { free_tmp(); return -1; }
-            CK(cudaMemcpyAsync(sc_ctl, ctx->sc_ctl.p, sizeof sc_ctl, cudaMemcpyDeviceToHost, ctx->stream));
-        }
-        fc_n_slots = n_slots;
-        scout_only_run = scout_only;
-        CK(cudaEventRecord(ctx->ev1, ctx->stream));
-        CK(cudaMemcpyAsync(h_found.data(), ctx->found.p, n_shards * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaMemcpyAsync(h_max.data(), ctx->maxrank.p, n_shards * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));
-        free_tmp();
-        float ms = 0;
-        CK(cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1));
-        kernel_s = ms * 1e-3;
-        configs = hc.configs;
-        probes = hc.probes;
-        ctx->last_configs = hc.configs;
-        {
-            unsigned long long* st = ctx->stats;
-            st[0] = hc.configs; st[1] = hc.probes; st[2] = hc.expansions; st[3] = hc.tail;
-            st[4] = hc.head; st[5] = hc.polls; st[6] = hc.max_probe_len; st[7] = n_slots;
-            st[8] = (unsigned long long)grid; st[9] = ring_entries; st[10] = (unsigned long long)attempts;
-            st[11] = (unsigned long long)(ms * 1e3);
-            st[12] += init_entries.size() * 8 + sizeof(Ctrl) + (size_t)n_shards * 4;
-            st[13] = (unsigned long long)attempts * sizeof(Ctrl) + (size_t)n_shards * 8;  // device -> host bytes
-            st[14] = (unsigned long long)((scout_only ? 0 : attempts) + 3 * (attempts - 1) + (n_scouts ? 1 : 0));  // search + compact/rehash/re-arm + scouts
-            st[15] = sc_ctl[2]; st[16] = sc_ctl[3]; st[17] = sc_ctl[4]; st[18] = (unsigned long long)n_scouts;
-        }
-        }   // engine
-        kernel_s += beam_kernel_s;
-        }   // something left for the exhaustive engines
-        for (int s = 0; s < n_shards; ++s)
-            if (beam_found[s]) shards[s].valid = JTB_VALID;
-        if (hc.stop == 2 && hc.cause == CAUSE_RING_FULL) hc.cause = JTB_CAUSE_BUDGET;
-        if (hc.overflow) {   // a ring slot was overwritten before it was consumed: no verdict may be derived from this search
-            hc.stop = 2;
-            hc.cause = JTB_CAUSE_BUDGET;
-            std::fill(h_found.begin(), h_found.end(), 0);
-        }
-        for (int s : searchable) {
-            jtb_lin_shard& r = shards[s];
-            if (h_found[s]) {
-                r.valid = JTB_VALID;
-            } else if (hc.stop == 2) {
-                r.valid = JTB_UNKNOWN;
-                r.cause = hc.cause;
-            } else {
-                r.valid = JTB_INVALID;
-                const int64_t g = h_max[s];
-                r.witness_index = P.ret_index[g];
-                if (g > P.rank_base[s]) r.previous_ok_index = P.ret_index[g - 1];
-            }
-        }
-        if (n_shards == 1) {
-            shards[0].configs_explored = configs;
-            shards[0].probes = probes;
-        }
-        ctx->fc.valid = !scout_only_run;
-        ctx->fc.n_events = h->n_events;
-        ctx->fc.n_shards = n_shards;
-        ctx->fc.kw = KW;
-        ctx->fc.n_slots = fc_n_slots;
-        ctx->fc.max_rank = h_max;
-        ctx->fc.verdict.assign(n_shards, JTB_UNKNOWN);
-        for (int s = 0; s < n_shards; ++s) ctx->fc.verdict[s] = shards[s].valid;
+        r.kernel_s += beam_kernel_s;
     }
-    for (int s = 0; s < n_shards; ++s) {
-        out->valid = std::max(out->valid, shards[s].valid);
-        out->n_failures += shards[s].valid != JTB_VALID;
-    }
-    out->configs_explored = configs;
-    out->probes = probes;
-    out->hbm_bytes_algorithmic = (uint64_t)KW * 8 * (probes + configs);
-    out->seconds_kernel = kernel_s;
-    out->seconds_total = now_s() - t_start;
-    return 0;
+    for (int s = 0; s < n_shards; ++s)
+        if (beam_found[s]) shards[s].valid = JTB_VALID;
+    set_verdicts(ctx, h, P, searchable, r, !scout_only, shards);
+    return finish(r);
 }
 
 int jtb_check_linearizable(jtb_ctx* ctx, const jtb_history* h, const jtb_model* m, jtb_lin_shard* shards,
                            jtb_lin_result* out) {
     if (!ctx) return -1;
     std::lock_guard<std::mutex> lk(ctx->mu);
-    return check_lin_impl(ctx, h, m, shards, out, 0);
+    return check_lin_impl(ctx, h, m, shards, out, false);
 }
 
 // -------------------------------------------------------------------------------------------------
@@ -1029,7 +955,7 @@ int jtb_final_configs(jtb_ctx* ctx, const jtb_history* h, const jtb_model* m, in
         // visited configuration (same verdict and witness; only asked for after an INVALID verdict)
         std::vector<jtb_lin_shard> tmp_shards((size_t)h->n_shards);
         jtb_lin_result tmp_out;
-        if (int rc = check_lin_impl(ctx, h, m, tmp_shards.data(), &tmp_out, 2)) return rc;
+        if (int rc = check_lin_impl(ctx, h, m, tmp_shards.data(), &tmp_out, true)) return rc;
     }
     if (!ctx->fc.valid || h->n_events != ctx->fc.n_events || h->n_shards != ctx->fc.n_shards || shard < 0 ||
         shard >= h->n_shards) {
@@ -1068,9 +994,12 @@ int jtb_final_configs(jtb_ctx* ctx, const jtb_history* h, const jtb_model* m, in
             if (pass == 1 && ensure(ctx, d_out, want * KW * 8)) { free_all(); return -1; }
             CK(cudaMemsetAsync(d_cnt.p, 0, 8, ctx->stream));
             const int grid = ctx->n_sms * 8;
-            if (KW == 2) table_collect_kernel<2><<<grid, 256, 0, ctx->stream>>>(table, ctx->fc.n_slots, (uint32_t)g, (uint64_t*)d_out.p, want, (unsigned long long*)d_cnt.p);
-            else if (KW == 4) table_collect_kernel<4><<<grid, 256, 0, ctx->stream>>>(table, ctx->fc.n_slots, (uint32_t)g, (uint64_t*)d_out.p, want, (unsigned long long*)d_cnt.p);
-            else table_collect_kernel<8><<<grid, 256, 0, ctx->stream>>>(table, ctx->fc.n_slots, (uint32_t)g, (uint64_t*)d_out.p, want, (unsigned long long*)d_cnt.p);
+            if (int rc = dispatch_model_kw(ctx, m->kind, KW, [&](auto, auto K) {
+                    table_collect_kernel<K()><<<grid, 256, 0, ctx->stream>>>(table, ctx->fc.n_slots, (uint32_t)g, (uint64_t*)d_out.p,
+                                                                             want, (unsigned long long*)d_cnt.p);
+                    return 0;
+                }))
+                return rc;
             CK(cudaGetLastError());
             CK(cudaMemcpyAsync(&total, d_cnt.p, 8, cudaMemcpyDeviceToHost, ctx->stream));
             CK(cudaStreamSynchronize(ctx->stream));

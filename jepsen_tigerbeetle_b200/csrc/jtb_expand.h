@@ -1,4 +1,4 @@
-// jtb_expand.h — ONE thread expands ONE configuration: the per-thread core of the search kernel (jtb_search.cuh).
+// jtb_expand.h — ONE thread expands ONE configuration: the per-thread core of the level engine (jtb_level.cuh).
 //
 // Replaces the inner loop of knossos.wgl/analysis (SURVEY.md A.5: `step` over every call entry that may be
 // linearized next, then `cache.add`).  The same code compiles for the device (inlined into the persistent kernel) and

@@ -2,7 +2,7 @@
 //
 // Replaces the hot loop of knossos.wgl/analysis (SURVEY.md A.5: `step` over every call entry that may be linearized
 // next, then `cache.add((linearized BitSet, model))`) for exhaustive searches.  Same configurations, same keys, same
-// per-thread expansion core (jtb_expand.h) as the work-list engines (jtb_wgl.cuh / jtb_search.cuh); what differs is the
+// per-thread expansion core (jtb_expand.h) as the work-list engine (jtb_wgl.cuh); what differs is the
 // ORDER, and what that order buys on an H100:
 //
 //   depth(config) = number of linearized ops = frontier rank + popcount(open-slot mask) + crashed-class counts is a

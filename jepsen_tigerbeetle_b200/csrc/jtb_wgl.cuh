@@ -65,8 +65,6 @@ struct WglParams {
     const int32_t* cls_inv_pos;
     uint64_t* table;        // slots of KW 64-bit words
     uint64_t slot_mask;     // n_slots - 1
-    uint64_t win_mask;      // rank-windowed placement: home slot = (rank * rank_stride + (hash & win_mask)) & slot_mask;
-    uint64_t rank_stride;   //   win_mask == slot_mask, rank_stride == 0 is the plain hash table
     uint64_t* ring;         // work queue: entries of EW words, word0 != 0 <=> slot holds an entry
     uint64_t ring_mask;     // ring entries - 1
     uint64_t ring_guard;    // pause when (tail - head) exceeds this
@@ -78,7 +76,6 @@ struct WglParams {
     int budget_cause;                 // JTB_CAUSE_BUDGET or JTB_CAUSE_TABLE_FULL (load guard)
     unsigned long long time_budget_ns;
     uint32_t deque_cap;     // entries in the CTA's shared-memory deque (power of two)
-    int cas_first;          // probe with atom.cas first (experiment switch, env JTB_CAS_FIRST)
     int eager_reads;        // linearize a consistent candidate read immediately and exclusively
 };
 
@@ -144,20 +141,11 @@ __device__ __forceinline__ uint64_t hash_key(const uint64_t (&k)[KW]) {
 }
 
 // Visited-table probe + insert.  Returns 1 = inserted (new config), 0 = already present,
-// -1 = table exhausted.  *plen gets the number of slots inspected.
-// Home slot of a key.  Plain table: hash & slot_mask.  Rank-windowed table (win_mask < slot_mask): the hash only picks
-// a position inside a window of win_mask + 1 slots whose origin moves with the key's frontier rank, so the probes of
-// a search that works on a narrow band of ranks stay inside a few windows (L2-resident) instead of all of HBM.
+// -1 = table exhausted.  *plen gets the number of slots inspected.  Linear probing from hash & slot_mask.
 template <int KW>
-__device__ __forceinline__ uint64_t table_home(const uint64_t (&k)[KW], uint64_t slot_mask, uint64_t win_mask,
-                                               uint64_t rank_stride) {
-    const uint64_t rank = (k[0] >> 32) & RANK_MASK;
-    return (rank * rank_stride + (hash_key<KW>(k) & win_mask)) & slot_mask;
-}
-
-template <int KW>
-__device__ __forceinline__ int table_insert_at(uint64_t* table, uint64_t slot_mask, uint64_t idx,
-                                               const uint64_t (&k)[KW], int* plen, bool cas_first = false) {
+__device__ __forceinline__ int table_insert(uint64_t* table, uint64_t slot_mask, const uint64_t (&k)[KW], int* plen,
+                                            bool cas_first = false) {
+    uint64_t idx = hash_key<KW>(k) & slot_mask;
     for (int i = 0; i < MAX_PROBE; ++i) {
         uint64_t* slot = table + idx * KW;
         // load-first: hits (the majority) cost one plain load; cas-first: new configs cost one round trip
@@ -193,18 +181,6 @@ __device__ __forceinline__ int table_insert_at(uint64_t* table, uint64_t slot_ma
     }
     *plen = MAX_PROBE;
     return -1;
-}
-
-template <int KW>
-__device__ __forceinline__ int table_insert(uint64_t* table, uint64_t slot_mask, const uint64_t (&k)[KW],
-                                            int* plen, bool cas_first = false) {
-    return table_insert_at<KW>(table, slot_mask, hash_key<KW>(k) & slot_mask, k, plen, cas_first);
-}
-
-template <int KW>
-__device__ __forceinline__ int table_insert_p(const WglParams& p, const uint64_t (&k)[KW], int* plen, bool cas_first = false) {
-    return table_insert_at<KW>(p.table, p.slot_mask, table_home<KW>(k, p.slot_mask, p.win_mask, p.rank_stride), k, plen,
-                               cas_first);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -263,8 +239,7 @@ __device__ __forceinline__ bool model_step(const int4 op, int32_t& reg, int32_t 
 // candidate round).  Shared by the search kernels; `wit_cache` is a shared-memory filter for the witness atomicMax.
 template <int MODEL, int KW, bool EAGER, typename Push>
 __device__ __forceinline__ void expand_config(const WglParams& p, Ctrl* ctrl, const int neg_ok, const uint64_t (&w)[KW],
-                                              const int32_t (&pbal)[8], const int lane, const bool cas_first,
-                                              unsigned long long* wit_cache, unsigned long long& my_probes,
+                                              const int32_t (&pbal)[8], const int lane, unsigned long long* wit_cache, unsigned long long& my_probes,
                                               int& my_max_probe, Push&& push) {
     constexpr int SW = MODEL == JTB_MODEL_BANK ? 12 : MODEL == JTB_MODEL_SET ? 8 : 4;  // = slot_words(MODEL)
     const int cand_rounds = p.S_pad / 32;
@@ -361,7 +336,7 @@ __device__ __forceinline__ void expand_config(const WglParams& p, Ctrl* ctrl, co
                 }
             } else {
                 int plen;
-                const int res = table_insert_p<KW>(p, cw, &plen, cas_first);
+                const int res = table_insert<KW>(p.table, p.slot_mask, cw, &plen);
                 my_probes++;
                 my_max_probe = max(my_max_probe, plen);
                 if (res < 0) {
@@ -416,7 +391,7 @@ __device__ __forceinline__ void expand_config(const WglParams& p, Ctrl* ctrl, co
         int is_new = 0;
         if (ok) {
             int plen;
-            const int res = table_insert_p<KW>(p, cw, &plen, cas_first);
+            const int res = table_insert<KW>(p.table, p.slot_mask, cw, &plen);
             my_probes++;
             my_max_probe = max(my_max_probe, plen);
             if (res < 0) {
@@ -616,7 +591,6 @@ __global__ void __launch_bounds__(WGL_THREADS, MINB) wgl_search_kernel(const Wgl
             pre_tail = ld_volatile(&ctrl->tail);
         }
 
-        const bool cas_first = p.cas_first != 0;
         // ---- self-scheduled expansion: next staged entry, else one poll of my ring ticket ---------------
         bool polled = false;
         unsigned n_done = 0;
@@ -734,7 +708,7 @@ __global__ void __launch_bounds__(WGL_THREADS, MINB) wgl_search_kernel(const Wgl
                 int res = 0;
                 if (lane == 0) {
                     int plen;
-                    res = table_insert_p<KW>(p, w, &plen, cas_first);
+                    res = table_insert<KW>(p.table, p.slot_mask, w, &plen);
                 }
                 res = __shfl_sync(0xffffffffu, res, 0);
                 if (res <= 0) {
@@ -754,7 +728,7 @@ __global__ void __launch_bounds__(WGL_THREADS, MINB) wgl_search_kernel(const Wgl
                 }
             }
             if (expand)
-                expand_config<MODEL, KW, EAGER>(p, ctrl, neg_ok, w, pbal, lane, cas_first, &sh.wit_cache, my_probes,
+                expand_config<MODEL, KW, EAGER>(p, ctrl, neg_ok, w, pbal, lane, &sh.wit_cache, my_probes,
                                                 my_max_probe, push_children);
             if (lane == 0) {
                 if (n_new_local) atomicAdd(&sh.n_new, (unsigned)n_new_local);
@@ -808,7 +782,7 @@ __global__ void ring_compact_kernel(const uint64_t* __restrict__ old_ring, uint6
 // Re-inserts every key of a full table into a larger one (table growth without losing work).
 template <int KW>
 __global__ void table_rehash_kernel(const uint64_t* __restrict__ old_table, uint64_t old_slots, uint64_t* new_table,
-                                    uint64_t new_mask, uint64_t win_mask, uint64_t rank_stride, int* lost = nullptr) {
+                                    uint64_t new_mask, int* lost = nullptr) {
     for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < old_slots; i += (uint64_t)gridDim.x * blockDim.x) {
         uint64_t k[KW];
 #pragma unroll
@@ -817,7 +791,7 @@ __global__ void table_rehash_kernel(const uint64_t* __restrict__ old_table, uint
         int plen;
         // a 4x larger table at load <= 1/8 cannot run out of probe slots; if it ever did, a visited key would be lost
         // and the search would re-expand it (wrong counts): the host turns the flag into UNKNOWN
-        if (table_insert_at<KW>(new_table, new_mask, table_home<KW>(k, new_mask, win_mask, rank_stride), k, &plen) < 0 && lost)
+        if (table_insert<KW>(new_table, new_mask, k, &plen) < 0 && lost)
             atomicExch(lost, 1);
     }
 }

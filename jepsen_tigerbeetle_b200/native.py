@@ -17,7 +17,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("JTB_LIB_PATH") or os.path.join(_HERE, "libjtb_check.so")  # env: A/B experiments only
 CSRC = os.path.join(_HERE, "csrc")
 _SOURCES = ["jtb_abi.cu", "jtb_prep.cpp", "jtb_multi.cpp"]
-_DEPS = _SOURCES + ["jtb_prep.h", "jtb_expand.h", "jtb_wgl.cuh", "jtb_search.cuh", "jtb_scout.cuh", "jtb_scans.cuh",
+_DEPS = _SOURCES + ["jtb_prep.h", "jtb_expand.h", "jtb_wgl.cuh", "jtb_scout.cuh", "jtb_scans.cuh",
                     "jtb_table_bench.cuh", "jtb_level.cuh", "jtb_partition.cuh"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared", "-ldl"]
