@@ -35,7 +35,7 @@
 (def model-code {:register 0 :cas-register 1 :set 2 :bank 3})
 (def NIL Integer/MIN_VALUE)
 (def verdict    {0 true 1 :unknown 2 false})
-(def cause      {0 nil 1 :table-full 2 :budget 3 :too-wide})
+(def cause      {0 nil 1 :table-full 2 :budget 3 :too-wide 4 :partial-read})
 (def bank-error {1 :unexpected-key 2 :nil-balance 3 :wrong-total 4 :negative-value})
 
 (defn- ledger->bank-op
@@ -53,6 +53,28 @@
       :l-t nil
       nil)))
 
+(defn- ledger->counters-op
+  "One client op for the monotonic-key check: an :ok :r keeps every account's two counters as [key value-lo value-hi]
+  triples, key = 2*account + field (0 debits-posted, 1 credits-posted); an account with nil amounts is left out (the
+  read is then partial).  nil for :l-t ops, as ledger->bank drops them."
+  [{:keys [type value] :as op}]
+  (let [[f _ _] (first value)]
+    (case f
+      :r   (assoc op :f :read
+                  :value (when (= :ok type)
+                           (vec (for [[_ id amounts] value
+                                      :when amounts
+                                      :let [_ (when-not (and (<= 0 id) (< id (bit-shift-left 1 30)))
+                                                (throw (IllegalArgumentException. (str "account " id " outside [0, 2^30)"))))]
+                                      [field k] [[0 :debits-posted] [1 :credits-posted]]
+                                      :let [x (get amounts k)]
+                                      :when (some? x)
+                                      :let [x (long x)]]
+                                  [(+ (* 2 id) field) (unchecked-int x) (unchecked-int (bit-shift-right x 32))]))))
+      :t   (let [[_ _ v] (first value)] (assoc op :f :transfer :value v))
+      :l-t nil
+      nil)))
+
 (defn- int-or-nil [x] (if (nil? x) NIL (int x)))
 
 (defn flatten-history
@@ -63,7 +85,9 @@
   [model history]
   (let [ops   (->> history
                    (filter (comp int? :process))
-                   (keep (fn [op] (if (= :txn (:f op)) (ledger->bank-op op) op)))
+                   (keep (fn [op] (if (= :txn (:f op))
+                                    ((if (= model :ledger-counters) ledger->counters-op ledger->bank-op) op)
+                                    op)))
                    (keep (fn [op]
                            (let [v (:value op)]
                              (if (independent/tuple? v)
@@ -102,7 +126,9 @@
           [:set :read]  (put-payload! (when (and value (= :ok (:type o))) (sort value)))
           [:bank :read] (put-payload! (when (and value (= :ok (:type o)))
                                         (mapcat (fn [[id bal]] [id (int-or-nil bal)]) value)))
-          [:bank :transfer] (do (aset a i (int (:amount value)))
+          [:ledger-counters :read] (put-payload! (when (and value (= :ok (:type o))) (apply concat value)))
+          ([:bank :transfer] [:ledger-counters :transfer])
+                            (do (aset a i (int (:amount value)))
                                 (aset b i (int (or (:debit-acct value) (:from value))))
                                 (aset c i (int (or (:credit-acct value) (:to value)))))
           nil)))                                    ; any other :f: opcode 0 with no value — ignored by every checker
@@ -289,6 +315,31 @@
           (assoc out :valid? :unknown
                  :error "java.lang.ArithmeticException: Divide by zero (err-badness, tests/ledger.clj:122-123)")
           out)))))
+
+;; ---- monotonic keys -------------------------------------------------------------------------------------------
+(def ^:private counter-field [:debits-posted :credits-posted])
+
+(defn monotonic-key-checker
+  "Elle's monotonic-key graph over the ledger's counters (src/tigerbeetle/elle/core.clj) plus real-time order, on the
+  GPU: a cycle proves that no (real-time respecting) serial order explains the reads.  Add it to the compose map at
+  tests/ledger.clj:363-367 as `:monotonic (monotonic-key-checker {})`; {:realtime? false} gives the literal
+  elle/core.clj graph.  Result: {:valid? :read-count :key-count [:cause] [:op :cycle :steps]}."
+  [{:keys [realtime?] :or {realtime? true}}]
+  (reify checker/Checker
+    (check [_ _test history _opts]
+      (let [{:keys [arrays by-index]} (flatten-history :ledger-counters history)
+            res  (Native/checkMonotonicKeys @ctx arrays (boolean realtime?))
+            at   (fn [i] (aget res (int i)))
+            s    6                                       ; shard 0: valid cause reads keys witness partner, edges
+            step (fn [o] (if (= 1 (at o))
+                           {:type :monotonic :key [(quot (at (+ o 1)) 2) (counter-field (rem (at (+ o 1)) 2))]
+                            :value (at (+ o 2)) :value' (at (+ o 3))}
+                           {:type :realtime :value (at (+ o 2)) :value' (at (+ o 3))}))]
+        (cond-> {:valid? (verdict (at s)) :read-count (at (+ s 2)) :key-count (at (+ s 3))}
+          (= 1 (at s)) (assoc :cause (cause (at (+ s 1))))
+          (= 2 (at s)) (assoc :op    (by-index (at (+ s 4)))
+                              :cycle [(by-index (at (+ s 5))) (by-index (at (+ s 4))) (by-index (at (+ s 5)))]
+                              :steps [(step (+ s 6)) (step (+ s 10))]))))))
 
 ;; ---- independent ----------------------------------------------------------------------------------------------
 (defn independent-checker

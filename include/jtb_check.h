@@ -24,7 +24,7 @@
 extern "C" {
 #endif
 
-#define JTB_ABI_VERSION 2
+#define JTB_ABI_VERSION 3
 
 /* ---- verdict lattice (jepsen.checker/merge-valid) ------------------------------------------- */
 #define JTB_VALID   0
@@ -149,6 +149,7 @@ typedef struct jtb_lin_shard {
 #define JTB_CAUSE_TABLE_FULL    1 /* visited table exhausted (knossos: out of memory -> :unknown)    */
 #define JTB_CAUSE_BUDGET        2 /* max_configs / time budget reached                                */
 #define JTB_CAUSE_TOO_WIDE      3 /* > 64 concurrently open completed ops, or key does not fit        */
+#define JTB_CAUSE_PARTIAL_READ  4 /* monotonic-key check: an :ok read does not observe every key of its shard */
 
 typedef struct jtb_lin_result {
     int32_t  valid;             /* merge-valid over shards                                            */
@@ -233,13 +234,50 @@ typedef struct jtb_bank_result {
     double  seconds_total;
 } jtb_bank_result;
 
+/* ---- monotonic-key check (Elle's monotonic-key graph, src/tigerbeetle/elle/core.clj) ------------------------------
+ * Nodes are the :ok reads (process >= 0, f == JTB_F_READ, type == JTB_T_OK, payload_len >= 0).  A read's payload is
+ * (key:int32, value_lo:int32, value_hi:int32) triples, value = int64; for ledger histories key = 2*account + field,
+ * field 0 = debits-posted, 1 = credits-posted (counters that only grow).  Edges:
+ *   monotonic  r -> s  when v_k(r) < v_k(s) for some key k both read
+ *   real-time  r -> s  when r's completion precedes s's invocation (the latest invoke of s's process before s
+ *                      completes; off with JTB_MONO_NO_REALTIME)
+ * A shard is JTB_INVALID when the graph has a cycle.  A shard in which some :ok read does not observe every key of
+ * the shard is JTB_UNKNOWN with JTB_CAUSE_PARTIAL_READ.  DESIGN.md "K7 monotonic-key check". */
+#define JTB_MONO_NO_REALTIME 1
+
+#define JTB_MONO_EDGE_NONE      0
+#define JTB_MONO_EDGE_MONOTONIC 1 /* edge_key = key, edge_value = v_key(source), edge_value2 = v_key(target)      */
+#define JTB_MONO_EDGE_REALTIME  2 /* edge_key = -1, edge_value = :index of the source's completion,
+                                     edge_value2 = :index of the target's invocation                             */
+
+typedef struct jtb_mono_shard {
+    int32_t valid;              /* JTB_VALID / JTB_UNKNOWN / JTB_INVALID                                          */
+    int32_t cause;              /* JTB_CAUSE_* when valid == JTB_UNKNOWN                                          */
+    int32_t n_reads;            /* :ok reads (graph nodes) of the shard                                           */
+    int32_t n_keys;             /* distinct keys the shard's :ok reads observe                                    */
+    int32_t witness_index;      /* :index of the earliest :ok read completion whose prefix has a cycle, -1        */
+    int32_t partner_index;      /* smallest completion :index of a read forming a 2-cycle with the witness, -1    */
+    int32_t edge_kind[2];       /* [0] partner -> witness, [1] witness -> partner: JTB_MONO_EDGE_*                */
+    int32_t edge_key[2];
+    int64_t edge_value[2];
+    int64_t edge_value2[2];
+} jtb_mono_shard;
+
+typedef struct jtb_mono_result {
+    int32_t valid;              /* merge-valid over shards                                                         */
+    int32_t n_failures;         /* shards whose verdict is not JTB_VALID                                           */
+    int64_t n_reads;            /* :ok reads over all shards                                                       */
+    double  seconds_kernel;     /* device time (CUDA events)                                                       */
+    double  seconds_total;      /* host wall time of the call incl. the host pass, H2D, D2H                        */
+} jtb_mono_result;
+
 typedef struct jtb_ctx jtb_ctx;
 
 /* ---- lifecycle -------------------------------------------------------------------------------- */
 int         jtb_abi_version(void);
 /* sizeof of the ABI structs as this library was compiled, for binding self-checks:
  * 0 jtb_history, 1 jtb_model, 2 jtb_opts, 3 jtb_lin_shard, 4 jtb_lin_result, 5 jtb_setfull_shard,
- * 6 jtb_setfull_out, 7 jtb_bank_result, 8 jtb_final_config; -1 otherwise */
+ * 6 jtb_setfull_out, 7 jtb_bank_result, 8 jtb_final_config, 9 jtb_mono_shard, 10 jtb_mono_result; -1 otherwise */
 long        jtb_struct_size(int which);
 int         jtb_device_count(void);                 /* number of CUDA devices, <0 on error          */
 jtb_ctx*    jtb_create(const jtb_opts* opts);       /* NULL on failure (no CUDA device etc.)        */
@@ -281,6 +319,13 @@ int jtb_check_set_full(jtb_ctx* ctx, const jtb_history* h, int linearizable, jtb
 /* ---- hot path A8: bank SI checker, tests/ledger.clj:154-192 (after ledger->bank) -------------- */
 int jtb_check_bank_totals(jtb_ctx* ctx, const jtb_history* h, const jtb_model* accounts,
                           int64_t total_amount, jtb_bank_result* out);
+
+/* ---- monotonic-key check (see jtb_mono_shard above) ------------------------------------------------------------ *
+ * shards[n_shards] is caller-allocated.  Returns 0 on success, <0 on a malformed read payload (length not a multiple
+ * of 3, out of range, a key twice in one read), more than 2^31-1 reads, or when the device cannot hold the dense
+ * value matrix (jtb_last_error says which). */
+int jtb_check_monotonic_keys(jtb_ctx* ctx, const jtb_history* h, int32_t flags, jtb_mono_shard* shards,
+                             jtb_mono_result* out);
 
 /* ---- multi-GPU fan-out inside the library (SURVEY §8(b) `n_gpus`, §8(e)) ----------------------------------- *
  * What `independent/checker` (set_full.clj:155) does over JVM threads, done over the GPUs of one box for a host

@@ -74,4 +74,15 @@ public final class Native {
      */
     public static native long[] checkBankTotals(long ctx, Object[] history, int[] accounts, long totalAmount,
                                                 boolean negativeOk);
+
+    /**
+     * {@code jtb_check_monotonic_keys}: Elle's monotonic-key graph over the :ok reads, real-time edges unless
+     * {@code realtime} is false.  Read payloads are (key, valueLo, valueHi) triples, key = 2 * account + field
+     * (0 debits-posted, 1 credits-posted).
+     *
+     * @return {@code [valid, nFailures, nReads, kernelNs, totalNs, nShards]} followed by 14 longs per shard:
+     *     {@code valid, cause, nReads, nKeys, witnessIndex, partnerIndex}, then for the edges partner -> witness and
+     *     witness -> partner {@code kind, key, value, value'}
+     */
+    public static native long[] checkMonotonicKeys(long ctx, Object[] history, boolean realtime);
 }

@@ -5,15 +5,17 @@ import ctypes as C
 
 from .history import MAX_ACCOUNTS
 
-ABI_VERSION = 2
+ABI_VERSION = 3
 OPT_NO_EAGER_READS = 1
 OPT_NO_SCOUTS = 2
 OPT_ENGINE_LEVEL = 4
 OPT_ENGINE_WORKLIST = 8
 OPT_NO_BEAM = 16
 
-CAUSE_NONE, CAUSE_TABLE_FULL, CAUSE_BUDGET, CAUSE_TOO_WIDE = 0, 1, 2, 3
-CAUSE_NAME = {0: None, 1: "table-full", 2: "budget", 3: "too-wide"}
+CAUSE_NONE, CAUSE_TABLE_FULL, CAUSE_BUDGET, CAUSE_TOO_WIDE, CAUSE_PARTIAL_READ = 0, 1, 2, 3, 4
+CAUSE_NAME = {0: None, 1: "table-full", 2: "budget", 3: "too-wide", 4: "partial-read"}
+MONO_NO_REALTIME = 1
+MONO_EDGE_NONE, MONO_EDGE_MONOTONIC, MONO_EDGE_REALTIME = 0, 1, 2
 SF_NEVER_READ, SF_STABLE, SF_LOST = 0, 1, 2
 BANK_OK, BANK_UNEXPECTED_KEY, BANK_NIL_BALANCE, BANK_WRONG_TOTAL, BANK_NEGATIVE_VALUE = range(5)
 BANK_ERR_NAME = {1: "unexpected-key", 2: "nil-balance", 3: "wrong-total", 4: "negative-value"}
@@ -127,4 +129,31 @@ def setfull_to_dict(out, shards, bufs) -> dict:
         "suspect_final_reads": [
             {"shard": int(bufs["suspect_shard"][i]), "index": int(bufs["suspect_index"][i]),
              "missing": [int(x) for x in bufs["missing_ids"][int(moff[i]):int(moff[i + 1])]]} for i in range(ns)],
+    }
+
+
+class CMonoShard(C.Structure):
+    """jtb_mono_shard: the monotonic-key verdict of one shard."""
+    _fields_ = [("valid", C.c_int32), ("cause", C.c_int32), ("n_reads", C.c_int32), ("n_keys", C.c_int32),
+                ("witness_index", C.c_int32), ("partner_index", C.c_int32), ("edge_kind", C.c_int32 * 2),
+                ("edge_key", C.c_int32 * 2), ("edge_value", C.c_int64 * 2), ("edge_value2", C.c_int64 * 2)]
+
+
+class CMonoResult(C.Structure):
+    _fields_ = [("valid", C.c_int32), ("n_failures", C.c_int32), ("n_reads", C.c_int64),
+                ("seconds_kernel", C.c_double), ("seconds_total", C.c_double)]
+
+
+MONO_SHARD_FIELDS = ("valid", "cause", "n_reads", "n_keys", "witness_index", "partner_index")
+
+
+def mono_to_dict(res, shards) -> dict:
+    """One result dict for the library and the oracle: edges are [partner -> witness, witness -> partner], each
+    (kind, key, value, value')."""
+    return {
+        "valid": res.valid, "n_failures": res.n_failures, "n_reads": res.n_reads,
+        "seconds_kernel": res.seconds_kernel, "seconds_total": res.seconds_total,
+        "shards": [dict({f: getattr(s, f) for f in MONO_SHARD_FIELDS},
+                        edges=[(s.edge_kind[i], s.edge_key[i], s.edge_value[i], s.edge_value2[i]) for i in (0, 1)])
+                   for s in shards],
     }

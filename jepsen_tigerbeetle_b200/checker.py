@@ -24,7 +24,7 @@ import numpy as np
 
 from . import abi
 from .history import (INVALID, MODEL_BANK, MODEL_CAS_REGISTER, MODEL_REGISTER, MODEL_SET, UNKNOWN,
-                      VALID, VERDICT_NAME, FlatHistory, flatten_ops, make_model, merge_valid)
+                      VALID, VERDICT_NAME, COUNTER_FIELDS, FlatHistory, flatten_ops, make_model, merge_valid)
 from .native import Context
 
 _MODEL_KIND = {"register": MODEL_REGISTER, "cas-register": MODEL_CAS_REGISTER, "set": MODEL_SET,
@@ -262,6 +262,57 @@ class BankTotals(Checker, _Native):
         return out
 
 
+class MonotonicKeys(Checker, _Native):
+    """Elle's monotonic-key graph over a ledger history's :ok reads (src/tigerbeetle/elle/core.clj), on the GPU (K7).
+
+    Every account has two counters that only grow, debits-posted and credits-posted; a read that saw a smaller
+    counter than another read must come before it.  Together with real-time order (on by default) a cycle proves
+    that no (real-time respecting) serial order explains the reads.  Polynomial, unaffected by crashed transfers,
+    any number of accounts; weaker than `linearizable` (it does not replay transfers).  Result:
+    {valid?, read-count, key-count, [cause], [op, cycle, steps]}, keys spelled [account "debits-posted"]."""
+
+    def __init__(self, checker_opts: Mapping[str, Any] | None = None, ctx: Context | None = None,
+                 **ctx_opts) -> None:
+        _Native.__init__(self, ctx, **ctx_opts)
+        self.realtime = bool((checker_opts or {}).get("realtime?", True))
+
+    @staticmethod
+    def _key(k: int) -> list:
+        return [k >> 1, COUNTER_FIELDS[k & 1]]
+
+    def _shard_map(self, s: dict) -> dict:
+        m: dict[str, Any] = {"valid?": VERDICT_NAME[s["valid"]], "read-count": s["n_reads"], "key-count": s["n_keys"]}
+        if s["valid"] == UNKNOWN:
+            m["cause"] = abi.CAUSE_NAME.get(s["cause"], "unknown")
+        if s["valid"] == INVALID:
+            w, p = {"index": s["witness_index"]}, {"index": s["partner_index"]}
+            m["op"] = w
+            m["cycle"] = [p, w, p]
+            steps = []
+            for kind, key, v, v2 in s["edges"]:
+                if kind == abi.MONO_EDGE_MONOTONIC:
+                    steps.append({"type": "monotonic", "key": self._key(key), "value": v, "value'": v2})
+                else:   # real time: completion :index of the source, invocation :index of the target
+                    steps.append({"type": "realtime", "value": v, "value'": v2})
+            m["steps"] = steps
+        return m
+
+    def check_flat(self, test, h: FlatHistory) -> tuple[dict, list[dict]]:
+        r = self.ctx.check_monotonic_keys(h, realtime=self.realtime)
+        top = {"valid?": VERDICT_NAME[r["valid"]], "read-count": r["n_reads"],
+               "seconds-kernel": r["seconds_kernel"], "seconds-total": r["seconds_total"]}
+        return top, [self._shard_map(s) for s in r["shards"]]
+
+    def check(self, test, history, opts=None) -> dict:
+        h = _flat(history, "ledger-counters")
+        if h.n_shards != 1:
+            raise ValueError("history has independent keys: wrap with independent_checker(...)")
+        top, per = self.check_flat(test, h)
+        out = dict(per[0])
+        out.update({k: v for k, v in top.items() if k not in ("valid?", "read-count")})
+        return out
+
+
 class Compose(Checker):
     """`(checker/compose {name checker ...})`: run each, `:valid?` = merge-valid of the results."""
 
@@ -292,10 +343,12 @@ class Independent(Checker):
             c = next(iter(c.checkers.values()))
         if isinstance(c, Linearizable):
             return c.model
+        if isinstance(c, MonotonicKeys):
+            return "ledger-counters"
         return "set"
 
     def _per_key(self, checker: Checker, test, h: FlatHistory, opts) -> list[dict]:
-        if isinstance(checker, (Linearizable, SetFull, ReadAllInvokedAdds)):
+        if isinstance(checker, (Linearizable, SetFull, ReadAllInvokedAdds, MonotonicKeys)):
             try:
                 return checker.check_flat(test, h)[1]
             except Exception:  # noqa: BLE001
@@ -342,6 +395,12 @@ def read_all_invoked_adds(**kw) -> ReadAllInvokedAdds:
 def bank_checker(opts: Mapping[str, Any] | None = None, **kw) -> BankTotals:
     """`(ledger/checker {:negative-balances? true})` — tests/ledger.clj:154-192, :363"""
     return BankTotals(opts, **kw)
+
+
+def monotonic_key_checker(opts: Mapping[str, Any] | None = None, **kw) -> MonotonicKeys:
+    """Elle's monotonic-key check over the ledger counters; {"realtime?": False} gives the literal elle/core.clj
+    graph without real-time edges."""
+    return MonotonicKeys(opts, **kw)
 
 
 def compose(checkers: Mapping[str, Checker]) -> Compose:
@@ -510,13 +569,15 @@ def final_reads() -> FinalReads:
 
 
 def ledger_checker(checker_opts: Mapping[str, Any] | None = None, ctx: Context | None = None,
-                   linear: bool = True) -> Compose:
+                   linear: bool = True, monotonic: bool = False) -> Compose:
     """The ledger test's checker (tests/ledger.clj:363-367) minus the gnuplot plotter, plus the
-    linearizability search the north-star adds:
-        {:SI (checker opts) :lookup-transfers ... :final-reads ... :unexpected-ops ... [:linear ...]}"""
+    linearizability search the north-star adds and, with monotonic=True, the monotonic-key check:
+        {:SI (checker opts) :lookup-transfers ... :final-reads ... :unexpected-ops ... [:linear ...] [:monotonic ...]}"""
     cs: dict[str, Checker] = {"SI": bank_checker(checker_opts, ctx=ctx),
                               "lookup-transfers": lookup_all_invoked_transfers(),
                               "final-reads": final_reads(), "unexpected-ops": unexpected_ops()}
     if linear:
         cs["linear"] = linearizable({"model": "bank"}, ctx=ctx)
+    if monotonic:
+        cs["monotonic"] = monotonic_key_checker(ctx=ctx)
     return compose(cs)

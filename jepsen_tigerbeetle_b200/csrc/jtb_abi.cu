@@ -17,6 +17,7 @@
 #include "jtb_scans.cuh"
 #include "jtb_table_bench.cuh"
 #include "jtb_partition.cuh"
+#include "jtb_monotonic.cuh"
 
 using namespace jtb;
 
@@ -720,6 +721,8 @@ long jtb_struct_size(int which) {
     case 6: return sizeof(jtb_setfull_out);
     case 7: return sizeof(jtb_bank_result);
     case 8: return sizeof(jtb_final_config);
+    case 9: return sizeof(jtb_mono_shard);
+    case 10: return sizeof(jtb_mono_result);
     }
     return -1;
 }
@@ -1089,6 +1092,16 @@ int jtb_check_bank_totals(jtb_ctx* ctx, const jtb_history* h, const jtb_model* a
     if (cudaSetDevice(ctx->device) != cudaSuccess) { ctx->err = "cudaSetDevice failed"; return -1; }
     ctx->fc.valid = false;
     return run_bank_totals(ctx->stream, ctx->ev0, ctx->ev1, h, accounts, total_amount, out, ctx->err);
+}
+
+// K7: the monotonic-key check (csrc/jtb_monotonic.cuh)
+int jtb_check_monotonic_keys(jtb_ctx* ctx, const jtb_history* h, int32_t flags, jtb_mono_shard* shards,
+                             jtb_mono_result* out) {
+    if (!ctx) return -1;
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    if (cudaSetDevice(ctx->device) != cudaSuccess) { ctx->err = "cudaSetDevice failed"; return -1; }
+    ctx->fc.valid = false;
+    return run_monotonic_keys(ctx->stream, ctx->ev0, ctx->ev1, h, flags, shards, out, ctx->err);
 }
 
 // SURVEY 8(f) N2: the step before the checkers (independent/subhistory, ledger->bank) on the device

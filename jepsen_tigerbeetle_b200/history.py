@@ -267,7 +267,11 @@ def is_tuple(v: Any) -> bool:
 
 def flatten_ops(ops: Sequence[Mapping[str, Any]], model: str) -> FlatHistory:
     """Flatten a Jepsen history (sequence of op maps) for `model` in
-    {'register','cas-register','set','bank'}.
+    {'register','cas-register','set','bank','ledger-counters'}.
+
+    'ledger-counters' keeps what 'bank' folds into a balance: every account of a ledger :r read becomes two
+    (key, value_lo, value_hi) triples, key = 2*account + field (0 debits-posted, 1 credits-posted), the input of the
+    monotonic-key check.
 
     For 'bank', ledger-form :txn ops are first mapped by `ledger->bank` (tests/ledger.clj:89-114);
     stock jepsen.tests.bank {:from :to :amount} spelling is accepted too (SURVEY App. D).
@@ -352,6 +356,55 @@ def flatten_ops(ops: Sequence[Mapping[str, Any]], model: str) -> FlatHistory:
                         a=int(_get(value, "amount")), b=int(d), c=int(cr))
             else:
                 raise ValueError(f"unknown :f {f!r} for model bank")
+        elif model == "ledger-counters":
+            if f != "txn":
+                raise ValueError(f"unknown :f {f!r} for model ledger-counters")
+            tag = _kw(value[0][0])
+            if tag == "r":
+                bld.add(key, type_, F_READ, flags, process, index, time,
+                        payload=_counter_triples(value, index) if type_ == T_OK else None)
+            elif tag == "t":
+                (_t, _id, tv) = value[0]
+                bld.add(key, type_, F_TRANSFER, flags, process, index, time,
+                        a=int(_get(tv, "amount")), b=int(_get(tv, "debit-acct")),
+                        c=int(_get(tv, "credit-acct")))
+            elif tag == "l-t":
+                continue  # dropped, as ledger->bank drops it (tests/ledger.clj:110-111)
+            else:
+                raise ValueError(f"unknown txn micro-op {tag!r}")
         else:
             raise ValueError(f"unknown model {model!r}")
     return bld.build({"model": model})
+
+
+COUNTER_FIELDS = ("debits-posted", "credits-posted")   # field 0, field 1 of a ledger-counters key
+MAX_COUNTER_ACCOUNT = 1 << 30
+
+
+def counter_key(account: int, field: int) -> int:
+    """The monotonic-key check's key of an account's counter: 2 * account + field (0 debits, 1 credits)."""
+    return 2 * int(account) + int(field)
+
+
+def _counter_triples(value, index) -> list[int]:
+    """A ledger :r txn's accounts as (key, value_lo, value_hi) triples; an account with nil amounts (or a nil
+    counter) is left out, which makes the read partial."""
+    pl: list[int] = []
+    for (_r, acct, amounts) in value:
+        acct = int(acct)
+        if not 0 <= acct < MAX_COUNTER_ACCOUNT:
+            raise ValueError(f"op {index}: account {acct} is outside [0, 2^30)")
+        if amounts is None:
+            continue
+        for field, name in enumerate(COUNTER_FIELDS):
+            v = _get(amounts, name)
+            if v is None:
+                continue
+            v = int(v)
+            if not -(1 << 63) <= v < (1 << 63):
+                raise ValueError(f"op {index}: {name} {v} of account {acct} does not fit in int64")
+            u = v & 0xFFFFFFFFFFFFFFFF
+            lo, hi = u & 0xFFFFFFFF, u >> 32
+            pl.extend((counter_key(acct, field), lo - (1 << 32) if lo >= 1 << 31 else lo,
+                       hi - (1 << 32) if hi >= 1 << 31 else hi))
+    return pl

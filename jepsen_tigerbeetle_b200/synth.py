@@ -84,6 +84,21 @@ class SynthSpec:
 
 
 def generate(spec: SynthSpec) -> FlatHistory:
+    return _generate(spec)
+
+
+def generate_ledger_counters(spec: SynthSpec, fractured: bool = False) -> FlatHistory:
+    """The ledger-counter form of a bank `spec` (what flatten_ops(..., "ledger-counters") makes of a ledger history):
+    the same events as generate(spec), but every :ok read carries each account's debits-posted and credits-posted
+    as (key, value_lo, value_hi) triples, key = 2 * account + field, and credits - debits is the balance generate(spec)
+    reports.  `spec.stale_read` makes the same read stale as in generate(spec).  fractured=True instead takes ONE account
+    of one read from an older snapshot (a "fractured read"; the oracle decides the ground truth)."""
+    if spec.model != "bank":
+        raise ValueError("the ledger-counter form needs a bank spec")
+    return _generate(spec, counters=True, fracture=fractured)
+
+
+def _generate(spec: SynthSpec, counters: bool = False, fracture: bool = False) -> FlatHistory:
     rng = PCG32(spec.seed, 1)
     C, K = spec.n_clients, spec.n_keys
     model = spec.model
@@ -150,7 +165,12 @@ def generate(spec: SynthSpec) -> FlatHistory:
     results: list = [None] * len(ops)   # read values / cas success
     snapshots: list[list] = [[] for _ in range(K)]  # per key: state snapshots per lin step (for stale reads)
     lin_pos = [0] * len(ops)
-    want_snap = spec.stale_read
+    want_snap = spec.stale_read or fracture
+    # ledger-counter form: per key and account the two counters that only grow, per read their values
+    debits = [[0] * spec.n_accounts for _ in range(K)]
+    credits = [[0] * spec.n_accounts for _ in range(K)]
+    cresults: list = [None] * len(ops)
+    csnapshots: list[list] = [[] for _ in range(K)]
     for i in order:
         (_ti, _tr, _tl, _t, _p, key, f, a, b, c, fate) = ops[i]
         if want_snap:
@@ -159,6 +179,8 @@ def generate(spec: SynthSpec) -> FlatHistory:
                 snapshots[key].append(reg[key])
             elif model == "bank":
                 snapshots[key].append(tuple(bal[key]))
+                if counters:
+                    csnapshots[key].append((tuple(debits[key]), tuple(credits[key])))
             else:
                 snapshots[key].append(len(sets[key]))
         if fate == 2:
@@ -168,6 +190,8 @@ def generate(spec: SynthSpec) -> FlatHistory:
                 results[i] = reg[key]
             elif model == "bank":
                 results[i] = tuple(bal[key])
+                if counters:
+                    cresults[i] = (tuple(debits[key]), tuple(credits[key]))
             else:
                 results[i] = len(sets[key])  # prefix length of sets[key] in lin order
         elif f == F_WRITE:
@@ -183,6 +207,9 @@ def generate(spec: SynthSpec) -> FlatHistory:
         elif f == F_TRANSFER:
             bal[key][b - 1] -= a
             bal[key][c - 1] += a
+            if counters:
+                debits[key][b - 1] += a
+                credits[key][c - 1] += a
     # ---- stale-read mutation --------------------------------------------------------------------
     mutated = -1
     if spec.stale_read:
@@ -197,8 +224,25 @@ def generate(spec: SynthSpec) -> FlatHistory:
                 old = snapshots[key][p]
                 if old != results[i] and not (model == "set" and old >= results[i]):
                     results[i] = old
+                    if counters:
+                        cresults[i] = csnapshots[key][p]
                     mutated = i
                     break
+    fractured_at = -1
+    if fracture:
+        cand = [i for i in sorted(range(len(ops)), key=lambda i: ops[i][1])
+                if ops[i][6] == F_READ and ops[i][10] == 0 and ops[i][5] == 0]
+        back = spec.stale_by or 8 * per_key_threads
+        start = int(spec.stale_frac * len(cand))
+        for i in cand[start:] + cand[:start][::-1]:
+            old_d, old_c = csnapshots[ops[i][5]][max(0, lin_pos[i] - back)]
+            cur_d, cur_c = cresults[i]
+            changed = [j for j in range(spec.n_accounts) if (old_d[j], old_c[j]) != (cur_d[j], cur_c[j])]
+            if changed:
+                j = changed[0]
+                cresults[i] = (cur_d[:j] + (old_d[j],) + cur_d[j + 1:], cur_c[:j] + (old_c[j],) + cur_c[j + 1:])
+                fractured_at = i
+                break
     # ---- phase 3: events ------------------------------------------------------------------------
     ev = []  # (time, seq, op, is_completion)
     for i, o in enumerate(ops):
@@ -256,6 +300,15 @@ def generate(spec: SynthSpec) -> FlatHistory:
         elif f == F_READ:
             if model in ("register", "cas-register"):
                 a_arr[e] = results[i]
+            elif model == "bank" and counters:
+                d, cr = cresults[i]
+                pl = np.zeros((spec.n_accounts, 2, 3), np.int64)
+                pl[:, 0, 0] = 2 * acct_ids
+                pl[:, 1, 0] = 2 * acct_ids + 1
+                pl[:, 0, 1] = d
+                pl[:, 1, 1] = cr   # counters of synthetic histories stay far below 2^31: value_hi = 0
+                payload_chunks[e] = pl.reshape(-1).astype(np.int32)
+                plen[e] = 6 * spec.n_accounts
             elif model == "bank":
                 r = results[i]
                 pl = np.empty(2 * spec.n_accounts, np.int32)
@@ -281,8 +334,10 @@ def generate(spec: SynthSpec) -> FlatHistory:
         np.cumsum(lens[:-1], out=poff[1:])
     chunks = [payload_chunks[j] for j in perm]
     payload = np.concatenate(chunks).astype(np.int32) if chunks else empty
-    meta = {"model": model, "spec": spec, "mutated_op_index": mutated,
+    meta = {"model": "ledger-counters" if counters else model, "spec": spec, "mutated_op_index": mutated,
             "n_ops": len(all_ops), "accounts": list(range(1, spec.n_accounts + 1))}
+    if counters:
+        meta["fractured_op_index"] = fractured_at
     h = FlatHistory(typ[perm], f_arr[perm], flags[perm], proc_arr[perm], idx[perm], time_arr[perm],
                     a_arr[perm], b_arr[perm], c_arr[perm], poff, plen_p, payload, shard_off,
                     np.arange(1, K + 1, dtype=np.int64), meta)

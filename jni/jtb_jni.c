@@ -351,3 +351,42 @@ JNIEXPORT jlongArray JNICALL Java_jtb_Native_checkBankTotals(JNIEnv* env, jclass
     if (out) (*env)->SetLongArrayRegion(env, out, 0, k, v);
     return out;
 }
+
+/* ---- K7: monotonic-key check ------------------------------------------------------------------------------ */
+JNIEXPORT jlongArray JNICALL Java_jtb_Native_checkMonotonicKeys(JNIEnv* env, jclass cls, jlong handle, jobjectArray history,
+                                                                jboolean realtime) {
+    (void)cls;
+    jtb_history hist;
+    hist_pins pins;
+    if (pin_history(env, history, &hist, &pins)) return NULL;
+    const int ns = hist.n_shards;
+    jtb_mono_shard* shards = (jtb_mono_shard*)calloc(ns > 0 ? (size_t)ns : 1, sizeof *shards);
+    jtb_mono_result r;
+    memset(&r, 0, sizeof r);
+    const int rc = jtb_check_monotonic_keys((jtb_ctx*)(intptr_t)handle, &hist, realtime ? 0 : JTB_MONO_NO_REALTIME,
+                                            shards, &r);
+    unpin_history(env, &pins);
+    if (rc != 0) {
+        free(shards);
+        throw_rt(env, jtb_last_error((jtb_ctx*)(intptr_t)handle));
+        return NULL;
+    }
+    const int64_t total = 6 + 14ll * ns;
+    jlong* v = (jlong*)calloc((size_t)total, sizeof *v);
+    int64_t k = 0;
+    v[k++] = r.valid; v[k++] = r.n_failures; v[k++] = r.n_reads; v[k++] = ns_of(r.seconds_kernel);
+    v[k++] = ns_of(r.seconds_total); v[k++] = ns;
+    for (int s = 0; s < ns; ++s) {
+        const jtb_mono_shard* q = &shards[s];
+        v[k++] = q->valid; v[k++] = q->cause; v[k++] = q->n_reads; v[k++] = q->n_keys; v[k++] = q->witness_index;
+        v[k++] = q->partner_index;
+        for (int e = 0; e < 2; ++e) {
+            v[k++] = q->edge_kind[e]; v[k++] = q->edge_key[e]; v[k++] = q->edge_value[e]; v[k++] = q->edge_value2[e];
+        }
+    }
+    jlongArray out = (*env)->NewLongArray(env, (jsize)k);
+    if (out) (*env)->SetLongArrayRegion(env, out, 0, (jsize)k, v);
+    free(v);
+    free(shards);
+    return out;
+}

@@ -1,0 +1,56 @@
+"""ctypes binding of the monotonic-key CPU oracle (libjtb_mono_oracle.so).  TEST INFRASTRUCTURE ONLY.
+
+MONO_GRAPH builds Elle's monotonic-key graph literally (plus real-time edges) and runs Tarjan; MONO_PAIRS searches
+for 2-cycles by brute force.  See mono_oracle.cpp."""
+from __future__ import annotations
+
+import ctypes as C
+import os
+import subprocess
+import tempfile
+
+from jepsen_tigerbeetle_b200 import abi
+from jepsen_tigerbeetle_b200.history import FlatHistory, as_c_history
+
+MONO_GRAPH, MONO_PAIRS = 0, 1
+DECIDE_PARTIAL = 1 << 16   # decide shards with partial reads instead of reporting them UNKNOWN
+_HERE = os.path.dirname(os.path.abspath(__file__))
+_LIB = None
+
+
+def build(force: bool = False) -> str:
+    """The library in mono_oracle/, rebuilt when stale; when the directory is read-only a rebuild goes to a fresh
+    temporary directory instead."""
+    so = os.path.join(_HERE, "libjtb_mono_oracle.so")
+    srcs = [os.path.join(_HERE, f) for f in ("mono_oracle.cpp", "Makefile")]
+    srcs.append(os.path.join(_HERE, "..", "include", "jtb_check.h"))
+    stale = not os.path.exists(so) or any(os.path.getmtime(s) > os.path.getmtime(so) for s in srcs)
+    if force or stale:
+        if not os.access(_HERE, os.W_OK):
+            so = os.path.join(tempfile.mkdtemp(prefix="jtb_mono_oracle_"), "libjtb_mono_oracle.so")
+            subprocess.check_call(["make", "-C", _HERE, "-B", "-s", f"LIB={so}"], stdout=subprocess.DEVNULL)
+            return so
+        subprocess.check_call(["make", "-C", _HERE, "-B", "-s"], stdout=subprocess.DEVNULL)
+    return so
+
+
+def lib() -> C.CDLL:
+    global _LIB
+    if _LIB is None:
+        _LIB = C.CDLL(build())
+        _LIB.jtbm_last_error.restype = C.c_char_p
+        _LIB.jtbm_check_monotonic_keys.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
+    return _LIB
+
+
+def check_monotonic_keys(h: FlatHistory, algo: int = MONO_GRAPH, realtime: bool = True,
+                         decide_partial: bool = False) -> dict:
+    """Twin of `jtb_check_monotonic_keys` (same result dict as `native.Context.check_monotonic_keys`)."""
+    ch = as_c_history(h)
+    shards = (abi.CMonoShard * max(1, h.n_shards))()
+    res = abi.CMonoResult()
+    flags = (0 if realtime else abi.MONO_NO_REALTIME) | (DECIDE_PARTIAL if decide_partial else 0)
+    rc = lib().jtbm_check_monotonic_keys(C.addressof(ch), flags, algo, C.addressof(shards), C.addressof(res))
+    if rc != 0:
+        raise RuntimeError(lib().jtbm_last_error().decode())
+    return abi.mono_to_dict(res, shards[:h.n_shards])
