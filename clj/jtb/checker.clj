@@ -341,6 +341,39 @@
                               :cycle [(by-index (at (+ s 5))) (by-index (at (+ s 4))) (by-index (at (+ s 5)))]
                               :steps [(step (+ s 6)) (step (+ s 10))]))))))
 
+;; ---- counter bounds -------------------------------------------------------------------------------------------
+(def ^:private cb-error-type {1 :below-completed-transfers 2 :above-invoked-transfers})
+
+(defn counter-bounds-checker
+  "Every counter an :ok ledger read observes against the transfers around it, on the GPU: at least the :ok transfers
+  that completed before the read was invoked, at most the non-:fail transfers invoked before it completed.  Below is a
+  lost transfer, above a phantom or duplicated one.  Add it to the compose map at tests/ledger.clj:363-367 as
+  `:counter-bounds (counter-bounds-checker {})`.  Transfer txns with more than one [:t ...] micro-op throw (only the
+  first is flattened, so the upper bounds would be too small), which check-safe reports as :unknown.
+  Result: {:valid? :read-count :transfer-count :error-count [:op :error]}."
+  [_opts]
+  (reify checker/Checker
+    (check [_ _test history _opts]
+      (let [multi (count (filter (fn [{:keys [f type value]}]
+                                   (and (= :txn f) (= :invoke type) (= :t (ffirst value)) (< 1 (count value))))
+                                 history))
+            _     (when (pos? multi)
+                    (throw (IllegalArgumentException.
+                             (str multi " transfer txns have more than one [:t ...] micro-op"))))
+            {:keys [arrays by-index]} (flatten-history :ledger-counters history)
+            res   (Native/checkCounterBounds @ctx arrays)
+            at    (fn [i] (aget res (int i)))
+            s     8                                      ; shard 0: valid reads transfers keys below above witness ...
+            key   (at (+ s 7))]
+        (cond-> {:valid? (verdict (at s)) :read-count (at (+ s 1)) :transfer-count (at (+ s 2))
+                 :error-count (+ (at (+ s 4)) (at (+ s 5)))}
+          (= 2 (at s)) (assoc :op    (by-index (at (+ s 6)))
+                              :error {:type     (cb-error-type (at (+ s 8)))
+                                      :key      [(quot key 2) (counter-field (rem key 2))]
+                                      :value    (at (+ s 10))
+                                      :bound    (at (+ s 11))
+                                      :transfer (when (<= 0 (at (+ s 9))) (by-index (at (+ s 9))))}))))))
+
 ;; ---- independent ----------------------------------------------------------------------------------------------
 (defn independent-checker
   "Like (independent/checker (checker/compose checkers)) for a map {name checker-kind} built from THIS namespace's

@@ -24,7 +24,7 @@
 extern "C" {
 #endif
 
-#define JTB_ABI_VERSION 3
+#define JTB_ABI_VERSION 4
 
 /* ---- verdict lattice (jepsen.checker/merge-valid) ------------------------------------------- */
 #define JTB_VALID   0
@@ -271,13 +271,54 @@ typedef struct jtb_mono_result {
     double  seconds_total;      /* host wall time of the call incl. the host pass, H2D, D2H                        */
 } jtb_mono_result;
 
+/* ---- counter-bounds check (DESIGN.md "K8 counter-bounds check") ------------------------------------------------------
+ * The same reads as the monotonic-key check (:ok, f == JTB_F_READ, (key, value_lo, value_hi) triples, key =
+ * 2*account + field).  A transfer is an invoke with f == JTB_F_TRANSFER, a = amount, b = debit account, c = credit
+ * account; its fate is the next event of its process (:ok, :info, :fail, or none).  It adds `a` to key 2b+0
+ * (debits-posted) and to key 2c+1 (credits-posted); :fail transfers add nothing.  Positions are event positions in the
+ * shard.  Counters start at zero and only grow, so under strict serializability every key k an :ok read r observes
+ * satisfies L_k(r) <= v_k(r) <= U_k(r):
+ *   L = the amounts of the :ok transfers on k that completed before r was invoked (0 when r has no invocation)
+ *   U = the amounts of the non-:fail transfers on k invoked before r completed
+ * A shard with some (read, key) outside [L, U] is JTB_INVALID, every other shard JTB_VALID. */
+#define JTB_CB_BELOW 1 /* v < L: a completed :ok transfer is missing from the read (value = v, bound = L)               */
+#define JTB_CB_ABOVE 2 /* v > U: the read holds more than every transfer invoked before it completed (bound = U)        */
+
+typedef struct jtb_cb_shard {
+    int32_t valid;              /* JTB_VALID / JTB_INVALID                                                            */
+    int32_t n_reads;            /* :ok reads of the shard                                                             */
+    int32_t n_transfers;        /* transfers of the shard whose fate is not :fail                                     */
+    int32_t n_keys;             /* distinct keys the shard's :ok reads observe                                        */
+    int64_t n_below;            /* (read, key) pairs with v < L                                                       */
+    int64_t n_above;            /* (read, key) pairs with v > U                                                       */
+    int32_t witness_index;      /* :index of the earliest-completing :ok read with a key out of bounds, -1            */
+    int32_t witness_key;        /* its smallest such key, -1                                                          */
+    int32_t kind;               /* JTB_CB_BELOW / JTB_CB_ABOVE, 0 when VALID                                          */
+    int32_t culprit_index;      /* BELOW: completion :index of the first transfer, in completion order, at which the
+                                   running sum of L's amounts exceeds value; ABOVE: invocation :index of the last
+                                   transfer counted in U (-1 when none)                                                */
+    int64_t value;              /* the witness read's value of witness_key                                            */
+    int64_t bound;              /* the bound it violates (L for BELOW, U for ABOVE)                                   */
+} jtb_cb_shard;
+
+typedef struct jtb_cb_result {
+    int32_t valid;              /* merge-valid over shards                                                            */
+    int32_t n_failures;         /* INVALID shards                                                                     */
+    int64_t n_reads;            /* :ok reads over all shards                                                          */
+    int64_t n_transfers;        /* non-:fail transfers over all shards                                                */
+    int64_t n_violations;       /* out-of-bounds (read, key) pairs over all shards                                    */
+    double  seconds_kernel;     /* device time (CUDA events)                                                          */
+    double  seconds_total;      /* host wall time of the call incl. the host pass, H2D, D2H                           */
+} jtb_cb_result;
+
 typedef struct jtb_ctx jtb_ctx;
 
 /* ---- lifecycle -------------------------------------------------------------------------------- */
 int         jtb_abi_version(void);
 /* sizeof of the ABI structs as this library was compiled, for binding self-checks:
  * 0 jtb_history, 1 jtb_model, 2 jtb_opts, 3 jtb_lin_shard, 4 jtb_lin_result, 5 jtb_setfull_shard,
- * 6 jtb_setfull_out, 7 jtb_bank_result, 8 jtb_final_config, 9 jtb_mono_shard, 10 jtb_mono_result; -1 otherwise */
+ * 6 jtb_setfull_out, 7 jtb_bank_result, 8 jtb_final_config, 9 jtb_mono_shard, 10 jtb_mono_result, 11 jtb_cb_shard,
+ * 12 jtb_cb_result; -1 otherwise */
 long        jtb_struct_size(int which);
 int         jtb_device_count(void);                 /* number of CUDA devices, <0 on error          */
 jtb_ctx*    jtb_create(const jtb_opts* opts);       /* NULL on failure (no CUDA device etc.)        */
@@ -326,6 +367,14 @@ int jtb_check_bank_totals(jtb_ctx* ctx, const jtb_history* h, const jtb_model* a
  * value matrix (jtb_last_error says which). */
 int jtb_check_monotonic_keys(jtb_ctx* ctx, const jtb_history* h, int32_t flags, jtb_mono_shard* shards,
                              jtb_mono_result* out);
+
+/* ---- counter-bounds check (see jtb_cb_shard above) -------------------------------------------------------------- *
+ * shards[n_shards] is caller-allocated; flags is reserved and must be 0.  Returns 0 on success, <0 on a malformed read
+ * payload (as jtb_check_monotonic_keys), a transfer with a negative amount or an account outside [0, 2^30), more than
+ * 2^31-1 reads or (transfer, observed key) contributions, flags != 0, or a device allocation failure (jtb_last_error
+ * says which; the context stays usable). */
+int jtb_check_counter_bounds(jtb_ctx* ctx, const jtb_history* h, int32_t flags, jtb_cb_shard* shards,
+                             jtb_cb_result* out);
 
 /* ---- multi-GPU fan-out inside the library (SURVEY §8(b) `n_gpus`, §8(e)) ----------------------------------- *
  * What `independent/checker` (set_full.clj:155) does over JVM threads, done over the GPUs of one box for a host

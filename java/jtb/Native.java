@@ -85,4 +85,15 @@ public final class Native {
      *     witness -> partner {@code kind, key, value, value'}
      */
     public static native long[] checkMonotonicKeys(long ctx, Object[] history, boolean realtime);
+
+    /**
+     * {@code jtb_check_counter_bounds}: every counter an :ok read observes against L (the :ok transfers completed
+     * before the read was invoked) and U (the non-:fail transfers invoked before it completed).  Input as for
+     * {@link #checkMonotonicKeys}; transfers carry amount, debit account and credit account in a, b, c.
+     *
+     * @return {@code [valid, nFailures, nReads, nTransfers, nViolations, kernelNs, totalNs, nShards]} followed by 12
+     *     longs per shard: {@code valid, nReads, nTransfers, nKeys, nBelow, nAbove, witnessIndex, witnessKey, kind,
+     *     culpritIndex, value, bound}
+     */
+    public static native long[] checkCounterBounds(long ctx, Object[] history);
 }

@@ -5,7 +5,7 @@ import ctypes as C
 
 from .history import MAX_ACCOUNTS
 
-ABI_VERSION = 3
+ABI_VERSION = 4
 OPT_NO_EAGER_READS = 1
 OPT_NO_SCOUTS = 2
 OPT_ENGINE_LEVEL = 4
@@ -16,6 +16,7 @@ CAUSE_NONE, CAUSE_TABLE_FULL, CAUSE_BUDGET, CAUSE_TOO_WIDE, CAUSE_PARTIAL_READ =
 CAUSE_NAME = {0: None, 1: "table-full", 2: "budget", 3: "too-wide", 4: "partial-read"}
 MONO_NO_REALTIME = 1
 MONO_EDGE_NONE, MONO_EDGE_MONOTONIC, MONO_EDGE_REALTIME = 0, 1, 2
+CB_BELOW, CB_ABOVE = 1, 2
 SF_NEVER_READ, SF_STABLE, SF_LOST = 0, 1, 2
 BANK_OK, BANK_UNEXPECTED_KEY, BANK_NIL_BALANCE, BANK_WRONG_TOTAL, BANK_NEGATIVE_VALUE = range(5)
 BANK_ERR_NAME = {1: "unexpected-key", 2: "nil-balance", 3: "wrong-total", 4: "negative-value"}
@@ -156,4 +157,30 @@ def mono_to_dict(res, shards) -> dict:
         "shards": [dict({f: getattr(s, f) for f in MONO_SHARD_FIELDS},
                         edges=[(s.edge_kind[i], s.edge_key[i], s.edge_value[i], s.edge_value2[i]) for i in (0, 1)])
                    for s in shards],
+    }
+
+
+class CCbShard(C.Structure):
+    """jtb_cb_shard: the counter-bounds verdict of one shard."""
+    _fields_ = [("valid", C.c_int32), ("n_reads", C.c_int32), ("n_transfers", C.c_int32), ("n_keys", C.c_int32),
+                ("n_below", C.c_int64), ("n_above", C.c_int64), ("witness_index", C.c_int32),
+                ("witness_key", C.c_int32), ("kind", C.c_int32), ("culprit_index", C.c_int32),
+                ("value", C.c_int64), ("bound", C.c_int64)]
+
+
+class CCbResult(C.Structure):
+    _fields_ = [("valid", C.c_int32), ("n_failures", C.c_int32), ("n_reads", C.c_int64), ("n_transfers", C.c_int64),
+                ("n_violations", C.c_int64), ("seconds_kernel", C.c_double), ("seconds_total", C.c_double)]
+
+
+CB_SHARD_FIELDS = ("valid", "n_reads", "n_transfers", "n_keys", "n_below", "n_above", "witness_index", "witness_key",
+                   "kind", "culprit_index", "value", "bound")
+
+
+def cb_to_dict(res, shards) -> dict:
+    """One result dict for the library and the oracle."""
+    return {
+        "valid": res.valid, "n_failures": res.n_failures, "n_reads": res.n_reads, "n_transfers": res.n_transfers,
+        "n_violations": res.n_violations, "seconds_kernel": res.seconds_kernel, "seconds_total": res.seconds_total,
+        "shards": [{f: getattr(s, f) for f in CB_SHARD_FIELDS} for s in shards],
     }

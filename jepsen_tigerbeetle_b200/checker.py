@@ -313,6 +313,52 @@ class MonotonicKeys(Checker, _Native):
         return out
 
 
+class CounterBounds(Checker, _Native):
+    """Every counter a ledger :ok read observes held to the transfers around it, on the GPU (K8).
+
+    debits-posted and credits-posted start at zero and only grow, so a read must hold every :ok transfer that completed
+    before it was invoked (L) and nothing beyond the non-:fail transfers invoked before it completed (U).  A value below
+    L is a lost transfer, above U a phantom or duplicated one.  Polynomial, any number of accounts, :info transfers only
+    widen U; sound but not complete (which concurrent transfers a read saw is not decided).  Result: {valid?, read-count,
+    transfer-count, error-count, [op, error]}, keys spelled [account "debits-posted"]."""
+
+    ERROR_TYPE = {abi.CB_BELOW: "below-completed-transfers", abi.CB_ABOVE: "above-invoked-transfers"}
+
+    def __init__(self, checker_opts: Mapping[str, Any] | None = None, ctx: Context | None = None,
+                 **ctx_opts) -> None:
+        _Native.__init__(self, ctx, **ctx_opts)
+
+    def _shard_map(self, s: dict) -> dict:
+        m: dict[str, Any] = {"valid?": VERDICT_NAME[s["valid"]], "read-count": s["n_reads"],
+                             "transfer-count": s["n_transfers"], "error-count": s["n_below"] + s["n_above"]}
+        if s["valid"] == INVALID:
+            m["op"] = {"index": s["witness_index"]}
+            k = s["witness_key"]
+            m["error"] = {"type": self.ERROR_TYPE[s["kind"]], "key": [k >> 1, COUNTER_FIELDS[k & 1]],
+                          "value": s["value"], "bound": s["bound"], "transfer": {"index": s["culprit_index"]}}
+        return m
+
+    def check_flat(self, test, h: FlatHistory) -> tuple[dict, list[dict]]:
+        n = h.meta.get("multi_transfer_txns", 0)
+        if n:
+            raise ValueError(f"{n} transfer txns have more than one [:t ...] micro-op; only the first is flattened, so "
+                             "the transfers' upper bounds would be too small")
+        r = self.ctx.check_counter_bounds(h)
+        top = {"valid?": VERDICT_NAME[r["valid"]], "read-count": r["n_reads"], "transfer-count": r["n_transfers"],
+               "error-count": r["n_violations"], "seconds-kernel": r["seconds_kernel"],
+               "seconds-total": r["seconds_total"]}
+        return top, [self._shard_map(s) for s in r["shards"]]
+
+    def check(self, test, history, opts=None) -> dict:
+        h = _flat(history, "ledger-counters")
+        if h.n_shards != 1:
+            raise ValueError("history has independent keys: wrap with independent_checker(...)")
+        top, per = self.check_flat(test, h)
+        out = dict(per[0])
+        out.update({k: v for k, v in top.items() if k.startswith("seconds-")})
+        return out
+
+
 class Compose(Checker):
     """`(checker/compose {name checker ...})`: run each, `:valid?` = merge-valid of the results."""
 
@@ -343,12 +389,12 @@ class Independent(Checker):
             c = next(iter(c.checkers.values()))
         if isinstance(c, Linearizable):
             return c.model
-        if isinstance(c, MonotonicKeys):
+        if isinstance(c, (MonotonicKeys, CounterBounds)):
             return "ledger-counters"
         return "set"
 
     def _per_key(self, checker: Checker, test, h: FlatHistory, opts) -> list[dict]:
-        if isinstance(checker, (Linearizable, SetFull, ReadAllInvokedAdds, MonotonicKeys)):
+        if isinstance(checker, (Linearizable, SetFull, ReadAllInvokedAdds, MonotonicKeys, CounterBounds)):
             try:
                 return checker.check_flat(test, h)[1]
             except Exception:  # noqa: BLE001
@@ -401,6 +447,11 @@ def monotonic_key_checker(opts: Mapping[str, Any] | None = None, **kw) -> Monoto
     """Elle's monotonic-key check over the ledger counters; {"realtime?": False} gives the literal elle/core.clj
     graph without real-time edges."""
     return MonotonicKeys(opts, **kw)
+
+
+def counter_bounds_checker(opts: Mapping[str, Any] | None = None, **kw) -> CounterBounds:
+    """Every ledger read's counters against the bounds the :ok and :info transfers around it put on them (K8)."""
+    return CounterBounds(opts, **kw)
 
 
 def compose(checkers: Mapping[str, Checker]) -> Compose:
@@ -569,10 +620,12 @@ def final_reads() -> FinalReads:
 
 
 def ledger_checker(checker_opts: Mapping[str, Any] | None = None, ctx: Context | None = None,
-                   linear: bool = True, monotonic: bool = False) -> Compose:
+                   linear: bool = True, monotonic: bool = False, counter_bounds: bool = False) -> Compose:
     """The ledger test's checker (tests/ledger.clj:363-367) minus the gnuplot plotter, plus the
-    linearizability search the north-star adds and, with monotonic=True, the monotonic-key check:
-        {:SI (checker opts) :lookup-transfers ... :final-reads ... :unexpected-ops ... [:linear ...] [:monotonic ...]}"""
+    linearizability search the north-star adds and, with monotonic=True, the monotonic-key check and, with
+    counter_bounds=True, the counter-bounds check:
+        {:SI (checker opts) :lookup-transfers ... :final-reads ... :unexpected-ops ... [:linear ...] [:monotonic ...]
+         [:counter-bounds ...]}"""
     cs: dict[str, Checker] = {"SI": bank_checker(checker_opts, ctx=ctx),
                               "lookup-transfers": lookup_all_invoked_transfers(),
                               "final-reads": final_reads(), "unexpected-ops": unexpected_ops()}
@@ -580,4 +633,6 @@ def ledger_checker(checker_opts: Mapping[str, Any] | None = None, ctx: Context |
         cs["linear"] = linearizable({"model": "bank"}, ctx=ctx)
     if monotonic:
         cs["monotonic"] = monotonic_key_checker(ctx=ctx)
+    if counter_bounds:
+        cs["counter-bounds"] = counter_bounds_checker(ctx=ctx)
     return compose(cs)

@@ -18,6 +18,7 @@
 #include "jtb_table_bench.cuh"
 #include "jtb_partition.cuh"
 #include "jtb_monotonic.cuh"
+#include "jtb_counter_bounds.cuh"
 
 using namespace jtb;
 
@@ -723,6 +724,8 @@ long jtb_struct_size(int which) {
     case 8: return sizeof(jtb_final_config);
     case 9: return sizeof(jtb_mono_shard);
     case 10: return sizeof(jtb_mono_result);
+    case 11: return sizeof(jtb_cb_shard);
+    case 12: return sizeof(jtb_cb_result);
     }
     return -1;
 }
@@ -1102,6 +1105,16 @@ int jtb_check_monotonic_keys(jtb_ctx* ctx, const jtb_history* h, int32_t flags, 
     if (cudaSetDevice(ctx->device) != cudaSuccess) { ctx->err = "cudaSetDevice failed"; return -1; }
     ctx->fc.valid = false;
     return run_monotonic_keys(ctx->stream, ctx->ev0, ctx->ev1, h, flags, shards, out, ctx->err);
+}
+
+// K8: the counter-bounds check (csrc/jtb_counter_bounds.cuh)
+int jtb_check_counter_bounds(jtb_ctx* ctx, const jtb_history* h, int32_t flags, jtb_cb_shard* shards,
+                             jtb_cb_result* out) {
+    if (!ctx) return -1;
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    if (cudaSetDevice(ctx->device) != cudaSuccess) { ctx->err = "cudaSetDevice failed"; return -1; }
+    ctx->fc.valid = false;
+    return run_counter_bounds(ctx->stream, ctx->ev0, ctx->ev1, h, flags, shards, out, ctx->err);
 }
 
 // SURVEY 8(f) N2: the step before the checkers (independent/subhistory, ledger->bank) on the device

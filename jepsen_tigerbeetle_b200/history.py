@@ -271,13 +271,16 @@ def flatten_ops(ops: Sequence[Mapping[str, Any]], model: str) -> FlatHistory:
 
     'ledger-counters' keeps what 'bank' folds into a balance: every account of a ledger :r read becomes two
     (key, value_lo, value_hi) triples, key = 2*account + field (0 debits-posted, 1 credits-posted), the input of the
-    monotonic-key check.
+    monotonic-key and counter-bounds checks.  Like ledger->bank it keeps only the first [:t ...] of a transfer txn;
+    meta["multi_transfer_txns"] counts the transfer txns (at their invocation) that had more than one micro-op, since
+    the counter-bounds check would miss the others' amounts.
 
     For 'bank', ledger-form :txn ops are first mapped by `ledger->bank` (tests/ledger.clj:89-114);
     stock jepsen.tests.bank {:from :to :amount} spelling is accepted too (SURVEY App. D).
     """
     model = _kw(model)
     bld = _Builder()
+    multi_transfer = 0
     for pos, op in enumerate(ops):
         type_ = TYPE_CODE[_kw(_get(op, "type"))]
         process = _get(op, "process")
@@ -365,6 +368,7 @@ def flatten_ops(ops: Sequence[Mapping[str, Any]], model: str) -> FlatHistory:
                         payload=_counter_triples(value, index) if type_ == T_OK else None)
             elif tag == "t":
                 (_t, _id, tv) = value[0]
+                multi_transfer += type_ == T_INVOKE and len(value) > 1
                 bld.add(key, type_, F_TRANSFER, flags, process, index, time,
                         a=int(_get(tv, "amount")), b=int(_get(tv, "debit-acct")),
                         c=int(_get(tv, "credit-acct")))
@@ -374,6 +378,8 @@ def flatten_ops(ops: Sequence[Mapping[str, Any]], model: str) -> FlatHistory:
                 raise ValueError(f"unknown txn micro-op {tag!r}")
         else:
             raise ValueError(f"unknown model {model!r}")
+    if model == "ledger-counters":
+        return bld.build({"model": model, "multi_transfer_txns": int(multi_transfer)})
     return bld.build({"model": model})
 
 

@@ -87,18 +87,27 @@ def generate(spec: SynthSpec) -> FlatHistory:
     return _generate(spec)
 
 
-def generate_ledger_counters(spec: SynthSpec, fractured: bool = False) -> FlatHistory:
+def generate_ledger_counters(spec: SynthSpec, fractured: bool = False, lost_transfer: bool = False,
+                             duplicated_transfer: bool = False) -> FlatHistory:
     """The ledger-counter form of a bank `spec` (what flatten_ops(..., "ledger-counters") makes of a ledger history):
     the same events as generate(spec), but every :ok read carries each account's debits-posted and credits-posted
     as (key, value_lo, value_hi) triples, key = 2 * account + field, and credits - debits is the balance generate(spec)
     reports.  `spec.stale_read` makes the same read stale as in generate(spec).  fractured=True instead takes ONE account
-    of one read from an older snapshot (a "fractured read"; the oracle decides the ground truth)."""
+    of one read from an older snapshot (a "fractured read"; the oracle decides the ground truth).  `spec.final_reads`
+    adds one quiesced :final? read per key that returns the final counters.
+    lost_transfer=True never applies the counters of one :ok transfer; duplicated_transfer=True applies them twice.  The
+    transfer is the middle one, in linearization order, of the :ok transfers of key 0 (no extra random draws, so the
+    events and every other value equal the unmutated history); its op number is meta["lost_op_index"] /
+    meta["duplicated_op_index"]."""
     if spec.model != "bank":
         raise ValueError("the ledger-counter form needs a bank spec")
-    return _generate(spec, counters=True, fracture=fractured)
+    if lost_transfer and duplicated_transfer:
+        raise ValueError("lost_transfer and duplicated_transfer are exclusive")
+    return _generate(spec, counters=True, fracture=fractured, lost=lost_transfer, duplicated=duplicated_transfer)
 
 
-def _generate(spec: SynthSpec, counters: bool = False, fracture: bool = False) -> FlatHistory:
+def _generate(spec: SynthSpec, counters: bool = False, fracture: bool = False, lost: bool = False,
+              duplicated: bool = False) -> FlatHistory:
     rng = PCG32(spec.seed, 1)
     C, K = spec.n_clients, spec.n_keys
     model = spec.model
@@ -171,6 +180,12 @@ def _generate(spec: SynthSpec, counters: bool = False, fracture: bool = False) -
     credits = [[0] * spec.n_accounts for _ in range(K)]
     cresults: list = [None] * len(ops)
     csnapshots: list[list] = [[] for _ in range(K)]
+    # the :ok transfer whose counters are applied 0 or 2 times (lost / duplicated), -1 = none
+    mutated_transfer = -1
+    if lost or duplicated:
+        cand = [i for i in order if ops[i][6] == F_TRANSFER and ops[i][10] == 0 and ops[i][5] == 0]
+        if cand:
+            mutated_transfer = cand[len(cand) // 2]
     for i in order:
         (_ti, _tr, _tl, _t, _p, key, f, a, b, c, fate) = ops[i]
         if want_snap:
@@ -208,8 +223,9 @@ def _generate(spec: SynthSpec, counters: bool = False, fracture: bool = False) -
             bal[key][b - 1] -= a
             bal[key][c - 1] += a
             if counters:
-                debits[key][b - 1] += a
-                credits[key][c - 1] += a
+                times = 1 if i != mutated_transfer else 0 if lost else 2
+                debits[key][b - 1] += times * a
+                credits[key][c - 1] += times * a
     # ---- stale-read mutation --------------------------------------------------------------------
     mutated = -1
     if spec.stale_read:
@@ -301,7 +317,7 @@ def _generate(spec: SynthSpec, counters: bool = False, fracture: bool = False) -
             if model in ("register", "cas-register"):
                 a_arr[e] = results[i]
             elif model == "bank" and counters:
-                d, cr = cresults[i]
+                d, cr = (tuple(debits[o[5]]), tuple(credits[o[5]])) if is_final else cresults[i]
                 pl = np.zeros((spec.n_accounts, 2, 3), np.int64)
                 pl[:, 0, 0] = 2 * acct_ids
                 pl[:, 1, 0] = 2 * acct_ids + 1
@@ -338,6 +354,10 @@ def _generate(spec: SynthSpec, counters: bool = False, fracture: bool = False) -
             "n_ops": len(all_ops), "accounts": list(range(1, spec.n_accounts + 1))}
     if counters:
         meta["fractured_op_index"] = fractured_at
+        if lost:
+            meta["lost_op_index"] = mutated_transfer
+        if duplicated:
+            meta["duplicated_op_index"] = mutated_transfer
     h = FlatHistory(typ[perm], f_arr[perm], flags[perm], proc_arr[perm], idx[perm], time_arr[perm],
                     a_arr[perm], b_arr[perm], c_arr[perm], poff, plen_p, payload, shard_off,
                     np.arange(1, K + 1, dtype=np.int64), meta)

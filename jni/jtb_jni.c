@@ -390,3 +390,38 @@ JNIEXPORT jlongArray JNICALL Java_jtb_Native_checkMonotonicKeys(JNIEnv* env, jcl
     free(shards);
     return out;
 }
+
+/* ---- K8: counter-bounds check -------------------------------------------------------------------------------- */
+JNIEXPORT jlongArray JNICALL Java_jtb_Native_checkCounterBounds(JNIEnv* env, jclass cls, jlong handle, jobjectArray history) {
+    (void)cls;
+    jtb_history hist;
+    hist_pins pins;
+    if (pin_history(env, history, &hist, &pins)) return NULL;
+    const int ns = hist.n_shards;
+    jtb_cb_shard* shards = (jtb_cb_shard*)calloc(ns > 0 ? (size_t)ns : 1, sizeof *shards);
+    jtb_cb_result r;
+    memset(&r, 0, sizeof r);
+    const int rc = jtb_check_counter_bounds((jtb_ctx*)(intptr_t)handle, &hist, 0, shards, &r);
+    unpin_history(env, &pins);
+    if (rc != 0) {
+        free(shards);
+        throw_rt(env, jtb_last_error((jtb_ctx*)(intptr_t)handle));
+        return NULL;
+    }
+    const int64_t total = 8 + 12ll * ns;
+    jlong* v = (jlong*)calloc((size_t)total, sizeof *v);
+    int64_t k = 0;
+    v[k++] = r.valid; v[k++] = r.n_failures; v[k++] = r.n_reads; v[k++] = r.n_transfers; v[k++] = r.n_violations;
+    v[k++] = ns_of(r.seconds_kernel); v[k++] = ns_of(r.seconds_total); v[k++] = ns;
+    for (int s = 0; s < ns; ++s) {
+        const jtb_cb_shard* q = &shards[s];
+        v[k++] = q->valid; v[k++] = q->n_reads; v[k++] = q->n_transfers; v[k++] = q->n_keys; v[k++] = q->n_below;
+        v[k++] = q->n_above; v[k++] = q->witness_index; v[k++] = q->witness_key; v[k++] = q->kind;
+        v[k++] = q->culprit_index; v[k++] = q->value; v[k++] = q->bound;
+    }
+    jlongArray out = (*env)->NewLongArray(env, (jsize)k);
+    if (out) (*env)->SetLongArrayRegion(env, out, 0, (jsize)k, v);
+    free(v);
+    free(shards);
+    return out;
+}

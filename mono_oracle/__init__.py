@@ -1,7 +1,9 @@
-"""ctypes binding of the monotonic-key CPU oracle (libjtb_mono_oracle.so).  TEST INFRASTRUCTURE ONLY.
+"""ctypes binding of the monotonic-key and counter-bounds CPU oracles (libjtb_mono_oracle.so).  TEST INFRASTRUCTURE
+ONLY.
 
 MONO_GRAPH builds Elle's monotonic-key graph literally (plus real-time edges) and runs Tarjan; MONO_PAIRS searches
-for 2-cycles by brute force.  See mono_oracle.cpp."""
+for 2-cycles by brute force.  See mono_oracle.cpp.  CB_LITERAL sums every transfer for every (read, key); CB_SWEEP
+keeps running sums over one walk of the events.  See counter_bounds.cpp."""
 from __future__ import annotations
 
 import ctypes as C
@@ -13,6 +15,7 @@ from jepsen_tigerbeetle_b200 import abi
 from jepsen_tigerbeetle_b200.history import FlatHistory, as_c_history
 
 MONO_GRAPH, MONO_PAIRS = 0, 1
+CB_LITERAL, CB_SWEEP = 0, 1
 DECIDE_PARTIAL = 1 << 16   # decide shards with partial reads instead of reporting them UNKNOWN
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB = None
@@ -22,7 +25,7 @@ def build(force: bool = False) -> str:
     """The library in mono_oracle/, rebuilt when stale; when the directory is read-only a rebuild goes to a fresh
     temporary directory instead."""
     so = os.path.join(_HERE, "libjtb_mono_oracle.so")
-    srcs = [os.path.join(_HERE, f) for f in ("mono_oracle.cpp", "Makefile")]
+    srcs = [os.path.join(_HERE, f) for f in ("mono_oracle.cpp", "counter_bounds.cpp", "Makefile")]
     srcs.append(os.path.join(_HERE, "..", "include", "jtb_check.h"))
     stale = not os.path.exists(so) or any(os.path.getmtime(s) > os.path.getmtime(so) for s in srcs)
     if force or stale:
@@ -40,6 +43,8 @@ def lib() -> C.CDLL:
         _LIB = C.CDLL(build())
         _LIB.jtbm_last_error.restype = C.c_char_p
         _LIB.jtbm_check_monotonic_keys.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
+        _LIB.jtbm_cb_last_error.restype = C.c_char_p
+        _LIB.jtbm_check_counter_bounds.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
     return _LIB
 
 
@@ -54,3 +59,14 @@ def check_monotonic_keys(h: FlatHistory, algo: int = MONO_GRAPH, realtime: bool 
     if rc != 0:
         raise RuntimeError(lib().jtbm_last_error().decode())
     return abi.mono_to_dict(res, shards[:h.n_shards])
+
+
+def check_counter_bounds(h: FlatHistory, algo: int = CB_SWEEP, flags: int = 0) -> dict:
+    """Twin of `jtb_check_counter_bounds` (same result dict as `native.Context.check_counter_bounds`)."""
+    ch = as_c_history(h)
+    shards = (abi.CCbShard * max(1, h.n_shards))()
+    res = abi.CCbResult()
+    rc = lib().jtbm_check_counter_bounds(C.addressof(ch), flags, algo, C.addressof(shards), C.addressof(res))
+    if rc != 0:
+        raise RuntimeError(lib().jtbm_cb_last_error().decode())
+    return abi.cb_to_dict(res, shards[:h.n_shards])
