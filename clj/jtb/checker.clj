@@ -31,7 +31,7 @@
 
 ;; ---- codes (include/jtb_check.h) ---------------------------------------------------------------------------
 (def type-code  {:invoke 0 :ok 1 :fail 2 :info 3})
-(def f-code     {:read 0 :write 1 :cas 2 :add 3 :transfer 4})
+(def f-code     {:read 0 :write 1 :cas 2 :add 3 :transfer 4 :lookup 5})
 (def model-code {:register 0 :cas-register 1 :set 2 :bank 3})
 (def NIL Integer/MIN_VALUE)
 (def verdict    {0 true 1 :unknown 2 false})
@@ -75,6 +75,35 @@
       :l-t nil
       nil)))
 
+(defn- transfer-records
+  "[:t id {...}] / [:l-t id {...}] micro-ops -> [id-lo id-hi debit credit amount ...]; a lookup micro-op without a
+  transfer map (not found) is left out."
+  [value]
+  (vec (for [[_ id v] value
+             :when v
+             x [(unchecked-int (long id)) (unchecked-int (bit-shift-right (long id) 32))
+                (:debit-acct v) (:credit-acct v) (:amount v)]]
+         x)))
+
+(defn- ledger->lookups-ops
+  "The ledger-lookups form of the client ops: ledger->counters-op, plus the records of a transfer invoke's [:t ...]
+  micro-ops (all of them) in ::records, and every [:l-t ...] op as :f :lookup with its :ok records as :value.  An
+  :ok lookup with an empty value takes its tag from its process's pending invoke."
+  [ops]
+  (first
+    (reduce (fn [[out pending] {:keys [type value process f] :as op}]
+              (if (not= :txn f)
+                [(conj out op) pending]
+                (let [tag     (or (ffirst value) (get pending process))
+                      pending (if (= :invoke type) (assoc pending process tag) (dissoc pending process))
+                      o       (case tag
+                                :l-t (assoc op :f :lookup :value (when (= :ok type) (transfer-records value)))
+                                :t   (cond-> (ledger->counters-op op)
+                                       (= :invoke type) (assoc ::records (transfer-records value)))
+                                (ledger->counters-op op))]
+                  [(if o (conj out o) out) pending])))
+            [[] {}] ops)))
+
 (defn- int-or-nil [x] (if (nil? x) NIL (int x)))
 
 (defn flatten-history
@@ -83,11 +112,13 @@
   [nil nil] tuple (set_full.clj:112-116 with a rejected account creation) is skipped, like an element that was never
   tracked."
   [model history]
-  (let [ops   (->> history
-                   (filter (comp int? :process))
-                   (keep (fn [op] (if (= :txn (:f op))
-                                    ((if (= model :ledger-counters) ledger->counters-op ledger->bank-op) op)
-                                    op)))
+  (let [ops   (->> history (filter (comp int? :process)))
+        ops   (->> (if (= model :ledger-lookups)
+                     (ledger->lookups-ops ops)
+                     (keep (fn [op] (if (= :txn (:f op))
+                                      ((if (= model :ledger-counters) ledger->counters-op ledger->bank-op) op)
+                                      op))
+                           ops))
                    (keep (fn [op]
                            (let [v (:value op)]
                              (if (independent/tuple? v)
@@ -126,11 +157,14 @@
           [:set :read]  (put-payload! (when (and value (= :ok (:type o))) (sort value)))
           [:bank :read] (put-payload! (when (and value (= :ok (:type o)))
                                         (mapcat (fn [[id bal]] [id (int-or-nil bal)]) value)))
-          [:ledger-counters :read] (put-payload! (when (and value (= :ok (:type o))) (apply concat value)))
-          ([:bank :transfer] [:ledger-counters :transfer])
+          ([:ledger-counters :read] [:ledger-lookups :read])
+                            (put-payload! (when (and value (= :ok (:type o))) (apply concat value)))
+          ([:bank :transfer] [:ledger-counters :transfer] [:ledger-lookups :transfer])
                             (do (aset a i (int (:amount value)))
                                 (aset b i (int (or (:debit-acct value) (:from value))))
-                                (aset c i (int (or (:credit-acct value) (:to value)))))
+                                (aset c i (int (or (:credit-acct value) (:to value))))
+                                (put-payload! (::records o)))
+          [:ledger-lookups :lookup] (put-payload! value)
           nil)))                                    ; any other :f: opcode 0 with no value — ignored by every checker
     {:arrays   (object-array [type f flags proc index time a b c poff plen (int-array payload)
                               (long-array (reductions + 0 (map (comp count by-k) ks)))
@@ -373,6 +407,39 @@
                                       :value    (at (+ s 10))
                                       :bound    (at (+ s 11))
                                       :transfer (when (<= 0 (at (+ s 9))) (by-index (at (+ s 9))))}))))))
+
+;; ---- transfer lookups ---------------------------------------------------------------------------------------
+(def ^:private tl-kind {1 :phantom 2 :mismatch 3 :failed-visible 4 :future 5 :duplicate 6 :lost 7 :vanished
+                        8 :read-below-lookup 9 :read-above-lookup})
+
+(defn transfer-lookup-checker
+  "The transfer records :ok [:l-t ...] lookups return, on the GPU, against the transfers clients issued (phantom,
+  mismatched, failed, future and duplicate records), against each other and the :ok transfers (a transfer seen once
+  must stay visible: lost, vanished), and against the counters reads show (read below / above a lookup's sums).
+  :info transfers are never required to appear.  Add it to the compose map at tests/ledger.clj:363-367 as
+  `:transfer-lookups (transfer-lookup-checker {})`.
+  Result: {:valid? :lookup-count :record-count :transfer-count :read-count :error-count :errors [:op :error]}."
+  [_opts]
+  (reify checker/Checker
+    (check [_ _test history _opts]
+      (let [{:keys [arrays by-index]} (flatten-history :ledger-lookups history)
+            res    (Native/checkTransferLookups @ctx arrays)
+            at     (fn [i] (aget res (int i)))
+            s      10                                     ; shard 0: valid lookups records transfers reads counts[9] ...
+            errors (into {} (for [k (range 9) :let [n (at (+ s 5 k))] :when (pos? n)] [(tl-kind (inc k)) n]))
+            kind   (at (+ s 15))
+            key    (at (+ s 17))
+            rel    (at (+ s 18))]
+        (cond-> {:valid? (verdict (at s)) :lookup-count (at (+ s 1)) :record-count (at (+ s 2))
+                 :transfer-count (at (+ s 3)) :read-count (at (+ s 4)) :error-count (reduce + (vals errors))
+                 :errors errors}
+          (= 2 (at s)) (assoc :op    (by-index (at (+ s 14)))
+                              :error (cond-> {:type (tl-kind kind)}
+                                       (< kind 8)  (assoc :transfer-id (at (+ s 16)))
+                                       (>= kind 8) (assoc :key   [(quot key 2) (counter-field (rem key 2))]
+                                                          :value (at (+ s 19))
+                                                          :bound (at (+ s 20)))
+                                       (<= 0 rel)  (assoc :related (by-index rel)))))))))
 
 ;; ---- independent ----------------------------------------------------------------------------------------------
 (defn independent-checker

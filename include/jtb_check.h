@@ -24,7 +24,7 @@
 extern "C" {
 #endif
 
-#define JTB_ABI_VERSION 4
+#define JTB_ABI_VERSION 5
 
 /* ---- verdict lattice (jepsen.checker/merge-valid) ------------------------------------------- */
 #define JTB_VALID   0
@@ -50,6 +50,8 @@ extern "C" {
 #define JTB_F_CAS      2
 #define JTB_F_ADD      3
 #define JTB_F_TRANSFER 4
+#define JTB_F_LOOKUP   5 /* ledger-lookups form only: a [:l-t ...] txn (tigerbeetle.clj:195-213); the :ok payload is the
+                            returned transfer records, 5 int32 each (id_lo, id_hi, debit, credit, amount) */
 
 #define JTB_NIL INT32_MIN /* Clojure nil in an int32 field (a nil register read matches any state) */
 
@@ -311,6 +313,66 @@ typedef struct jtb_cb_result {
     double  seconds_total;      /* host wall time of the call incl. the host pass, H2D, D2H                           */
 } jtb_cb_result;
 
+/* ---- transfer-lookup check (DESIGN.md "K9 transfer-lookup check") ----------------------------------------------------
+ * Input: the ledger-lookups form.  Reads are the monotonic-key check's.  A transfer invoke (f == JTB_F_TRANSFER) carries
+ * one 5-int32 record (id_lo, id_hi, debit, credit, amount) per [:t ...] micro-op; each is one transfer with the txn's
+ * interval and fate (the next event of its process).  A lookup is an :ok event with f == JTB_F_LOOKUP whose payload is
+ * the returned records in the same layout; its invocation is the latest invoke of its process.  Ids are int64
+ * (id_hi << 32 | id_lo).  With l an :ok lookup and t a transfer of the same shard, each of these proves an anomaly:
+ *   1 PHANTOM            a record whose id no transfer invoke of the shard carries
+ *   2 MISMATCH           a record whose (debit, credit, amount) differs from its invocation's
+ *   3 FAILED_VISIBLE     a record of a transfer whose fate is :fail
+ *   4 FUTURE             a record of a transfer invoked after l completed
+ *   5 DUPLICATE          an id twice in one lookup
+ *   6 LOST / 7 VANISHED  M(t) = min(t's :ok completion, the earliest completion of an :ok lookup returning t); every
+ *                        :ok lookup invoked after M(t) must contain t (LOST when M is the :ok completion)
+ *   8 READ_BELOW_LOOKUP  an :ok read's value of key k is below S_k(l) for a lookup l completed before it was invoked
+ *   9 READ_ABOVE_LOOKUP  ... above S_k(l) for a lookup l invoked after it completed
+ * S_k(l) = the sum over l's distinct ids (first record of each) of the record's amount on k (key 2*debit+0 and
+ * 2*credit+1); only keys the shard's :ok reads observe count. */
+#define JTB_TL_PHANTOM           1
+#define JTB_TL_MISMATCH          2
+#define JTB_TL_FAILED_VISIBLE    3
+#define JTB_TL_FUTURE            4
+#define JTB_TL_DUPLICATE         5
+#define JTB_TL_LOST              6
+#define JTB_TL_VANISHED          7
+#define JTB_TL_READ_BELOW_LOOKUP 8
+#define JTB_TL_READ_ABOVE_LOOKUP 9
+#define JTB_TL_KINDS             9
+
+typedef struct jtb_tl_shard {
+    int32_t valid;              /* JTB_VALID / JTB_INVALID                                                            */
+    int32_t n_lookups;          /* :ok lookups of the shard                                                           */
+    int64_t n_records;          /* records of those lookups                                                           */
+    int32_t n_transfers;        /* transfer micro-ops of the shard (every fate)                                       */
+    int32_t n_reads;            /* :ok reads of the shard                                                             */
+    int64_t count_by_kind[JTB_TL_KINDS]; /* [kind - 1]: records (1-4), repeated records (5), (lookup, missing
+                                   transfer) pairs (6-7), (read, key) pairs (8-9)                                     */
+    int32_t witness_index;      /* completion :index of the earliest-completing :ok lookup or read with a violation  */
+    int32_t kind;               /* the smallest code among its violations, 0 when VALID                               */
+    int64_t transfer_id;        /* lookup kinds: the smallest transfer id of that kind; read kinds: 0                 */
+    int32_t key;                /* read kinds: the smallest key of that kind; lookup kinds: -1                        */
+    int32_t related_index;      /* LOST: the transfer's completion :index; VANISHED: the earlier lookup's completion
+                                   :index; 2-4: the transfer's invocation :index; BELOW: completion :index of the
+                                   earliest-completing qualifying lookup with S > value; ABOVE: of the
+                                   earliest-invoked qualifying lookup with S < value; PHANTOM, DUPLICATE: -1          */
+    int64_t value;              /* read kinds: the read's value of key                                               */
+    int64_t bound;              /* read kinds: max S (BELOW) / min S (ABOVE) over the qualifying lookups             */
+} jtb_tl_shard;
+
+typedef struct jtb_tl_result {
+    int32_t valid;              /* merge-valid over shards                                                            */
+    int32_t n_failures;         /* INVALID shards                                                                     */
+    int64_t n_lookups;          /* :ok lookups over all shards                                                        */
+    int64_t n_records;          /* their records                                                                      */
+    int64_t n_transfers;        /* transfer micro-ops                                                                 */
+    int64_t n_reads;            /* :ok reads                                                                          */
+    int64_t n_violations;       /* sum of count_by_kind over shards and kinds                                         */
+    double  seconds_kernel;     /* device time (CUDA events)                                                          */
+    double  seconds_total;      /* host wall time of the call incl. the host pass, H2D, D2H                           */
+} jtb_tl_result;
+
 typedef struct jtb_ctx jtb_ctx;
 
 /* ---- lifecycle -------------------------------------------------------------------------------- */
@@ -318,7 +380,7 @@ int         jtb_abi_version(void);
 /* sizeof of the ABI structs as this library was compiled, for binding self-checks:
  * 0 jtb_history, 1 jtb_model, 2 jtb_opts, 3 jtb_lin_shard, 4 jtb_lin_result, 5 jtb_setfull_shard,
  * 6 jtb_setfull_out, 7 jtb_bank_result, 8 jtb_final_config, 9 jtb_mono_shard, 10 jtb_mono_result, 11 jtb_cb_shard,
- * 12 jtb_cb_result; -1 otherwise */
+ * 12 jtb_cb_result, 13 jtb_tl_shard, 14 jtb_tl_result; -1 otherwise */
 long        jtb_struct_size(int which);
 int         jtb_device_count(void);                 /* number of CUDA devices, <0 on error          */
 jtb_ctx*    jtb_create(const jtb_opts* opts);       /* NULL on failure (no CUDA device etc.)        */
@@ -375,6 +437,15 @@ int jtb_check_monotonic_keys(jtb_ctx* ctx, const jtb_history* h, int32_t flags, 
  * says which; the context stays usable). */
 int jtb_check_counter_bounds(jtb_ctx* ctx, const jtb_history* h, int32_t flags, jtb_cb_shard* shards,
                              jtb_cb_result* out);
+
+/* ---- transfer-lookup check (see jtb_tl_shard above) ------------------------------------------------------------- *
+ * shards[n_shards] is caller-allocated; flags is reserved and must be 0.  Returns 0 on success, <0 on a malformed read
+ * payload (as jtb_check_monotonic_keys), a transfer or lookup payload whose length is not a multiple of 5, a transfer
+ * invoke without ids, two transfer invokes of one shard carrying the same id, a negative amount or an account outside
+ * [0, 2^30) in a transfer invoke, more than 2^31-1 records or reads, an S matrix (lookups x observed keys) the device
+ * cannot hold, flags != 0, or a device allocation failure (jtb_last_error says which; the context stays usable). */
+int jtb_check_transfer_lookups(jtb_ctx* ctx, const jtb_history* h, int32_t flags, jtb_tl_shard* shards,
+                               jtb_tl_result* out);
 
 /* ---- multi-GPU fan-out inside the library (SURVEY §8(b) `n_gpus`, §8(e)) ----------------------------------- *
  * What `independent/checker` (set_full.clj:155) does over JVM threads, done over the GPUs of one box for a host

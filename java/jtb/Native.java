@@ -96,4 +96,15 @@ public final class Native {
      *     culpritIndex, value, bound}
      */
     public static native long[] checkCounterBounds(long ctx, Object[] history);
+
+    /**
+     * {@code jtb_check_transfer_lookups}: the transfer records :ok lookups return against the transfers clients issued
+     * and the counters reads show.  Input: the ledger-lookups form (transfer invokes and :ok lookups carry records of
+     * 5 ints: id lo, id hi, debit, credit, amount; lookups have f = 5).
+     *
+     * @return {@code [valid, nFailures, nLookups, nRecords, nTransfers, nReads, nViolations, kernelNs, totalNs,
+     *     nShards]} followed by 21 longs per shard: {@code valid, nLookups, nRecords, nTransfers, nReads}, the 9 counts
+     *     by kind, {@code witnessIndex, kind, transferId, key, relatedIndex, value, bound}
+     */
+    public static native long[] checkTransferLookups(long ctx, Object[] history);
 }

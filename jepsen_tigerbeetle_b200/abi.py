@@ -5,7 +5,7 @@ import ctypes as C
 
 from .history import MAX_ACCOUNTS
 
-ABI_VERSION = 4
+ABI_VERSION = 5
 OPT_NO_EAGER_READS = 1
 OPT_NO_SCOUTS = 2
 OPT_ENGINE_LEVEL = 4
@@ -17,6 +17,11 @@ CAUSE_NAME = {0: None, 1: "table-full", 2: "budget", 3: "too-wide", 4: "partial-
 MONO_NO_REALTIME = 1
 MONO_EDGE_NONE, MONO_EDGE_MONOTONIC, MONO_EDGE_REALTIME = 0, 1, 2
 CB_BELOW, CB_ABOVE = 1, 2
+(TL_PHANTOM, TL_MISMATCH, TL_FAILED_VISIBLE, TL_FUTURE, TL_DUPLICATE, TL_LOST, TL_VANISHED, TL_READ_BELOW_LOOKUP,
+ TL_READ_ABOVE_LOOKUP) = range(1, 10)
+TL_KINDS = 9
+TL_KIND_NAME = {1: "phantom", 2: "mismatch", 3: "failed-visible", 4: "future", 5: "duplicate", 6: "lost",
+                7: "vanished", 8: "read-below-lookup", 9: "read-above-lookup"}
 SF_NEVER_READ, SF_STABLE, SF_LOST = 0, 1, 2
 BANK_OK, BANK_UNEXPECTED_KEY, BANK_NIL_BALANCE, BANK_WRONG_TOTAL, BANK_NEGATIVE_VALUE = range(5)
 BANK_ERR_NAME = {1: "unexpected-key", 2: "nil-balance", 3: "wrong-total", 4: "negative-value"}
@@ -183,4 +188,33 @@ def cb_to_dict(res, shards) -> dict:
         "valid": res.valid, "n_failures": res.n_failures, "n_reads": res.n_reads, "n_transfers": res.n_transfers,
         "n_violations": res.n_violations, "seconds_kernel": res.seconds_kernel, "seconds_total": res.seconds_total,
         "shards": [{f: getattr(s, f) for f in CB_SHARD_FIELDS} for s in shards],
+    }
+
+
+class CTlShard(C.Structure):
+    """jtb_tl_shard: the transfer-lookup verdict of one shard."""
+    _fields_ = [("valid", C.c_int32), ("n_lookups", C.c_int32), ("n_records", C.c_int64), ("n_transfers", C.c_int32),
+                ("n_reads", C.c_int32), ("count_by_kind", C.c_int64 * TL_KINDS), ("witness_index", C.c_int32),
+                ("kind", C.c_int32), ("transfer_id", C.c_int64), ("key", C.c_int32), ("related_index", C.c_int32),
+                ("value", C.c_int64), ("bound", C.c_int64)]
+
+
+class CTlResult(C.Structure):
+    _fields_ = [("valid", C.c_int32), ("n_failures", C.c_int32), ("n_lookups", C.c_int64), ("n_records", C.c_int64),
+                ("n_transfers", C.c_int64), ("n_reads", C.c_int64), ("n_violations", C.c_int64),
+                ("seconds_kernel", C.c_double), ("seconds_total", C.c_double)]
+
+
+TL_SHARD_FIELDS = ("valid", "n_lookups", "n_records", "n_transfers", "n_reads", "count_by_kind", "witness_index",
+                   "kind", "transfer_id", "key", "related_index", "value", "bound")
+
+
+def tl_to_dict(res, shards) -> dict:
+    """One result dict for the library and the oracle (count_by_kind as a list indexed by kind - 1)."""
+    return {
+        "valid": res.valid, "n_failures": res.n_failures, "n_lookups": res.n_lookups, "n_records": res.n_records,
+        "n_transfers": res.n_transfers, "n_reads": res.n_reads, "n_violations": res.n_violations,
+        "seconds_kernel": res.seconds_kernel, "seconds_total": res.seconds_total,
+        "shards": [{f: (list(s.count_by_kind) if f == "count_by_kind" else getattr(s, f)) for f in TL_SHARD_FIELDS}
+                   for s in shards],
     }

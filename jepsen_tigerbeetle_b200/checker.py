@@ -359,6 +359,57 @@ class CounterBounds(Checker, _Native):
         return out
 
 
+class TransferLookups(Checker, _Native):
+    """The transfer records :ok lookups return held to the transfers clients issued and the counters reads show, on the
+    GPU (K9).
+
+    Reads the ledger-lookups form.  A record no transfer invoke carries (phantom), one that differs from its invocation
+    (mismatch), one of a :fail transfer (failed-visible) or of a transfer invoked after the lookup completed (future),
+    an id twice in one lookup (duplicate), a transfer missing from a lookup invoked after it was :ok (lost) or after an
+    earlier lookup returned it (vanished), and a read's counter below the sums of a lookup completed before it or above
+    those of a lookup invoked after it each prove an anomaly.  :info transfers are never required to appear.  Result:
+    {valid?, lookup-count, record-count, transfer-count, read-count, error-count, errors {kind count}, [op, error]}."""
+
+    def __init__(self, checker_opts: Mapping[str, Any] | None = None, ctx: Context | None = None,
+                 **ctx_opts) -> None:
+        _Native.__init__(self, ctx, **ctx_opts)
+
+    def _shard_map(self, s: dict) -> dict:
+        errors = {abi.TL_KIND_NAME[k + 1]: n for k, n in enumerate(s["count_by_kind"]) if n}
+        m: dict[str, Any] = {"valid?": VERDICT_NAME[s["valid"]], "lookup-count": s["n_lookups"],
+                             "record-count": s["n_records"], "transfer-count": s["n_transfers"],
+                             "read-count": s["n_reads"], "error-count": sum(errors.values()), "errors": errors}
+        if s["valid"] == INVALID:
+            m["op"] = {"index": s["witness_index"]}
+            kind = s["kind"]
+            err: dict[str, Any] = {"type": abi.TL_KIND_NAME[kind]}
+            if kind >= abi.TL_READ_BELOW_LOOKUP:
+                k = s["key"]
+                err.update({"key": [k >> 1, COUNTER_FIELDS[k & 1]], "value": s["value"], "bound": s["bound"]})
+            else:
+                err["transfer-id"] = s["transfer_id"]
+            if s["related_index"] >= 0:
+                err["related"] = {"index": s["related_index"]}
+            m["error"] = err
+        return m
+
+    def check_flat(self, test, h: FlatHistory) -> tuple[dict, list[dict]]:
+        r = self.ctx.check_transfer_lookups(h)
+        top = {"valid?": VERDICT_NAME[r["valid"]], "lookup-count": r["n_lookups"], "record-count": r["n_records"],
+               "transfer-count": r["n_transfers"], "read-count": r["n_reads"], "error-count": r["n_violations"],
+               "seconds-kernel": r["seconds_kernel"], "seconds-total": r["seconds_total"]}
+        return top, [self._shard_map(s) for s in r["shards"]]
+
+    def check(self, test, history, opts=None) -> dict:
+        h = _flat(history, "ledger-lookups")
+        if h.n_shards != 1:
+            raise ValueError("history has independent keys: wrap with independent_checker(...)")
+        top, per = self.check_flat(test, h)
+        out = dict(per[0])
+        out.update({k: v for k, v in top.items() if k.startswith("seconds-")})
+        return out
+
+
 class Compose(Checker):
     """`(checker/compose {name checker ...})`: run each, `:valid?` = merge-valid of the results."""
 
@@ -391,10 +442,13 @@ class Independent(Checker):
             return c.model
         if isinstance(c, (MonotonicKeys, CounterBounds)):
             return "ledger-counters"
+        if isinstance(c, TransferLookups):
+            return "ledger-lookups"
         return "set"
 
     def _per_key(self, checker: Checker, test, h: FlatHistory, opts) -> list[dict]:
-        if isinstance(checker, (Linearizable, SetFull, ReadAllInvokedAdds, MonotonicKeys, CounterBounds)):
+        if isinstance(checker, (Linearizable, SetFull, ReadAllInvokedAdds, MonotonicKeys, CounterBounds,
+                                TransferLookups)):
             try:
                 return checker.check_flat(test, h)[1]
             except Exception:  # noqa: BLE001
@@ -452,6 +506,11 @@ def monotonic_key_checker(opts: Mapping[str, Any] | None = None, **kw) -> Monoto
 def counter_bounds_checker(opts: Mapping[str, Any] | None = None, **kw) -> CounterBounds:
     """Every ledger read's counters against the bounds the :ok and :info transfers around it put on them (K8)."""
     return CounterBounds(opts, **kw)
+
+
+def transfer_lookup_checker(opts: Mapping[str, Any] | None = None, **kw) -> TransferLookups:
+    """The looked-up transfer records against the transfers clients issued and the counters reads show (K9)."""
+    return TransferLookups(opts, **kw)
 
 
 def compose(checkers: Mapping[str, Checker]) -> Compose:
@@ -620,12 +679,13 @@ def final_reads() -> FinalReads:
 
 
 def ledger_checker(checker_opts: Mapping[str, Any] | None = None, ctx: Context | None = None,
-                   linear: bool = True, monotonic: bool = False, counter_bounds: bool = False) -> Compose:
+                   linear: bool = True, monotonic: bool = False, counter_bounds: bool = False,
+                   transfer_lookups: bool = False) -> Compose:
     """The ledger test's checker (tests/ledger.clj:363-367) minus the gnuplot plotter, plus the
-    linearizability search the north-star adds and, with monotonic=True, the monotonic-key check and, with
-    counter_bounds=True, the counter-bounds check:
+    linearizability search the north-star adds and, with monotonic=True, the monotonic-key check, with
+    counter_bounds=True, the counter-bounds check and, with transfer_lookups=True, the transfer-lookup check:
         {:SI (checker opts) :lookup-transfers ... :final-reads ... :unexpected-ops ... [:linear ...] [:monotonic ...]
-         [:counter-bounds ...]}"""
+         [:counter-bounds ...] [:transfer-lookups ...]}"""
     cs: dict[str, Checker] = {"SI": bank_checker(checker_opts, ctx=ctx),
                               "lookup-transfers": lookup_all_invoked_transfers(),
                               "final-reads": final_reads(), "unexpected-ops": unexpected_ops()}
@@ -635,4 +695,6 @@ def ledger_checker(checker_opts: Mapping[str, Any] | None = None, ctx: Context |
         cs["monotonic"] = monotonic_key_checker(ctx=ctx)
     if counter_bounds:
         cs["counter-bounds"] = counter_bounds_checker(ctx=ctx)
+    if transfer_lookups:
+        cs["transfer-lookups"] = transfer_lookup_checker(ctx=ctx)
     return compose(cs)

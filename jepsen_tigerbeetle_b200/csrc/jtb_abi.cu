@@ -19,6 +19,7 @@
 #include "jtb_partition.cuh"
 #include "jtb_monotonic.cuh"
 #include "jtb_counter_bounds.cuh"
+#include "jtb_transfer_lookups.cuh"
 
 using namespace jtb;
 
@@ -726,6 +727,8 @@ long jtb_struct_size(int which) {
     case 10: return sizeof(jtb_mono_result);
     case 11: return sizeof(jtb_cb_shard);
     case 12: return sizeof(jtb_cb_result);
+    case 13: return sizeof(jtb_tl_shard);
+    case 14: return sizeof(jtb_tl_result);
     }
     return -1;
 }
@@ -1115,6 +1118,16 @@ int jtb_check_counter_bounds(jtb_ctx* ctx, const jtb_history* h, int32_t flags, 
     if (cudaSetDevice(ctx->device) != cudaSuccess) { ctx->err = "cudaSetDevice failed"; return -1; }
     ctx->fc.valid = false;
     return run_counter_bounds(ctx->stream, ctx->ev0, ctx->ev1, h, flags, shards, out, ctx->err);
+}
+
+// K9: the transfer-lookup check (csrc/jtb_transfer_lookups.cuh)
+int jtb_check_transfer_lookups(jtb_ctx* ctx, const jtb_history* h, int32_t flags, jtb_tl_shard* shards,
+                               jtb_tl_result* out) {
+    if (!ctx) return -1;
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    if (cudaSetDevice(ctx->device) != cudaSuccess) { ctx->err = "cudaSetDevice failed"; return -1; }
+    ctx->fc.valid = false;
+    return run_transfer_lookups(ctx->stream, ctx->ev0, ctx->ev1, h, flags, shards, out, ctx->err);
 }
 
 // SURVEY 8(f) N2: the step before the checkers (independent/subhistory, ledger->bank) on the device

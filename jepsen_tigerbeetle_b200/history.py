@@ -10,7 +10,7 @@ Op shapes accepted (reference file:line):
                 {:final? true}                                   set_full.clj:45
   * ledger:     {:f :txn :value [[:r id {:credits-posted c :debits-posted d}] ...]}
                 {:f :txn :value [[:t id {:debit-acct d :credit-acct c :amount a}]]}
-                {:f :txn :value [[:l-t ...]]}  (dropped)          tests/ledger.clj:27-62,89-114
+                {:f :txn :value [[:l-t ...]]}  (dropped; kept by 'ledger-lookups')  tests/ledger.clj:27-62,89-114
   * bank (jepsen.tests.bank): {:f :read :value {id bal}} / {:f :transfer :value {:from :to :amount}}
   * register / cas-register (knossos.model): :read v|nil, :write v, :cas [old new]
 
@@ -29,7 +29,7 @@ import numpy as np
 # ---- constants mirrored from include/jtb_check.h ------------------------------------------------
 VALID, UNKNOWN, INVALID = 0, 1, 2
 T_INVOKE, T_OK, T_FAIL, T_INFO = 0, 1, 2, 3
-F_READ, F_WRITE, F_CAS, F_ADD, F_TRANSFER = 0, 1, 2, 3, 4
+F_READ, F_WRITE, F_CAS, F_ADD, F_TRANSFER, F_LOOKUP = 0, 1, 2, 3, 4, 5
 NIL = -(2 ** 31)
 FLAG_FINAL = 1
 MODEL_REGISTER, MODEL_CAS_REGISTER, MODEL_SET, MODEL_BANK = 0, 1, 2, 3
@@ -267,7 +267,7 @@ def is_tuple(v: Any) -> bool:
 
 def flatten_ops(ops: Sequence[Mapping[str, Any]], model: str) -> FlatHistory:
     """Flatten a Jepsen history (sequence of op maps) for `model` in
-    {'register','cas-register','set','bank','ledger-counters'}.
+    {'register','cas-register','set','bank','ledger-counters','ledger-lookups'}.
 
     'ledger-counters' keeps what 'bank' folds into a balance: every account of a ledger :r read becomes two
     (key, value_lo, value_hi) triples, key = 2*account + field (0 debits-posted, 1 credits-posted), the input of the
@@ -275,12 +275,19 @@ def flatten_ops(ops: Sequence[Mapping[str, Any]], model: str) -> FlatHistory:
     meta["multi_transfer_txns"] counts the transfer txns (at their invocation) that had more than one micro-op, since
     the counter-bounds check would miss the others' amounts.
 
+    'ledger-lookups' is 'ledger-counters' plus the transfer-lookup check's evidence: a transfer invoke also carries one
+    record (id_lo, id_hi, debit, credit, amount) per [:t ...] micro-op (a multi-transfer txn is kept whole; a, b, c
+    stay the first micro-op's), and every [:l-t ...] op becomes an F_LOOKUP event whose :ok payload is the returned
+    records in the same layout (nil on the invoke, :info and :fail).  An :ok lookup with an empty value takes its tag
+    from its process's pending invoke.
+
     For 'bank', ledger-form :txn ops are first mapped by `ledger->bank` (tests/ledger.clj:89-114);
     stock jepsen.tests.bank {:from :to :amount} spelling is accepted too (SURVEY App. D).
     """
     model = _kw(model)
     bld = _Builder()
     multi_transfer = 0
+    pending_tag: dict = {}   # ledger-lookups: process -> the txn tag of its pending invoke
     for pos, op in enumerate(ops):
         type_ = TYPE_CODE[_kw(_get(op, "type"))]
         process = _get(op, "process")
@@ -376,9 +383,37 @@ def flatten_ops(ops: Sequence[Mapping[str, Any]], model: str) -> FlatHistory:
                 continue  # dropped, as ledger->bank drops it (tests/ledger.clj:110-111)
             else:
                 raise ValueError(f"unknown txn micro-op {tag!r}")
+        elif model == "ledger-lookups":
+            if f != "txn":
+                raise ValueError(f"unknown :f {f!r} for model ledger-lookups")
+            if value:
+                tag = _kw(value[0][0])
+            elif type_ != T_INVOKE and process in pending_tag:
+                tag = pending_tag[process]   # an empty :ok lookup: value[0][0] does not exist
+            else:
+                raise ValueError(f"op {index}: a txn without micro-ops")
+            if type_ == T_INVOKE:
+                pending_tag[process] = tag
+            else:
+                pending_tag.pop(process, None)
+            if tag == "r":
+                bld.add(key, type_, F_READ, flags, process, index, time,
+                        payload=_counter_triples(value, index) if type_ == T_OK else None)
+            elif tag == "t":
+                (_t, _id, tv) = value[0]
+                multi_transfer += type_ == T_INVOKE and len(value) > 1
+                bld.add(key, type_, F_TRANSFER, flags, process, index, time,
+                        a=int(_get(tv, "amount")), b=int(_get(tv, "debit-acct")),
+                        c=int(_get(tv, "credit-acct")),
+                        payload=_transfer_records(value, index) if type_ == T_INVOKE else None)
+            elif tag == "l-t":
+                bld.add(key, type_, F_LOOKUP, flags, process, index, time,
+                        payload=_transfer_records(value or [], index) if type_ == T_OK else None)
+            else:
+                raise ValueError(f"unknown txn micro-op {tag!r}")
         else:
             raise ValueError(f"unknown model {model!r}")
-    if model == "ledger-counters":
+    if model in ("ledger-counters", "ledger-lookups"):
         return bld.build({"model": model, "multi_transfer_txns": int(multi_transfer)})
     return bld.build({"model": model})
 
@@ -414,3 +449,34 @@ def _counter_triples(value, index) -> list[int]:
             pl.extend((counter_key(acct, field), lo - (1 << 32) if lo >= 1 << 31 else lo,
                        hi - (1 << 32) if hi >= 1 << 31 else hi))
     return pl
+
+
+TRANSFER_RECORD = 5   # int32 per transfer record of the ledger-lookups form: id_lo, id_hi, debit, credit, amount
+
+
+def _i32(x: int) -> int:
+    return x - (1 << 32) if x >= 1 << 31 else x
+
+
+def _transfer_records(value, index) -> list[int]:
+    """The [:t id {...}] or [:l-t id {...}] micro-ops of a txn as (id_lo, id_hi, debit, credit, amount) records; a
+    lookup micro-op without a transfer map (not found) is left out."""
+    pl: list[int] = []
+    for (_tag, tid, tv) in value:
+        if tv is None:
+            continue
+        if tid is None:
+            raise ValueError(f"op {index}: a transfer without an id")
+        tid = int(tid)
+        if not -(1 << 63) <= tid < (1 << 63):
+            raise ValueError(f"op {index}: transfer id {tid} does not fit in int64")
+        u = tid & 0xFFFFFFFFFFFFFFFF
+        pl.extend((_i32(u & 0xFFFFFFFF), _i32(u >> 32), int(_get(tv, "debit-acct")), int(_get(tv, "credit-acct")),
+                   int(_get(tv, "amount"))))
+    return pl
+
+
+def transfer_id(lo: int, hi: int) -> int:
+    """The int64 id of a record's (id_lo, id_hi) pair."""
+    u = ((int(hi) & 0xFFFFFFFF) << 32) | (int(lo) & 0xFFFFFFFF)
+    return u - (1 << 64) if u >= 1 << 63 else u

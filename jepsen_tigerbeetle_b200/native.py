@@ -19,13 +19,13 @@ CSRC = os.path.join(_HERE, "csrc")
 _SOURCES = ["jtb_abi.cu", "jtb_prep.cpp", "jtb_multi.cpp"]
 _DEPS = _SOURCES + ["jtb_prep.h", "jtb_expand.h", "jtb_wgl.cuh", "jtb_scout.cuh", "jtb_scans.cuh",
                     "jtb_table_bench.cuh", "jtb_level.cuh", "jtb_partition.cuh", "jtb_monotonic.cuh",
-                    "jtb_counter_bounds.cuh"]
+                    "jtb_counter_bounds.cuh", "jtb_transfer_lookups.cuh"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared", "-ldl"]
 
 EXPORTS = ["jtb_abi_version", "jtb_device_count", "jtb_create", "jtb_destroy", "jtb_last_error",
            "jtb_check_linearizable", "jtb_check_set_full", "jtb_check_bank_totals", "jtb_check_monotonic_keys",
-           "jtb_check_counter_bounds",
+           "jtb_check_counter_bounds", "jtb_check_transfer_lookups",
            "jtb_table_bench", "jtb_get_stats", "jtb_struct_size", "jtb_prepare_seconds", "jtb_prepare_info",
            "jtb_final_configs", "jtb_gather_bench", "jtb_host_alloc", "jtb_host_free", "jtb_partition_by_key", "jtb_ledger_balances", "jtb_multi_create", "jtb_multi_create_error", "jtb_multi_destroy", "jtb_multi_n_gpus",
            "jtb_multi_last_error", "jtb_multi_check_linearizable", "jtb_multi_check_set_full"]
@@ -76,6 +76,7 @@ def lib() -> C.CDLL:
             L.jtb_check_bank_totals.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]
             L.jtb_check_monotonic_keys.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
             L.jtb_check_counter_bounds.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
+            L.jtb_check_transfer_lookups.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
             L.jtb_table_bench.argtypes = [C.c_void_p, C.c_uint64, C.c_int, C.c_int, C.c_void_p,
                                           C.c_void_p, C.c_void_p]
             L.jtb_gather_bench.argtypes = [C.c_void_p, C.c_uint64, C.c_int, C.c_int, C.c_uint32, C.c_int, C.c_int,
@@ -207,6 +208,21 @@ class Context:
         if rc != 0:
             raise NativeError(f"jtb_check_counter_bounds rc={rc}: {self._err()}")
         return abi.cb_to_dict(res, shards[:h.n_shards])
+
+    # ---- K9: transfer-lookup check ------------------------------------------------------------------
+    def check_transfer_lookups(self, h: FlatHistory) -> dict:
+        """The transfer records :ok lookups return against the transfers clients issued and the counters reads show
+        (input: the ledger-lookups form).  {"valid", "n_failures", "n_lookups", "n_records", "n_transfers", "n_reads",
+        "n_violations", "seconds_kernel", "seconds_total", "shards": [{"valid", "n_lookups", "n_records",
+        "n_transfers", "n_reads", "count_by_kind", "witness_index", "kind", "transfer_id", "key", "related_index",
+        "value", "bound"}]}; count_by_kind[kind - 1]."""
+        ch = as_c_history(h)
+        shards = (abi.CTlShard * max(1, h.n_shards))()
+        res = abi.CTlResult()
+        rc = lib().jtb_check_transfer_lookups(self._h, C.addressof(ch), 0, C.addressof(shards), C.addressof(res))
+        if rc != 0:
+            raise NativeError(f"jtb_check_transfer_lookups rc={rc}: {self._err()}")
+        return abi.tl_to_dict(res, shards[:h.n_shards])
 
     def final_configs(self, h: FlatHistory, model: CModel, shard: int = 0, cap: int = 10) -> dict:
         """knossos' :configs of an INVALID shard (`jtb_final_configs`): call directly after `check_linearizable`

@@ -19,8 +19,8 @@ from dataclasses import dataclass
 
 import numpy as np
 
-from .history import (F_ADD, F_CAS, F_READ, F_TRANSFER, F_WRITE, NIL, T_FAIL, T_INFO, T_INVOKE,
-                      T_OK, FlatHistory)
+from .history import (F_ADD, F_CAS, F_LOOKUP, F_READ, F_TRANSFER, F_WRITE, FLAG_FINAL, NIL, T_FAIL, T_INFO,
+                      T_INVOKE, T_OK, TRANSFER_RECORD, FlatHistory)
 
 MASK64 = (1 << 64) - 1
 
@@ -106,8 +106,124 @@ def generate_ledger_counters(spec: SynthSpec, fractured: bool = False, lost_tran
     return _generate(spec, counters=True, fracture=fractured, lost=lost_transfer, duplicated=duplicated_transfer)
 
 
+def generate_ledger_lookups(spec: SynthSpec, p_lookup: float = 0.0, lost_transfer: bool = False,
+                            phantom_record: bool = False, mismatched_record: bool = False,
+                            vanished_record: bool = False, inflated_read: bool = False) -> FlatHistory:
+    """The ledger-lookups form of a one-key bank `spec` (what flatten_ops(..., "ledger-lookups") makes of a ledger
+    history): the events of generate_ledger_counters(spec), every transfer invoke carrying its record (id, debit,
+    credit, amount) with ids 1, 2, ... in invocation order, then one quiesced :final? lookup per client, one after
+    another, each returning every committed transfer (the :ok ones and the :info ones that took effect) in id order.
+    p_lookup > 0 (small histories only) adds about p_lookup * n_ops mid-history lookups, each on a process of its own,
+    drawn from a second random stream; each returns the committed transfers linearized before a point inside its
+    interval, and every event's :index is then its position.
+    Mutations (no extra random draws; several may be combined):
+      lost_transfer      generate_ledger_counters' lost transfer, missing from every lookup as well (LOST)
+      phantom_record     the first final lookup also returns an id no transfer carries (PHANTOM)
+      mismatched_record  the first final lookup returns its middle record with amount + 1 (MISMATCH)
+      vanished_record    the last final lookup drops the middle committed :info transfer (VANISHED, and the final
+                         read, which completes first, now lies above that lookup's sums; needs p_info > 0 and two
+                         clients)
+      inflated_read      the final read's first counter is one more than it was (READ_ABOVE_LOOKUP; needs
+                         spec.final_reads)"""
+    if spec.model != "bank" or spec.n_keys != 1:
+        raise ValueError("the ledger-lookups form needs a one-key bank spec")
+    if inflated_read and not spec.final_reads:
+        raise ValueError("inflated_read needs spec.final_reads")
+    ex: dict = {}
+    base = _generate(spec, counters=True, lost=lost_transfer, extra=ex)
+    ops, op_ev, C = ex["ops"], ex["op_of_event"], spec.n_clients
+    n = base.n_events
+    # ---- transfer records: ids 1, 2, ... in invocation order ----------------------------------------------------
+    tin = np.nonzero((base.f == F_TRANSFER) & (base.type == T_INVOKE))[0]
+    t_ops = op_ev[tin]
+    o_arr = np.array([ops[i] for i in t_ops], np.int64).reshape(-1, 11)
+    ids = np.arange(1, len(tin) + 1, dtype=np.int64)
+    rec = np.zeros((len(tin), TRANSFER_RECORD), np.int32)
+    rec[:, 0], rec[:, 2], rec[:, 3], rec[:, 4] = ids, o_arr[:, 8], o_arr[:, 9], o_arr[:, 7]
+    committed = o_arr[:, 10] < 2
+    if lost_transfer and ex["mutated_transfer"] >= 0:
+        committed &= t_ops != ex["mutated_transfer"]
+    t_lin = o_arr[:, 2]
+    # ---- lookups: (time, process, records) ----------------------------------------------------------------------
+    lookups: list[tuple[int, int, int, np.ndarray, bool]] = []   # (invoke time, completion time, process, recs, final)
+    max_proc = int(base.process.max()) if n else -1
+    if p_lookup > 0 and n:
+        rng = PCG32(spec.seed, 2)
+        t0, t1 = int(base.time_ns[0]), int(base.time_ns[~(base.flags & FLAG_FINAL).astype(bool)].max())
+        for j in range(int(round(p_lookup * spec.n_ops))):
+            q = t0 + 1 + rng.below(max(1, t1 - t0))
+            lookups.append((q - rng.exp_ns(spec.tau_op_ns), q + rng.exp_ns(spec.tau_op_ns), max_proc + 1 + j,
+                            rec[committed & (t_lin < q)], False))
+    tq = int(base.time_ns.max()) + 1_000_000_000 if n else 0
+    last_proc = list(range(C))
+    for p in np.unique(base.process):
+        last_proc[int(p) % C] = max(last_proc[int(p) % C], int(p))
+    fin = rec[committed]
+    for t in range(C):
+        lookups.append((tq + 2 * t, tq + 2 * t + 1, last_proc[t], fin, True))
+    n_final = C
+    finals = [i for i, lk in enumerate(lookups) if lk[4]]
+    if phantom_record:
+        i = finals[0]
+        extra = fin[len(fin) // 2].copy() if len(fin) else np.array([0, 0, 1, 2, 1], np.int32)
+        extra[0], extra[1] = len(tin) + 1, 0
+        lookups[i] = lookups[i][:3] + (np.concatenate([lookups[i][3], extra[None]]),) + lookups[i][4:]
+    if mismatched_record:
+        i = finals[0]
+        r = lookups[i][3].copy()
+        r[len(r) // 2, 4] += 1
+        lookups[i] = lookups[i][:3] + (r,) + lookups[i][4:]
+    if vanished_record:
+        info = np.nonzero(committed & (o_arr[:, 10] == 1))[0]
+        if len(info) == 0 or n_final < 2:
+            raise ValueError("vanished_record needs a committed :info transfer and two clients")
+        gone = ids[info[len(info) // 2]]
+        i = finals[-1]
+        lookups[i] = lookups[i][:3] + (lookups[i][3][lookups[i][3][:, 0] != gone],) + lookups[i][4:]
+    # ---- events, payload ----------------------------------------------------------------------------------------
+    L = len(lookups)
+    plen_pre = np.concatenate([base.payload_len, np.full(2 * L, -1, np.int32)])
+    plen_pre[tin] = TRANSFER_RECORD
+    for j, lk in enumerate(lookups):
+        plen_pre[n + 2 * j + 1] = lk[3].size
+    lens = np.maximum(plen_pre, 0).astype(np.int64)
+    poff_pre = np.zeros(n + 2 * L, np.int64)
+    np.cumsum(lens[:-1], out=poff_pre[1:])
+    payload = np.zeros(int(lens.sum()), np.int32)
+    reads = np.nonzero(base.payload_len > 0)[0]
+    if len(reads):
+        rl = base.payload_len[reads].astype(np.int64)
+        within = np.arange(int(rl.sum())) - np.repeat(np.cumsum(rl) - rl, rl)
+        payload[np.repeat(poff_pre[reads], rl) + within] = base.payload[np.repeat(base.payload_off[reads], rl) + within]
+    payload[poff_pre[tin][:, None] + np.arange(TRANSFER_RECORD)] = rec
+    for j, lk in enumerate(lookups):
+        o = poff_pre[n + 2 * j + 1]
+        payload[o:o + lk[3].size] = lk[3].reshape(-1)
+    if inflated_read:
+        e = np.nonzero((base.flags & FLAG_FINAL).astype(bool) & (base.type == T_OK) & (base.f == F_READ))[0][0]
+        payload[poff_pre[e] + 1] += 1
+    lt = np.array([x for lk in lookups for x in lk[:2]], np.int64)
+    time_pre = np.concatenate([base.time_ns, lt])
+    order = np.argsort(time_pre, kind="stable")
+    cat = lambda arr, tail: np.concatenate([arr, np.asarray(tail, arr.dtype)])[order]   # noqa: E731
+    typ = cat(base.type, [T_INVOKE, T_OK] * L)
+    f = cat(base.f, [F_LOOKUP] * (2 * L))
+    flags = cat(base.flags, [FLAG_FINAL if lk[4] else 0 for lk in lookups for _ in (0, 1)])
+    proc = cat(base.process, [lk[2] for lk in lookups for _ in (0, 1)])
+    zeros = [0] * (2 * L)
+    index = (cat(base.index, np.arange(n, n + 2 * L)) if p_lookup <= 0 else
+             np.arange(n + 2 * L, dtype=np.int32))
+    meta = dict(base.meta, model="ledger-lookups", n_ops=base.meta["n_ops"] + L, multi_transfer_txns=0,
+                n_lookups=L)
+    h = FlatHistory(typ, f, flags, proc, index.astype(np.int32), time_pre[order], cat(base.a, zeros),
+                    cat(base.b, zeros), cat(base.c, zeros), poff_pre[order], plen_pre[order], payload,
+                    np.array([0, n + 2 * L], np.int64), base.key_ids.copy(), meta)
+    h.validate()
+    return h
+
+
 def _generate(spec: SynthSpec, counters: bool = False, fracture: bool = False, lost: bool = False,
-              duplicated: bool = False) -> FlatHistory:
+              duplicated: bool = False, extra: dict | None = None) -> FlatHistory:
     rng = PCG32(spec.seed, 1)
     C, K = spec.n_clients, spec.n_keys
     model = spec.model
@@ -358,6 +474,9 @@ def _generate(spec: SynthSpec, counters: bool = False, fracture: bool = False, l
             meta["lost_op_index"] = mutated_transfer
         if duplicated:
             meta["duplicated_op_index"] = mutated_transfer
+    if extra is not None:   # what generate_ledger_lookups builds on
+        extra.update(ops=all_ops, op_of_event=np.array([e[2] for e in ev], np.int64)[perm],
+                     mutated_transfer=mutated_transfer)
     h = FlatHistory(typ[perm], f_arr[perm], flags[perm], proc_arr[perm], idx[perm], time_arr[perm],
                     a_arr[perm], b_arr[perm], c_arr[perm], poff, plen_p, payload, shard_off,
                     np.arange(1, K + 1, dtype=np.int64), meta)

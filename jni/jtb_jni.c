@@ -425,3 +425,42 @@ JNIEXPORT jlongArray JNICALL Java_jtb_Native_checkCounterBounds(JNIEnv* env, jcl
     free(shards);
     return out;
 }
+
+/* ---- K9: transfer-lookup check ------------------------------------------------------------------------------- */
+JNIEXPORT jlongArray JNICALL Java_jtb_Native_checkTransferLookups(JNIEnv* env, jclass cls, jlong handle,
+                                                                   jobjectArray history) {
+    (void)cls;
+    jtb_history hist;
+    hist_pins pins;
+    if (pin_history(env, history, &hist, &pins)) return NULL;
+    const int ns = hist.n_shards;
+    jtb_tl_shard* shards = (jtb_tl_shard*)calloc(ns > 0 ? (size_t)ns : 1, sizeof *shards);
+    jtb_tl_result r;
+    memset(&r, 0, sizeof r);
+    const int rc = jtb_check_transfer_lookups((jtb_ctx*)(intptr_t)handle, &hist, 0, shards, &r);
+    unpin_history(env, &pins);
+    if (rc != 0) {
+        free(shards);
+        throw_rt(env, jtb_last_error((jtb_ctx*)(intptr_t)handle));
+        return NULL;
+    }
+    const int64_t per = 12 + JTB_TL_KINDS;
+    const int64_t total = 10 + per * ns;
+    jlong* v = (jlong*)calloc((size_t)total, sizeof *v);
+    int64_t k = 0;
+    v[k++] = r.valid; v[k++] = r.n_failures; v[k++] = r.n_lookups; v[k++] = r.n_records; v[k++] = r.n_transfers;
+    v[k++] = r.n_reads; v[k++] = r.n_violations; v[k++] = ns_of(r.seconds_kernel); v[k++] = ns_of(r.seconds_total);
+    v[k++] = ns;
+    for (int s = 0; s < ns; ++s) {
+        const jtb_tl_shard* q = &shards[s];
+        v[k++] = q->valid; v[k++] = q->n_lookups; v[k++] = q->n_records; v[k++] = q->n_transfers; v[k++] = q->n_reads;
+        for (int j = 0; j < JTB_TL_KINDS; ++j) v[k++] = q->count_by_kind[j];
+        v[k++] = q->witness_index; v[k++] = q->kind; v[k++] = q->transfer_id; v[k++] = q->key;
+        v[k++] = q->related_index; v[k++] = q->value; v[k++] = q->bound;
+    }
+    jlongArray out = (*env)->NewLongArray(env, (jsize)k);
+    if (out) (*env)->SetLongArrayRegion(env, out, 0, (jsize)k, v);
+    free(v);
+    free(shards);
+    return out;
+}

@@ -3,7 +3,9 @@ ONLY.
 
 MONO_GRAPH builds Elle's monotonic-key graph literally (plus real-time edges) and runs Tarjan; MONO_PAIRS searches
 for 2-cycles by brute force.  See mono_oracle.cpp.  CB_LITERAL sums every transfer for every (read, key); CB_SWEEP
-keeps running sums over one walk of the events.  See counter_bounds.cpp."""
+keeps running sums over one walk of the events.  See counter_bounds.cpp.  TL_LITERAL checks every (lookup, transfer)
+pair and every (read, key, lookup) triple; TL_SWEEP walks with hash maps, sorted M lists, prefix maxima and suffix
+minima.  See transfer_lookups.cpp."""
 from __future__ import annotations
 
 import ctypes as C
@@ -16,6 +18,7 @@ from jepsen_tigerbeetle_b200.history import FlatHistory, as_c_history
 
 MONO_GRAPH, MONO_PAIRS = 0, 1
 CB_LITERAL, CB_SWEEP = 0, 1
+TL_LITERAL, TL_SWEEP = 0, 1
 DECIDE_PARTIAL = 1 << 16   # decide shards with partial reads instead of reporting them UNKNOWN
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB = None
@@ -25,7 +28,7 @@ def build(force: bool = False) -> str:
     """The library in mono_oracle/, rebuilt when stale; when the directory is read-only a rebuild goes to a fresh
     temporary directory instead."""
     so = os.path.join(_HERE, "libjtb_mono_oracle.so")
-    srcs = [os.path.join(_HERE, f) for f in ("mono_oracle.cpp", "counter_bounds.cpp", "Makefile")]
+    srcs = [os.path.join(_HERE, f) for f in ("mono_oracle.cpp", "counter_bounds.cpp", "transfer_lookups.cpp", "Makefile")]
     srcs.append(os.path.join(_HERE, "..", "include", "jtb_check.h"))
     stale = not os.path.exists(so) or any(os.path.getmtime(s) > os.path.getmtime(so) for s in srcs)
     if force or stale:
@@ -45,6 +48,8 @@ def lib() -> C.CDLL:
         _LIB.jtbm_check_monotonic_keys.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
         _LIB.jtbm_cb_last_error.restype = C.c_char_p
         _LIB.jtbm_check_counter_bounds.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
+        _LIB.jtbm_tl_last_error.restype = C.c_char_p
+        _LIB.jtbm_check_transfer_lookups.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
     return _LIB
 
 
@@ -70,3 +75,14 @@ def check_counter_bounds(h: FlatHistory, algo: int = CB_SWEEP, flags: int = 0) -
     if rc != 0:
         raise RuntimeError(lib().jtbm_cb_last_error().decode())
     return abi.cb_to_dict(res, shards[:h.n_shards])
+
+
+def check_transfer_lookups(h: FlatHistory, algo: int = TL_SWEEP, flags: int = 0) -> dict:
+    """Twin of `jtb_check_transfer_lookups` (same result dict as `native.Context.check_transfer_lookups`)."""
+    ch = as_c_history(h)
+    shards = (abi.CTlShard * max(1, h.n_shards))()
+    res = abi.CTlResult()
+    rc = lib().jtbm_check_transfer_lookups(C.addressof(ch), flags, algo, C.addressof(shards), C.addressof(res))
+    if rc != 0:
+        raise RuntimeError(lib().jtbm_tl_last_error().decode())
+    return abi.tl_to_dict(res, shards[:h.n_shards])
