@@ -23,6 +23,7 @@
 #include <cuda_runtime.h>
 
 #include "../../include/jtb_check.h"
+#include "jtb_call.cuh"
 #include "jtb_monotonic.cuh"
 
 namespace jtb {
@@ -75,10 +76,6 @@ __device__ __forceinline__ void cb_bounds(const CbDev& d, int32_t r, int32_t slo
     U = ju > lo ? d.sumU[ju - 1] : 0;
 }
 
-__device__ __forceinline__ int64_t cb_value(const int32_t* p) {
-    return (int64_t)(((uint64_t)(uint32_t)p[2] << 32) | (uint32_t)p[1]);
-}
-
 // thread per contribution: both sort keys (completion INT_MAX for transfers that are not :ok)
 __global__ void cb_keys(int32_t n, const int32_t* __restrict__ slot, const int32_t* __restrict__ inv,
                         const int32_t* __restrict__ comp, uint64_t* __restrict__ keyL, uint64_t* __restrict__ keyU,
@@ -114,13 +111,8 @@ __global__ void cb_check(CbDev d, unsigned long long* __restrict__ n_below, unsi
     unsigned below = 0, above = 0;
     int32_t first = INT_MAX;
     for (int32_t j = lane; j < nt; j += 32) {
-        const int32_t key = p[3 * j];
-        int32_t a = 0, b = K;   // lower_bound: the host pass put every observed key in the table
-        while (a < b) {
-            const int32_t c = (a + b) >> 1;
-            if (kt[c] < key) a = c + 1; else b = c;
-        }
-        const int64_t v = cb_value(p + 3 * j);
+        const int32_t a = mono_col(kt, K, p[3 * j]);   // the host pass put every observed key in the table
+        const int64_t v = mono_join(p[3 * j + 1], p[3 * j + 2]);
         int64_t L, U;
         int32_t jl, ju;
         cb_bounds(d, r, (int32_t)d.key_off[sh] + a, L, U, jl, ju);
@@ -157,7 +149,7 @@ __global__ void cb_explain(CbDev d, int32_t n_shards, const unsigned long long* 
     const int32_t* p = d.payload + d.poff[r];
     int64_t v = 0;
     for (int32_t j = 0; j < d.ntrip[r]; ++j)
-        if (p[3 * j] == key) { v = cb_value(p + 3 * j); break; }
+        if (p[3 * j] == key) { v = mono_join(p[3 * j + 1], p[3 * j + 2]); break; }
     int64_t L, U;
     int32_t jl, ju;
     cb_bounds(d, r, slot, L, U, jl, ju);
@@ -198,7 +190,6 @@ inline int cb_transfer_pass(const jtb_history* h, const MonoHost& H, CbContrib& 
     C.n_transfers.assign(S, 0);
     std::vector<int64_t> cnt(H.keys.size() + 1, 0);
     std::unordered_map<int32_t, int64_t> open;   // process -> event of its pending transfer invoke
-    char buf[256];
     for (int32_t s = 0; s < S; ++s) {
         const int64_t lo = h->shard_off[s], hi = h->shard_off[s + 1];
         const int32_t* kt = H.keys.data() + H.key_off[s];
@@ -211,7 +202,7 @@ inline int cb_transfer_pass(const jtb_history* h, const MonoHost& H, CbContrib& 
             const int32_t acct[2] = {h->b[ie], h->c[ie]};
             for (int field = 0; field < 2; ++field) {
                 const int32_t key = 2 * acct[field] + field;
-                const int32_t col = (int32_t)(std::lower_bound(kt, kt + K, key) - kt);
+                const int32_t col = mono_col(kt, K, key);
                 if (col == K || kt[col] != key) continue;   // no :ok read of the shard observes it
                 if (C.slot.size() >= (size_t)INT_MAX) { err = "more than 2^31-1 transfer contributions"; return -2; }
                 const int32_t slot = (int32_t)H.key_off[s] + col;
@@ -236,16 +227,9 @@ inline int cb_transfer_pass(const jtb_history* h, const MonoHost& H, CbContrib& 
                 if (int rc = resolve(ie, h->type[e] == JTB_T_INVOKE ? -1 : e)) return rc;
             }
             if (h->type[e] != JTB_T_INVOKE || h->f[e] != JTB_F_TRANSFER) continue;
-            if (h->a[e] < 0) {
-                snprintf(buf, sizeof buf, "transfer at :index %d: negative amount %d", h->index[e], h->a[e]);
-                err = buf;
-                return -2;
-            }
-            if (h->b[e] < 0 || h->b[e] >= (1 << 30) || h->c[e] < 0 || h->c[e] >= (1 << 30)) {
-                snprintf(buf, sizeof buf, "transfer at :index %d: account outside [0, 2^30)", h->index[e]);
-                err = buf;
-                return -2;
-            }
+            if (h->a[e] < 0) return input_error(err, "transfer at :index %d: negative amount %d", h->index[e], h->a[e]);
+            if (h->b[e] < 0 || h->b[e] >= (1 << 30) || h->c[e] < 0 || h->c[e] >= (1 << 30))
+                return input_error(err, "transfer at :index %d: account outside [0, 2^30)", h->index[e]);
             open.emplace(p, e);
         }
         // never completed, in invocation order (the order only decides the record order, which the sorts erase)
@@ -260,24 +244,12 @@ inline int cb_transfer_pass(const jtb_history* h, const MonoHost& H, CbContrib& 
     return 0;
 }
 
-#define CBOK(call)                                                                                        \
-    do {                                                                                                  \
-        cudaError_t e_ = (call);                                                                          \
-        if (e_ != cudaSuccess) { err = std::string(#call) + ": " + cudaGetErrorString(e_); return -1; }  \
-    } while (0)
-
 inline int run_counter_bounds(cudaStream_t st, cudaEvent_t ev0, cudaEvent_t ev1, const jtb_history* h, int32_t flags,
                               jtb_cb_shard* shards, jtb_cb_result* out, std::string& err) {
     const auto t0 = std::chrono::steady_clock::now();
     if (!h || !shards || !out) { err = "null argument"; return -2; }
     if (flags != 0) { err = "flags must be 0 (reserved)"; return -2; }
-    if (h->n_events < 0 || h->n_shards < 0 || (h->n_events > 0 && (!h->type || !h->f || !h->process || !h->index ||
-                                                                  !h->a || !h->b || !h->c || !h->payload_off ||
-                                                                  !h->payload_len)) ||
-        !h->shard_off || (h->n_payload > 0 && !h->payload)) {
-        err = "malformed jtb_history";
-        return -2;
-    }
+    if (int rc = check_history(h, true, err)) return rc;
     const int32_t S = h->n_shards;
     MonoHost H;
     if (int rc = mono_host_pass(h, H, err)) return rc;
@@ -298,105 +270,84 @@ inline int run_counter_bounds(cudaStream_t st, cudaEvent_t ev0, cudaEvent_t ev1,
     const int32_t m = (int32_t)H.r_shard.size(), n = (int32_t)C.slot.size();
     float ms = 0;
     if (m > 0) {
-        MonoAllocs A;
+        CallAllocs A;
+        CbDev d;
+        d.m = m;
         const size_t slots = H.keys.size();
-        void *p_payload, *p_poff, *p_ntrip, *p_shard, *p_inv, *p_comp, *p_nk, *p_koff, *p_keys, *p_off, *p_cslot, *p_cinv,
-            *p_ccomp, *p_camt, *p_ciidx, *p_ccidx, *p_k0, *p_k1, *p_kL, *p_kU, *p_id0, *p_idL, *p_idU, *p_aL, *p_aU, *p_sL,
-            *p_sU, *p_below, *p_above, *p_wkey, *p_wit, *p_tmp;
-        CBOK(A.get(&p_payload, (size_t)h->n_payload * 4));
-        CBOK(A.get(&p_poff, (size_t)m * 8)); CBOK(A.get(&p_ntrip, (size_t)m * 4)); CBOK(A.get(&p_shard, (size_t)m * 4));
-        CBOK(A.get(&p_inv, (size_t)m * 4)); CBOK(A.get(&p_comp, (size_t)m * 4));
-        CBOK(A.get(&p_nk, (size_t)S * 4)); CBOK(A.get(&p_koff, ((size_t)S + 1) * 8)); CBOK(A.get(&p_keys, slots * 4));
-        CBOK(A.get(&p_off, (slots + 1) * 4));
-        CBOK(A.get(&p_cslot, (size_t)n * 4)); CBOK(A.get(&p_cinv, (size_t)n * 4)); CBOK(A.get(&p_ccomp, (size_t)n * 4));
-        CBOK(A.get(&p_camt, (size_t)n * 4)); CBOK(A.get(&p_ciidx, (size_t)n * 4)); CBOK(A.get(&p_ccidx, (size_t)n * 4));
-        CBOK(A.get(&p_k0, (size_t)n * 8)); CBOK(A.get(&p_k1, (size_t)n * 8));
-        CBOK(A.get(&p_kL, (size_t)n * 8)); CBOK(A.get(&p_kU, (size_t)n * 8));
-        CBOK(A.get(&p_id0, (size_t)n * 4)); CBOK(A.get(&p_idL, (size_t)n * 4)); CBOK(A.get(&p_idU, (size_t)n * 4));
-        CBOK(A.get(&p_aL, (size_t)n * 8)); CBOK(A.get(&p_aU, (size_t)n * 8));
-        CBOK(A.get(&p_sL, (size_t)n * 8)); CBOK(A.get(&p_sU, (size_t)n * 8));
-        CBOK(A.get(&p_below, (size_t)S * 8)); CBOK(A.get(&p_above, (size_t)S * 8)); CBOK(A.get(&p_wkey, (size_t)S * 8));
-        CBOK(A.get(&p_wit, (size_t)S * sizeof(CbWitness)));
+        const int32_t *cslot, *cinv, *ccomp, *camt, *ciidx, *ccidx;
+        uint64_t *k0, *k1, *kL, *kU;
+        int32_t *id0, *idL, *idU;
+        int64_t *aL, *aU, *sL, *sU;
+        unsigned long long *below, *above, *wkey;
+        CbWitness* wit;
+        uint8_t* tmp;
+        JTB_OK(A.put(&d.payload, h->payload, (size_t)h->n_payload, st));
+        JTB_OK(A.put(&d.poff, H.r_poff, st)); JTB_OK(A.put(&d.ntrip, H.r_ntrip, st)); JTB_OK(A.put(&d.shard, H.r_shard, st));
+        JTB_OK(A.put(&d.inv, H.r_inv, st)); JTB_OK(A.put(&d.comp, H.r_comp, st));
+        JTB_OK(A.put(&d.n_keys, H.n_keys, st)); JTB_OK(A.put(&d.key_off, H.key_off, st)); JTB_OK(A.put(&d.keys, H.keys, st));
+        JTB_OK(A.put(&d.off, C.off, st));
+        JTB_OK(A.put(&cslot, C.slot, st)); JTB_OK(A.put(&cinv, C.inv, st)); JTB_OK(A.put(&ccomp, C.comp, st));
+        JTB_OK(A.put(&camt, C.amount, st)); JTB_OK(A.put(&ciidx, C.iidx, st)); JTB_OK(A.put(&ccidx, C.cidx, st));
+        JTB_OK(A.alloc(&k0, n)); JTB_OK(A.alloc(&k1, n));
+        JTB_OK(A.alloc(&kL, n)); JTB_OK(A.alloc(&kU, n));
+        JTB_OK(A.alloc(&id0, n)); JTB_OK(A.alloc(&idL, n)); JTB_OK(A.alloc(&idU, n));
+        JTB_OK(A.alloc(&aL, n)); JTB_OK(A.alloc(&aU, n));
+        JTB_OK(A.alloc(&sL, n)); JTB_OK(A.alloc(&sU, n));
+        JTB_OK(A.alloc(&below, S)); JTB_OK(A.alloc(&above, S)); JTB_OK(A.alloc(&wkey, S));
+        JTB_OK(A.alloc(&wit, S));
+        d.keyL = kL; d.keyU = kU;
+        d.idL = idL; d.idU = idU;
+        d.sumL = sL; d.sumU = sU;
         // keys = slot << 32 | position: the bits above the largest slot are zero
         int end_bit = 32;
         while (end_bit < 64 && (slots >> (end_bit - 32)) != 0) ++end_bit;
         size_t tmp_sort = 0, tmp_scan = 0;
         if (n > 0) {
-            CBOK(cub::DeviceRadixSort::SortPairs(nullptr, tmp_sort, (uint64_t*)p_k0, (uint64_t*)p_kL, (int32_t*)p_id0,
-                                                 (int32_t*)p_idL, n, 0, end_bit, st));
-            CBOK(cub::DeviceScan::InclusiveSumByKey(nullptr, tmp_scan, (const uint64_t*)p_kL, (const int64_t*)p_aL,
-                                                    (int64_t*)p_sL, n, CbSlotEq{}, st));
+            JTB_OK(cub::DeviceRadixSort::SortPairs(nullptr, tmp_sort, k0, kL, id0, idL, n, 0, end_bit, st));
+            JTB_OK(cub::DeviceScan::InclusiveSumByKey(nullptr, tmp_scan, d.keyL, (const int64_t*)aL, sL, n, CbSlotEq{},
+                                                      st));
         }
         const size_t tmp_bytes = std::max(tmp_sort, tmp_scan);
-        CBOK(A.get(&p_tmp, tmp_bytes));
-        auto up = [&](void* dst, const void* src, size_t bytes) {
-            return bytes ? cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, st) : cudaSuccess;
-        };
-        CBOK(up(p_payload, h->payload, (size_t)h->n_payload * 4));
-        CBOK(up(p_poff, H.r_poff.data(), (size_t)m * 8)); CBOK(up(p_ntrip, H.r_ntrip.data(), (size_t)m * 4));
-        CBOK(up(p_shard, H.r_shard.data(), (size_t)m * 4)); CBOK(up(p_inv, H.r_inv.data(), (size_t)m * 4));
-        CBOK(up(p_comp, H.r_comp.data(), (size_t)m * 4));
-        CBOK(up(p_nk, H.n_keys.data(), (size_t)S * 4)); CBOK(up(p_koff, H.key_off.data(), ((size_t)S + 1) * 8));
-        CBOK(up(p_keys, H.keys.data(), slots * 4)); CBOK(up(p_off, C.off.data(), (slots + 1) * 4));
-        CBOK(up(p_cslot, C.slot.data(), (size_t)n * 4)); CBOK(up(p_cinv, C.inv.data(), (size_t)n * 4));
-        CBOK(up(p_ccomp, C.comp.data(), (size_t)n * 4)); CBOK(up(p_camt, C.amount.data(), (size_t)n * 4));
-        CBOK(up(p_ciidx, C.iidx.data(), (size_t)n * 4)); CBOK(up(p_ccidx, C.cidx.data(), (size_t)n * 4));
-
-        CbDev d;
-        d.m = m;
-        d.payload = (const int32_t*)p_payload; d.poff = (const int64_t*)p_poff; d.ntrip = (const int32_t*)p_ntrip;
-        d.shard = (const int32_t*)p_shard; d.inv = (const int32_t*)p_inv; d.comp = (const int32_t*)p_comp;
-        d.n_keys = (const int32_t*)p_nk; d.key_off = (const int64_t*)p_koff; d.keys = (const int32_t*)p_keys;
-        d.off = (const int32_t*)p_off;
-        d.keyL = (const uint64_t*)p_kL; d.keyU = (const uint64_t*)p_kU;
-        d.idL = (const int32_t*)p_idL; d.idU = (const int32_t*)p_idU;
-        d.sumL = (const int64_t*)p_sL; d.sumU = (const int64_t*)p_sU;
+        JTB_OK(A.alloc(&tmp, tmp_bytes));
         const unsigned c_grid = (unsigned)(((int64_t)n + 255) / 256);
         const unsigned warp_grid = (unsigned)(((int64_t)m * 32 + 255) / 256);
         const unsigned sh_grid = (unsigned)((S + 255) / 256);
 
-        CBOK(cudaEventRecord(ev0, st));
-        CBOK(cudaMemsetAsync(p_below, 0, (size_t)S * 8, st));
-        CBOK(cudaMemsetAsync(p_above, 0, (size_t)S * 8, st));
-        CBOK(cudaMemsetAsync(p_wkey, 0xff, (size_t)S * 8, st));
+        JTB_OK(cudaEventRecord(ev0, st));
+        JTB_OK(cudaMemsetAsync(below, 0, (size_t)S * 8, st));
+        JTB_OK(cudaMemsetAsync(above, 0, (size_t)S * 8, st));
+        JTB_OK(cudaMemsetAsync(wkey, 0xff, (size_t)S * 8, st));
         if (n > 0) {
-            cb_keys<<<c_grid, 256, 0, st>>>(n, (const int32_t*)p_cslot, (const int32_t*)p_cinv,
-                                            (const int32_t*)p_ccomp, (uint64_t*)p_k0, (uint64_t*)p_k1, (int32_t*)p_id0);
+            cb_keys<<<c_grid, 256, 0, st>>>(n, cslot, cinv, ccomp, k0, k1, id0);
             size_t tb = tmp_bytes;
-            CBOK(cub::DeviceRadixSort::SortPairs(p_tmp, tb, (uint64_t*)p_k0, (uint64_t*)p_kL, (int32_t*)p_id0,
-                                                 (int32_t*)p_idL, n, 0, end_bit, st));
+            JTB_OK(cub::DeviceRadixSort::SortPairs(tmp, tb, k0, kL, id0, idL, n, 0, end_bit, st));
             tb = tmp_bytes;
-            CBOK(cub::DeviceRadixSort::SortPairs(p_tmp, tb, (uint64_t*)p_k1, (uint64_t*)p_kU, (int32_t*)p_id0,
-                                                 (int32_t*)p_idU, n, 0, end_bit, st));
-            cb_gather<<<c_grid, 256, 0, st>>>(n, (const int32_t*)p_camt, d.idL, d.idU, (int64_t*)p_aL, (int64_t*)p_aU);
+            JTB_OK(cub::DeviceRadixSort::SortPairs(tmp, tb, k1, kU, id0, idU, n, 0, end_bit, st));
+            cb_gather<<<c_grid, 256, 0, st>>>(n, camt, d.idL, d.idU, aL, aU);
             tb = tmp_bytes;
-            CBOK(cub::DeviceScan::InclusiveSumByKey(p_tmp, tb, d.keyL, (const int64_t*)p_aL, (int64_t*)p_sL, n,
-                                                    CbSlotEq{}, st));
+            JTB_OK(cub::DeviceScan::InclusiveSumByKey(tmp, tb, d.keyL, (const int64_t*)aL, sL, n, CbSlotEq{}, st));
             tb = tmp_bytes;
-            CBOK(cub::DeviceScan::InclusiveSumByKey(p_tmp, tb, d.keyU, (const int64_t*)p_aU, (int64_t*)p_sU, n,
-                                                    CbSlotEq{}, st));
+            JTB_OK(cub::DeviceScan::InclusiveSumByKey(tmp, tb, d.keyU, (const int64_t*)aU, sU, n, CbSlotEq{}, st));
         }
-        cb_check<<<warp_grid, 256, 0, st>>>(d, (unsigned long long*)p_below, (unsigned long long*)p_above,
-                                            (unsigned long long*)p_wkey);
-        cb_explain<<<sh_grid, 256, 0, st>>>(d, S, (const unsigned long long*)p_wkey, (const int32_t*)p_ccidx,
-                                            (const int32_t*)p_ciidx, (CbWitness*)p_wit);
-        CBOK(cudaGetLastError());
-        CBOK(cudaEventRecord(ev1, st));
-        std::vector<unsigned long long> below(S), above(S), wkey(S);
-        std::vector<CbWitness> wit(S);
-        CBOK(cudaMemcpyAsync(below.data(), p_below, (size_t)S * 8, cudaMemcpyDeviceToHost, st));
-        CBOK(cudaMemcpyAsync(above.data(), p_above, (size_t)S * 8, cudaMemcpyDeviceToHost, st));
-        CBOK(cudaMemcpyAsync(wkey.data(), p_wkey, (size_t)S * 8, cudaMemcpyDeviceToHost, st));
-        CBOK(cudaMemcpyAsync(wit.data(), p_wit, (size_t)S * sizeof(CbWitness), cudaMemcpyDeviceToHost, st));
-        CBOK(cudaStreamSynchronize(st));
-        CBOK(cudaEventElapsedTime(&ms, ev0, ev1));
+        cb_check<<<warp_grid, 256, 0, st>>>(d, below, above, wkey);
+        cb_explain<<<sh_grid, 256, 0, st>>>(d, S, wkey, ccidx, ciidx, wit);
+        JTB_OK(cudaGetLastError());
+        JTB_OK(cudaEventRecord(ev1, st));
+        std::vector<unsigned long long> below_h(S), above_h(S), wkey_h(S);
+        std::vector<CbWitness> wit_h(S);
+        JTB_OK(cudaMemcpyAsync(below_h.data(), below, (size_t)S * 8, cudaMemcpyDeviceToHost, st));
+        JTB_OK(cudaMemcpyAsync(above_h.data(), above, (size_t)S * 8, cudaMemcpyDeviceToHost, st));
+        JTB_OK(cudaMemcpyAsync(wkey_h.data(), wkey, (size_t)S * 8, cudaMemcpyDeviceToHost, st));
+        JTB_OK(cudaMemcpyAsync(wit_h.data(), wit, (size_t)S * sizeof(CbWitness), cudaMemcpyDeviceToHost, st));
+        JTB_OK(cudaStreamSynchronize(st));
+        JTB_OK(cudaEventElapsedTime(&ms, ev0, ev1));
         for (int32_t s = 0; s < S; ++s) {
             jtb_cb_shard& o = shards[s];
-            o.n_below = (int64_t)below[s];
-            o.n_above = (int64_t)above[s];
+            o.n_below = (int64_t)below_h[s];
+            o.n_above = (int64_t)above_h[s];
             out->n_violations += o.n_below + o.n_above;
-            if (wkey[s] == ~0ull) continue;
-            const CbWitness& w = wit[s];
+            if (wkey_h[s] == ~0ull) continue;
+            const CbWitness& w = wit_h[s];
             o.valid = JTB_INVALID;
             o.witness_index = h->index[H.r_ev[w.read]];
             o.witness_key = w.key;
@@ -406,14 +357,8 @@ inline int run_counter_bounds(cudaStream_t st, cudaEvent_t ev0, cudaEvent_t ev1,
             o.bound = w.bound;
         }
     }
-    for (int32_t s = 0; s < S; ++s) {
-        out->valid = std::max(out->valid, shards[s].valid);
-        if (shards[s].valid != JTB_VALID) out->n_failures++;
-    }
-    out->seconds_kernel = ms * 1e-3;
-    out->seconds_total = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+    roll_up(out, shards, S, ms, t0);
     return 0;
 }
-#undef CBOK
 
 }  // namespace jtb

@@ -26,6 +26,7 @@
 #include <cuda_runtime.h>
 
 #include "../../include/jtb_check.h"
+#include "jtb_call.cuh"
 
 namespace jtb {
 
@@ -64,6 +65,21 @@ struct MonoDev {
     const int64_t* V = nullptr;
 };
 
+// A shard's key table (MonoHost::keys, kt[0, K), ascending): the column of key, i.e. the first c with kt[c] >= key
+__host__ __device__ __forceinline__ int32_t mono_col(const int32_t* kt, int32_t K, int32_t key) {
+    int32_t a = 0, b = K;
+    while (a < b) {
+        const int32_t c = (a + b) >> 1;
+        if (kt[c] < key) a = c + 1; else b = c;
+    }
+    return a;
+}
+
+// the int64 a payload stores as two int32 words, the low word first
+__host__ __device__ __forceinline__ int64_t mono_join(int32_t lo, int32_t hi) {
+    return (int64_t)(((uint64_t)(uint32_t)hi << 32) | (uint32_t)lo);
+}
+
 __device__ __forceinline__ void mono_add128(uint64_t& lo, uint64_t& hi, uint64_t blo, uint64_t bhi) {
     const uint64_t l = lo + blo;
     hi = hi + bhi + (l < lo ? 1ull : 0ull);
@@ -87,13 +103,8 @@ __global__ void mono_scatter(int32_t m, const int32_t* __restrict__ payload, con
     uint64_t lo = 0, hi = 0;
     for (int32_t j = lane; j < K; j += 32) {
         const int32_t key = p[3 * j];
-        const int64_t v = (int64_t)(((uint64_t)(uint32_t)p[3 * j + 2] << 32) | (uint32_t)p[3 * j + 1]);
-        int32_t a = 0, b = K;   // lower_bound: the host checked that every key is in the table
-        while (a < b) {
-            const int32_t c = (a + b) >> 1;
-            if (kt[c] < key) a = c + 1; else b = c;
-        }
-        vr[a] = v;
+        const int64_t v = mono_join(p[3 * j + 1], p[3 * j + 2]);
+        vr[mono_col(kt, K, key)] = v;   // the host checked that every key is in the table
         mono_add128(lo, hi, (uint64_t)v, v < 0 ? ~0ull : 0ull);
     }
     for (int o = 16; o; o >>= 1) {
@@ -216,7 +227,6 @@ inline int mono_host_pass(const jtb_history* h, MonoHost& H, std::string& err) {
     std::unordered_map<int32_t, int64_t> last_map;
     std::unordered_map<int32_t, int32_t> col_of;
     std::vector<int32_t> prov, hint, seen;
-    char buf[256];
     for (int32_t s = 0; s < S; ++s) {
         const int64_t lo = h->shard_off[s], hi = h->shard_off[s + 1];
         if (lo < 0 || hi < lo || hi > h->n_events) { err = "shard_off is not a CSR partition of the events"; return -2; }
@@ -241,16 +251,10 @@ inline int mono_host_pass(const jtb_history* h, MonoHost& H, std::string& err) {
             const int32_t inv = (li >= 0 && (li >> 32) == s) ? (int32_t)(li & 0xffffffff) : -1;
             const int32_t len = h->payload_len[e];
             const int64_t off = h->payload_off[e];
-            if (len % 3 != 0) {
-                snprintf(buf, sizeof buf, "read at :index %d: payload length %d is not a multiple of 3", h->index[e], len);
-                err = buf;
-                return -2;
-            }
-            if (off < 0 || off + len > h->n_payload) {
-                snprintf(buf, sizeof buf, "read at :index %d: payload out of range", h->index[e]);
-                err = buf;
-                return -2;
-            }
+            if (len % 3 != 0)
+                return input_error(err, "read at :index %d: payload length %d is not a multiple of 3", h->index[e], len);
+            if (off < 0 || off + len > h->n_payload)
+                return input_error(err, "read at :index %d: payload out of range", h->index[e]);
             if (H.r_shard.size() >= (size_t)INT_MAX) { err = "more than 2^31-1 reads"; return -2; }
             const int32_t rid = (int32_t)H.r_shard.size(), nt = len / 3;
             const int32_t* p3 = h->payload + off;
@@ -268,11 +272,8 @@ inline int mono_host_pass(const jtb_history* h, MonoHost& H, std::string& err) {
                     } else col = it->second;
                     if (j < (int32_t)hint.size()) hint[j] = col; else hint.push_back(col);
                 }
-                if (seen[col] == rid) {
-                    snprintf(buf, sizeof buf, "read at :index %d observes key %d twice", h->index[e], key);
-                    err = buf;
-                    return -2;
-                }
+                if (seen[col] == rid)
+                    return input_error(err, "read at :index %d observes key %d twice", h->index[e], key);
                 seen[col] = rid;
             }
             H.r_shard.push_back(s);
@@ -300,10 +301,7 @@ inline void mono_row(const jtb_history* h, const MonoHost& H, int32_t r, std::ve
     const int32_t* kt = H.keys.data() + H.key_off[s];
     out.assign(K, 0);
     const int32_t* p = h->payload + H.r_poff[r];
-    for (int32_t j = 0; j < H.r_ntrip[r]; ++j) {
-        const int32_t c = (int32_t)(std::lower_bound(kt, kt + K, p[3 * j]) - kt);
-        out[c] = (int64_t)(((uint64_t)(uint32_t)p[3 * j + 2] << 32) | (uint32_t)p[3 * j + 1]);
-    }
+    for (int32_t j = 0; j < H.r_ntrip[r]; ++j) out[mono_col(kt, K, p[3 * j])] = mono_join(p[3 * j + 1], p[3 * j + 2]);
 }
 
 // the explanation of the edge x -> y: the smallest key with a strict increase, else real time
@@ -332,35 +330,11 @@ inline void mono_explain(const jtb_history* h, const MonoHost& H, int32_t x, int
     }
 }
 
-#define MOK(call)                                                                                         \
-    do {                                                                                                  \
-        cudaError_t e_ = (call);                                                                          \
-        if (e_ != cudaSuccess) { err = std::string(#call) + ": " + cudaGetErrorString(e_); return -1; }  \
-    } while (0)
-
-// device allocations of one call, released on every return path
-struct MonoAllocs {
-    std::vector<void*> ptrs;
-    ~MonoAllocs() { for (void* p : ptrs) cudaFree(p); }
-    cudaError_t get(void** p, size_t bytes) {
-        *p = nullptr;
-        cudaError_t e = cudaMalloc(p, std::max<size_t>(bytes, 16));
-        if (e == cudaSuccess) ptrs.push_back(*p);
-        else (void)cudaGetLastError();
-        return e;
-    }
-};
-
 inline int run_monotonic_keys(cudaStream_t st, cudaEvent_t ev0, cudaEvent_t ev1, const jtb_history* h, int32_t flags,
                               jtb_mono_shard* shards, jtb_mono_result* out, std::string& err) {
     const auto t0 = std::chrono::steady_clock::now();
     if (!h || !shards || !out) { err = "null argument"; return -2; }
-    if (h->n_events < 0 || h->n_shards < 0 || (h->n_events > 0 && (!h->type || !h->f || !h->process || !h->index ||
-                                                                  !h->payload_off || !h->payload_len)) ||
-        !h->shard_off || (h->n_payload > 0 && !h->payload)) {
-        err = "malformed jtb_history";
-        return -2;
-    }
+    if (int rc = check_history(h, false, err)) return rc;
     const int realtime = !(flags & JTB_MONO_NO_REALTIME);
     const int32_t S = h->n_shards;
     MonoHost H;
@@ -402,76 +376,66 @@ inline int run_monotonic_keys(cudaStream_t st, cudaEvent_t ev0, cudaEvent_t ev1,
     const int32_t m = (int32_t)d_of.size();
     float ms_a = 0, ms_b = 0;
     if (m > 0) {
-        MonoAllocs A;
-        const size_t v_bytes = (size_t)cells * sizeof(int64_t);
-        void *p_payload, *p_poff, *p_shard, *p_inv, *p_comp, *p_cidx, *p_row, *p_nk, *p_koff, *p_keys, *p_V, *p_key0,
-            *p_key1, *p_id0, *p_id1, *p_rev, *p_scan, *p_bound, *p_bad, *p_lo, *p_hi, *p_wit, *p_pkey, *p_tmp;
-        if (A.get(&p_V, v_bytes) != cudaSuccess) {
-            err = "cannot allocate the dense value matrix (" + std::to_string(v_bytes) + " bytes on the device)";
-            return -3;
-        }
-        MOK(A.get(&p_payload, (size_t)h->n_payload * 4));
-        MOK(A.get(&p_poff, (size_t)m * 8)); MOK(A.get(&p_row, (size_t)m * 8));
-        MOK(A.get(&p_shard, (size_t)m * 4)); MOK(A.get(&p_inv, (size_t)m * 4)); MOK(A.get(&p_comp, (size_t)m * 4));
-        MOK(A.get(&p_cidx, (size_t)m * 4));
-        MOK(A.get(&p_nk, (size_t)S * 4)); MOK(A.get(&p_koff, ((size_t)S + 1) * 8));
-        MOK(A.get(&p_keys, H.keys.size() * 4));
-        MOK(A.get(&p_key0, (size_t)m * sizeof(MonoKey))); MOK(A.get(&p_key1, (size_t)m * sizeof(MonoKey)));
-        MOK(A.get(&p_id0, (size_t)m * 4)); MOK(A.get(&p_id1, (size_t)m * 4));
-        MOK(A.get(&p_rev, (size_t)m * sizeof(MonoSuffix))); MOK(A.get(&p_scan, (size_t)m * sizeof(MonoSuffix)));
-        MOK(A.get(&p_bound, (size_t)S * 4)); MOK(A.get(&p_bad, (size_t)S * 4));
-        MOK(A.get(&p_lo, (size_t)S * 4)); MOK(A.get(&p_hi, (size_t)S * 4)); MOK(A.get(&p_wit, (size_t)S * 4));
-        MOK(A.get(&p_pkey, (size_t)S * 8));
-        size_t tmp_sort = 0, tmp_scan = 0;
-        MOK(cub::DeviceRadixSort::SortPairs(nullptr, tmp_sort, (MonoKey*)p_key0, (MonoKey*)p_key1, (int32_t*)p_id0,
-                                            (int32_t*)p_id1, m, MonoKeyDecomposer{}, st));
-        MOK(cub::DeviceScan::InclusiveScan(nullptr, tmp_scan, (MonoSuffix*)p_rev, (MonoSuffix*)p_scan, MonoSuffixMin{}, m,
-                                           st));
-        const size_t tmp_bytes = std::max(tmp_sort, tmp_scan);
-        MOK(A.get(&p_tmp, tmp_bytes));
-        auto up = [&](void* d, const void* src, size_t bytes) {
-            return bytes ? cudaMemcpyAsync(d, src, bytes, cudaMemcpyHostToDevice, st) : cudaSuccess;
-        };
-        MOK(up(p_payload, h->payload, (size_t)h->n_payload * 4));
-        MOK(up(p_poff, poff_v.data(), (size_t)m * 8)); MOK(up(p_row, row_v.data(), (size_t)m * 8));
-        MOK(up(p_shard, shard_v.data(), (size_t)m * 4)); MOK(up(p_inv, inv_v.data(), (size_t)m * 4));
-        MOK(up(p_comp, comp_v.data(), (size_t)m * 4)); MOK(up(p_cidx, cidx_v.data(), (size_t)m * 4));
-        MOK(up(p_nk, H.n_keys.data(), (size_t)S * 4)); MOK(up(p_koff, H.key_off.data(), ((size_t)S + 1) * 8));
-        MOK(up(p_keys, H.keys.data(), H.keys.size() * 4));
-
+        CallAllocs A;
         MonoDev d;
         d.m = m;
-        d.shard = (const int32_t*)p_shard; d.inv = (const int32_t*)p_inv; d.comp = (const int32_t*)p_comp;
-        d.row = (const int64_t*)p_row; d.n_keys = (const int32_t*)p_nk; d.ord = (const int32_t*)p_id1;
-        d.V = (const int64_t*)p_V;
-        int32_t* bound = (int32_t*)p_bound;
-        int32_t* bad = (int32_t*)p_bad;
+        int64_t* V;
+        if (A.alloc(&V, (size_t)cells) != cudaSuccess) {
+            err = "cannot allocate the dense value matrix (" + std::to_string((size_t)cells * sizeof(int64_t)) +
+                  " bytes on the device)";
+            return -3;
+        }
+        d.V = V;
+        const int32_t *payload, *cidx, *keys;
+        const int64_t *poff, *key_off;
+        MonoKey *key0, *key1;
+        MonoSuffix *rev, *scan;
+        int32_t *id0, *id1, *bound, *bad, *lo, *hi, *wit;
+        unsigned long long* pkey;
+        uint8_t* tmp;
+        JTB_OK(A.put(&payload, h->payload, (size_t)h->n_payload, st));
+        JTB_OK(A.put(&poff, poff_v, st)); JTB_OK(A.put(&d.row, row_v, st));
+        JTB_OK(A.put(&d.shard, shard_v, st)); JTB_OK(A.put(&d.inv, inv_v, st)); JTB_OK(A.put(&d.comp, comp_v, st));
+        JTB_OK(A.put(&cidx, cidx_v, st));
+        JTB_OK(A.put(&d.n_keys, H.n_keys, st)); JTB_OK(A.put(&key_off, H.key_off, st));
+        JTB_OK(A.put(&keys, H.keys, st));
+        JTB_OK(A.alloc(&key0, m)); JTB_OK(A.alloc(&key1, m));
+        JTB_OK(A.alloc(&id0, m)); JTB_OK(A.alloc(&id1, m));
+        JTB_OK(A.alloc(&rev, m)); JTB_OK(A.alloc(&scan, m));
+        JTB_OK(A.alloc(&bound, S)); JTB_OK(A.alloc(&bad, S));
+        JTB_OK(A.alloc(&lo, S)); JTB_OK(A.alloc(&hi, S)); JTB_OK(A.alloc(&wit, S));
+        JTB_OK(A.alloc(&pkey, S));
+        d.ord = id1;
+        size_t tmp_sort = 0, tmp_scan = 0;
+        JTB_OK(cub::DeviceRadixSort::SortPairs(nullptr, tmp_sort, key0, key1, id0, id1, m, MonoKeyDecomposer{}, st));
+        JTB_OK(cub::DeviceScan::InclusiveScan(nullptr, tmp_scan, rev, scan, MonoSuffixMin{}, m, st));
+        const size_t tmp_bytes = std::max(tmp_sort, tmp_scan);
+        JTB_OK(A.alloc(&tmp, tmp_bytes));
+
         const unsigned warp_grid = (unsigned)(((int64_t)m * 32 + 255) / 256);
         const unsigned thr_grid = (unsigned)(((int64_t)m + 255) / 256);
         const unsigned sh_grid = (unsigned)((S + 255) / 256);
         auto decide = [&]() -> int {
-            mono_suffix_init<<<thr_grid, 256, 0, st>>>(d, bound, (MonoSuffix*)p_rev);
+            mono_suffix_init<<<thr_grid, 256, 0, st>>>(d, bound, rev);
             size_t tb = tmp_bytes;
-            MOK(cub::DeviceScan::InclusiveScan(p_tmp, tb, (MonoSuffix*)p_rev, (MonoSuffix*)p_scan, MonoSuffixMin{}, m, st));
-            mono_check<<<warp_grid, 256, 0, st>>>(d, bound, (const MonoSuffix*)p_scan, realtime, bad);
+            JTB_OK(cub::DeviceScan::InclusiveScan(tmp, tb, rev, scan, MonoSuffixMin{}, m, st));
+            mono_check<<<warp_grid, 256, 0, st>>>(d, bound, scan, realtime, bad);
             return 0;
         };
 
-        MOK(cudaEventRecord(ev0, st));
-        mono_scatter<<<warp_grid, 256, 0, st>>>(m, (const int32_t*)p_payload, (const int64_t*)p_poff, d.shard, d.inv,
-                                                d.row, d.n_keys, (const int64_t*)p_koff, (const int32_t*)p_keys,
-                                                (int64_t*)p_V, (MonoKey*)p_key0, (int32_t*)p_id0);
+        JTB_OK(cudaEventRecord(ev0, st));
+        mono_scatter<<<warp_grid, 256, 0, st>>>(m, payload, poff, d.shard, d.inv, d.row, d.n_keys, key_off, keys, V,
+                                                key0, id0);
         size_t tb = tmp_bytes;
-        MOK(cub::DeviceRadixSort::SortPairs(p_tmp, tb, (MonoKey*)p_key0, (MonoKey*)p_key1, (int32_t*)p_id0,
-                                            (int32_t*)p_id1, m, MonoKeyDecomposer{}, st));
+        JTB_OK(cub::DeviceRadixSort::SortPairs(tmp, tb, key0, key1, id0, id1, m, MonoKeyDecomposer{}, st));
         mono_bound_all<<<sh_grid, 256, 0, st>>>(S, bound, bad);
         if (decide()) return -1;
-        MOK(cudaGetLastError());
-        MOK(cudaEventRecord(ev1, st));
+        JTB_OK(cudaGetLastError());
+        JTB_OK(cudaEventRecord(ev1, st));
         std::vector<int32_t> bad_h(S, 0);
-        MOK(cudaMemcpyAsync(bad_h.data(), bad, (size_t)S * 4, cudaMemcpyDeviceToHost, st));
-        MOK(cudaStreamSynchronize(st));
-        MOK(cudaEventElapsedTime(&ms_a, ev0, ev1));
+        JTB_OK(cudaMemcpyAsync(bad_h.data(), bad, (size_t)S * 4, cudaMemcpyDeviceToHost, st));
+        JTB_OK(cudaStreamSynchronize(st));
+        JTB_OK(cudaEventElapsedTime(&ms_a, ev0, ev1));
 
         // witness and partner of the INVALID shards
         std::vector<int32_t> lo_h(S, 0), hi_h(S, 0);
@@ -487,33 +451,32 @@ inline int run_monotonic_keys(cudaStream_t st, cudaEvent_t ev0, cudaEvent_t ev1,
         if (any) {
             int rounds = 0;
             while ((1ll << rounds) < widest) ++rounds;
-            MOK(cudaEventRecord(ev0, st));
-            MOK(up(p_lo, lo_h.data(), (size_t)S * 4));
-            MOK(up(p_hi, hi_h.data(), (size_t)S * 4));
+            JTB_OK(cudaEventRecord(ev0, st));
+            JTB_OK(cudaMemcpyAsync(lo, lo_h.data(), (size_t)S * 4, cudaMemcpyHostToDevice, st));
+            JTB_OK(cudaMemcpyAsync(hi, hi_h.data(), (size_t)S * 4, cudaMemcpyHostToDevice, st));
             for (int k = 0; k < rounds; ++k) {
-                mono_bound_mid<<<sh_grid, 256, 0, st>>>(S, (const int32_t*)p_lo, (const int32_t*)p_hi, bound, bad);
+                mono_bound_mid<<<sh_grid, 256, 0, st>>>(S, lo, hi, bound, bad);
                 if (decide()) return -1;
-                mono_bound_update<<<sh_grid, 256, 0, st>>>(S, (int32_t*)p_lo, (int32_t*)p_hi, bound, bad);
+                mono_bound_update<<<sh_grid, 256, 0, st>>>(S, lo, hi, bound, bad);
             }
             // wpos: the converged bound of an INVALID shard, -1 elsewhere
             std::vector<int32_t> wpos(S, -1);
-            MOK(cudaMemcpyAsync(lo_h.data(), p_lo, (size_t)S * 4, cudaMemcpyDeviceToHost, st));
-            MOK(cudaStreamSynchronize(st));
+            JTB_OK(cudaMemcpyAsync(lo_h.data(), lo, (size_t)S * 4, cudaMemcpyDeviceToHost, st));
+            JTB_OK(cudaStreamSynchronize(st));
             for (int32_t s = 0; s < S; ++s)
                 if (shards[s].valid == JTB_INVALID && dev[s]) wpos[s] = lo_h[s];
-            MOK(up(p_lo, wpos.data(), (size_t)S * 4));
-            MOK(cudaMemsetAsync(p_pkey, 0xff, (size_t)S * 8, st));
-            mono_find_witness<<<thr_grid, 256, 0, st>>>(d, (const int32_t*)p_lo, (int32_t*)p_wit);
-            mono_partner<<<thr_grid, 256, 0, st>>>(d, (const int32_t*)p_lo, (const int32_t*)p_wit,
-                                                   (const int32_t*)p_cidx, realtime, (unsigned long long*)p_pkey);
-            MOK(cudaGetLastError());
-            MOK(cudaEventRecord(ev1, st));
+            JTB_OK(cudaMemcpyAsync(lo, wpos.data(), (size_t)S * 4, cudaMemcpyHostToDevice, st));
+            JTB_OK(cudaMemsetAsync(pkey, 0xff, (size_t)S * 8, st));
+            mono_find_witness<<<thr_grid, 256, 0, st>>>(d, lo, wit);
+            mono_partner<<<thr_grid, 256, 0, st>>>(d, lo, wit, cidx, realtime, pkey);
+            JTB_OK(cudaGetLastError());
+            JTB_OK(cudaEventRecord(ev1, st));
             std::vector<int32_t> wit_h(S, -1);
             std::vector<unsigned long long> pkey_h(S, ~0ull);
-            MOK(cudaMemcpyAsync(wit_h.data(), p_wit, (size_t)S * 4, cudaMemcpyDeviceToHost, st));
-            MOK(cudaMemcpyAsync(pkey_h.data(), p_pkey, (size_t)S * 8, cudaMemcpyDeviceToHost, st));
-            MOK(cudaStreamSynchronize(st));
-            MOK(cudaEventElapsedTime(&ms_b, ev0, ev1));
+            JTB_OK(cudaMemcpyAsync(wit_h.data(), wit, (size_t)S * 4, cudaMemcpyDeviceToHost, st));
+            JTB_OK(cudaMemcpyAsync(pkey_h.data(), pkey, (size_t)S * 8, cudaMemcpyDeviceToHost, st));
+            JTB_OK(cudaStreamSynchronize(st));
+            JTB_OK(cudaEventElapsedTime(&ms_b, ev0, ev1));
             for (int32_t s = 0; s < S; ++s) {
                 if (wpos[s] < 0) continue;
                 jtb_mono_shard& o = shards[s];
@@ -526,14 +489,8 @@ inline int run_monotonic_keys(cudaStream_t st, cudaEvent_t ev0, cudaEvent_t ev1,
             }
         }
     }
-    for (int32_t s = 0; s < S; ++s) {
-        out->valid = std::max(out->valid, shards[s].valid);
-        if (shards[s].valid != JTB_VALID) out->n_failures++;
-    }
-    out->seconds_kernel = (ms_a + ms_b) * 1e-3;
-    out->seconds_total = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+    roll_up(out, shards, S, ms_a + ms_b, t0);
     return 0;
 }
-#undef MOK
 
 }  // namespace jtb

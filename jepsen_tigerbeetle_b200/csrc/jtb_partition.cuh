@@ -6,10 +6,13 @@
 //    i-th event of the partitioned history; events of one key keep their history order (stable sort).
 //  * ledger->bank (tests/ledger.clj:100-105): a read's `{:credits-posted c :debits-posted d}` -> balance c - d, elementwise.
 #pragma once
+#include <algorithm>
 #include <cstdint>
 #include <string>
 #include <cub/cub.cuh>
 #include <cuda_runtime.h>
+
+#include "jtb_call.cuh"
 
 namespace jtb {
 
@@ -35,64 +38,56 @@ __global__ void pt_balances(const int64_t* __restrict__ credits, const int64_t* 
     if (i < n) out[i] = (int32_t)(credits[i] - debits[i]);
 }
 
-#define PTK(call)                                                                          \
-    do {                                                                                   \
-        cudaError_t e_ = (call);                                                           \
-        if (e_ != cudaSuccess) { err = std::string(#call) + ": " + cudaGetErrorString(e_); free_all(); return -1; } \
-    } while (0)
-
 inline int run_partition_by_key(cudaStream_t st, int64_t n, const int64_t* event_key, int32_t* order, int64_t* shard_off,
                                 int64_t* key_ids, int32_t key_cap, int32_t* n_keys, std::string& err) {
-    void *d_key = nullptr, *d_k0 = nullptr, *d_k1 = nullptr, *d_i0 = nullptr, *d_i1 = nullptr, *d_head = nullptr, *d_run = nullptr,
-         *d_off = nullptr, *d_ids = nullptr, *d_tmp = nullptr;
-    auto free_all = [&]() { for (void* p : {d_key, d_k0, d_k1, d_i0, d_i1, d_head, d_run, d_off, d_ids, d_tmp}) if (p) cudaFree(p); };
     *n_keys = 0;
     if (n <= 0) { if (key_cap >= 0) shard_off[0] = 0; return 0; }
     if (n >= (1ll << 31)) { err = "too many events"; return -2; }
     const unsigned grid = (unsigned)((n + 255) / 256);
-    PTK(cudaMalloc(&d_key, n * 8)); PTK(cudaMalloc(&d_k0, n * 8)); PTK(cudaMalloc(&d_k1, n * 8));
-    PTK(cudaMalloc(&d_i0, n * 4)); PTK(cudaMalloc(&d_i1, n * 4)); PTK(cudaMalloc(&d_head, n * 4)); PTK(cudaMalloc(&d_run, n * 4));
-    PTK(cudaMalloc(&d_off, ((size_t)key_cap + 1) * 8)); PTK(cudaMalloc(&d_ids, ((size_t)key_cap + 1) * 8));
-    PTK(cudaMemcpyAsync(d_key, event_key, n * 8, cudaMemcpyHostToDevice, st));
-    pt_init<<<grid, 256, 0, st>>>((const int64_t*)d_key, n, (uint64_t*)d_k0, (int32_t*)d_i0);
+    CallAllocs A;
+    const int64_t* d_key;
+    uint64_t *d_k0, *d_k1;
+    int32_t *d_i0, *d_i1, *d_head, *d_run;
+    int64_t *d_off, *d_ids;
+    uint8_t* d_tmp;
+    JTB_OK(A.put(&d_key, event_key, (size_t)n, st)); JTB_OK(A.alloc(&d_k0, n)); JTB_OK(A.alloc(&d_k1, n));
+    JTB_OK(A.alloc(&d_i0, n)); JTB_OK(A.alloc(&d_i1, n)); JTB_OK(A.alloc(&d_head, n)); JTB_OK(A.alloc(&d_run, n));
+    JTB_OK(A.alloc(&d_off, (size_t)key_cap + 1)); JTB_OK(A.alloc(&d_ids, (size_t)key_cap + 1));
+    pt_init<<<grid, 256, 0, st>>>(d_key, n, d_k0, d_i0);
     size_t tmp_sort = 0, tmp_scan = 0;
-    PTK(cub::DeviceRadixSort::SortPairs(nullptr, tmp_sort, (const uint64_t*)d_k0, (uint64_t*)d_k1, (const int32_t*)d_i0, (int32_t*)d_i1, (int)n, 0, 64, st));
-    PTK(cub::DeviceScan::InclusiveSum(nullptr, tmp_scan, (const int32_t*)d_head, (int32_t*)d_run, (int)n, st));
-    PTK(cudaMalloc(&d_tmp, std::max(tmp_sort, tmp_scan)));
+    JTB_OK(cub::DeviceRadixSort::SortPairs(nullptr, tmp_sort, (const uint64_t*)d_k0, d_k1, (const int32_t*)d_i0, d_i1, (int)n, 0, 64, st));
+    JTB_OK(cub::DeviceScan::InclusiveSum(nullptr, tmp_scan, (const int32_t*)d_head, d_run, (int)n, st));
+    JTB_OK(A.alloc(&d_tmp, std::max(tmp_sort, tmp_scan)));
     size_t tb = std::max(tmp_sort, tmp_scan);
-    PTK(cub::DeviceRadixSort::SortPairs(d_tmp, tb, (const uint64_t*)d_k0, (uint64_t*)d_k1, (const int32_t*)d_i0, (int32_t*)d_i1, (int)n, 0, 64, st));
-    pt_heads<<<grid, 256, 0, st>>>((const uint64_t*)d_k1, n, (int32_t*)d_head);
+    JTB_OK(cub::DeviceRadixSort::SortPairs(d_tmp, tb, (const uint64_t*)d_k0, d_k1, (const int32_t*)d_i0, d_i1, (int)n, 0, 64, st));
+    pt_heads<<<grid, 256, 0, st>>>(d_k1, n, d_head);
     tb = std::max(tmp_sort, tmp_scan);
-    PTK(cub::DeviceScan::InclusiveSum(d_tmp, tb, (const int32_t*)d_head, (int32_t*)d_run, (int)n, st));
-    pt_emit<<<grid, 256, 0, st>>>((const uint64_t*)d_k1, (const int32_t*)d_head, (const int32_t*)d_run, n, (int64_t*)d_off, (int64_t*)d_ids, key_cap);
-    PTK(cudaGetLastError());
+    JTB_OK(cub::DeviceScan::InclusiveSum(d_tmp, tb, (const int32_t*)d_head, d_run, (int)n, st));
+    pt_emit<<<grid, 256, 0, st>>>(d_k1, d_head, d_run, n, d_off, d_ids, key_cap);
+    JTB_OK(cudaGetLastError());
     int32_t total = 0;
-    PTK(cudaMemcpyAsync(&total, (int32_t*)d_run + (n - 1), 4, cudaMemcpyDeviceToHost, st));
-    PTK(cudaMemcpyAsync(order, d_i1, n * 4, cudaMemcpyDeviceToHost, st));
-    PTK(cudaStreamSynchronize(st));
-    if (total > key_cap) { err = "key_cap too small"; free_all(); return -4; }
-    PTK(cudaMemcpy(shard_off, d_off, (size_t)total * 8, cudaMemcpyDeviceToHost));
-    PTK(cudaMemcpy(key_ids, d_ids, (size_t)total * 8, cudaMemcpyDeviceToHost));
+    JTB_OK(cudaMemcpyAsync(&total, d_run + (n - 1), 4, cudaMemcpyDeviceToHost, st));
+    JTB_OK(cudaMemcpyAsync(order, d_i1, n * 4, cudaMemcpyDeviceToHost, st));
+    JTB_OK(cudaStreamSynchronize(st));
+    if (total > key_cap) { err = "key_cap too small"; return -4; }
+    JTB_OK(cudaMemcpy(shard_off, d_off, (size_t)total * 8, cudaMemcpyDeviceToHost));
+    JTB_OK(cudaMemcpy(key_ids, d_ids, (size_t)total * 8, cudaMemcpyDeviceToHost));
     shard_off[total] = n;
     *n_keys = total;
-    free_all();
     return 0;
 }
 
 inline int run_ledger_balances(cudaStream_t st, int64_t n, const int64_t* credits, const int64_t* debits, int32_t* out, std::string& err) {
-    void *d_c = nullptr, *d_d = nullptr, *d_o = nullptr;
-    auto free_all = [&]() { for (void* p : {d_c, d_d, d_o}) if (p) cudaFree(p); };
     if (n <= 0) return 0;
-    PTK(cudaMalloc(&d_c, n * 8)); PTK(cudaMalloc(&d_d, n * 8)); PTK(cudaMalloc(&d_o, n * 4));
-    PTK(cudaMemcpyAsync(d_c, credits, n * 8, cudaMemcpyHostToDevice, st));
-    PTK(cudaMemcpyAsync(d_d, debits, n * 8, cudaMemcpyHostToDevice, st));
-    pt_balances<<<(unsigned)((n + 255) / 256), 256, 0, st>>>((const int64_t*)d_c, (const int64_t*)d_d, n, (int32_t*)d_o);
-    PTK(cudaGetLastError());
-    PTK(cudaMemcpyAsync(out, d_o, n * 4, cudaMemcpyDeviceToHost, st));
-    PTK(cudaStreamSynchronize(st));
-    free_all();
+    CallAllocs A;
+    const int64_t *d_c, *d_d;
+    int32_t* d_o;
+    JTB_OK(A.put(&d_c, credits, (size_t)n, st)); JTB_OK(A.put(&d_d, debits, (size_t)n, st)); JTB_OK(A.alloc(&d_o, n));
+    pt_balances<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d_c, d_d, n, d_o);
+    JTB_OK(cudaGetLastError());
+    JTB_OK(cudaMemcpyAsync(out, d_o, n * 4, cudaMemcpyDeviceToHost, st));
+    JTB_OK(cudaStreamSynchronize(st));
     return 0;
 }
-#undef PTK
 
 }  // namespace jtb

@@ -23,6 +23,7 @@
 #include <cuda_runtime.h>
 
 #include "../../include/jtb_check.h"
+#include "jtb_call.cuh"
 
 namespace jtb {
 
@@ -291,15 +292,6 @@ struct SfBuffers {
     void release() { for (auto& x : b) { if (x.p) cudaFree(x.p); x = Buf(); } }
 };
 
-#define SFK(call)                                                                  \
-    do {                                                                           \
-        cudaError_t e_ = (call);                                                   \
-        if (e_ != cudaSuccess) {                                                   \
-            err = std::string(#call) + ": " + cudaGetErrorString(e_);              \
-            return -1;                                                             \
-        }                                                                          \
-    } while (0)
-
 inline int run_set_full(cudaStream_t st, cudaEvent_t e0, cudaEvent_t e1, SfBuffers& B, const jtb_history* h,
                         int linearizable, jtb_setfull_out* out, std::string& err, unsigned long long* stats) {
     const double t_start = std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count();
@@ -407,7 +399,11 @@ inline int run_set_full(cudaStream_t st, cudaEvent_t e0, cudaEvent_t e1, SfBuffe
         if (bytes > x.cap) {
             if (x.p) cudaFree(x.p);
             x.p = nullptr; x.cap = 0;
-            if (cudaMalloc(&x.p, bytes + bytes / 8) != cudaSuccess) { x.p = nullptr; return nullptr; }
+            if (cudaMalloc(&x.p, bytes + bytes / 8) != cudaSuccess) {
+                x.p = nullptr;
+                (void)cudaGetLastError();   // the refusal would otherwise stay behind as the thread's last error
+                return nullptr;
+            }
             x.cap = bytes + bytes / 8;
         }
         return x.p;
@@ -437,72 +433,72 @@ inline int run_set_full(cudaStream_t st, cudaEvent_t e0, cudaEvent_t e1, SfBuffe
         h2d += bytes;
         return bytes ? cudaMemcpyAsync(d, src, bytes, cudaMemcpyHostToDevice, st) : cudaSuccess;
     };
-    SFK(cudaMemsetAsync(d_missing, 0, std::max<size_t>(n_reads * 4, 16), st));
-    SFK(up(d_shards, shards.data(), n_shards * sizeof(SfShard)));
-    SFK(up(d_elems, elems.data(), n_elems * sizeof(SfElem)));
-    SFK(up(d_elem_shard, elem_shard.data(), n_elems * 4));
-    SFK(up(d_reads, reads.data(), n_reads * sizeof(SfRead)));
-    SFK(up(d_lut, lut.data(), lut.size() * 4));
-    SFK(up(d_sorted, sorted.data(), sorted.size() * sizeof(int2)));
-    SFK(up(d_order, order_desc.data(), order_desc.size() * 4));
+    JTB_OK(cudaMemsetAsync(d_missing, 0, std::max<size_t>(n_reads * 4, 16), st));
+    JTB_OK(up(d_shards, shards.data(), n_shards * sizeof(SfShard)));
+    JTB_OK(up(d_elems, elems.data(), n_elems * sizeof(SfElem)));
+    JTB_OK(up(d_elem_shard, elem_shard.data(), n_elems * 4));
+    JTB_OK(up(d_reads, reads.data(), n_reads * sizeof(SfRead)));
+    JTB_OK(up(d_lut, lut.data(), lut.size() * 4));
+    JTB_OK(up(d_sorted, sorted.data(), sorted.size() * sizeof(int2)));
+    JTB_OK(up(d_order, order_desc.data(), order_desc.size() * 4));
     // the id lists: a true DMA when the caller's buffer is page-locked (jtb_host_alloc / cudaHostRegister), staged
     // through the driver's bounce buffer otherwise
-    SFK(up(d_payload, h->payload, (size_t)h->n_payload * 4));
-    SFK(cudaEventRecord(e0, st));
-    SFK(cudaMemsetAsync(d_bits, 0, std::max<size_t>((size_t)bits_words * 4, 16), st));
-    SFK(cudaMemsetAsync(d_flag, 0, std::max<size_t>(n_reads * 4, 16), st));
-    SFK(cudaMemsetAsync(d_tally, 0, std::max<size_t>(n_shards * sizeof(SfShardOut), 16), st));
+    JTB_OK(up(d_payload, h->payload, (size_t)h->n_payload * 4));
+    JTB_OK(cudaEventRecord(e0, st));
+    JTB_OK(cudaMemsetAsync(d_bits, 0, std::max<size_t>((size_t)bits_words * 4, 16), st));
+    JTB_OK(cudaMemsetAsync(d_flag, 0, std::max<size_t>(n_reads * 4, 16), st));
+    JTB_OK(cudaMemsetAsync(d_tally, 0, std::max<size_t>(n_shards * sizeof(SfShardOut), 16), st));
     int launches = 0;
     std::vector<int> flag((size_t)n_reads, 0);
     if (n_elems > 0) {
         sf_init_acc<<<(unsigned)((n_elems + 255) / 256), 256, 0, st>>>(d_acc, n_elems);
-        SFK(cudaGetLastError());
+        JTB_OK(cudaGetLastError());
         ++launches;
     }
     if (n_reads > 0 && n_elems > 0) {
         const int64_t threads = n_reads * 32;
         sf_build_bits<<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(d_reads, n_reads, d_shards, d_lut, d_sorted, d_payload, d_bits, d_flag);
-        SFK(cudaGetLastError());
+        JTB_OK(cudaGetLastError());
         int max_w = 0, max_r = 0;
         for (auto& sd : shards) { max_w = std::max(max_w, sd.words_per_row); max_r = std::max(max_r, sd.n_reads); }
         dim3 grid((max_w + 127) / 128, (max_r + SF_RCHUNK - 1) / SF_RCHUNK, n_shards);
         sf_column_scan<<<grid, 128, 0, st>>>(d_reads, d_shards, d_order, d_bits, d_acc);
-        SFK(cudaGetLastError());
+        JTB_OK(cudaGetLastError());
         sf_final_missing<<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(d_reads, n_reads, d_shards, d_bits, d_missing);
-        SFK(cudaGetLastError());
+        JTB_OK(cudaGetLastError());
         launches += 3;
         // duplicates (rare): exact multiplicities for flagged reads
-        SFK(cudaMemcpyAsync(flag.data(), d_flag, n_reads * 4, cudaMemcpyDeviceToHost, st));
-        SFK(cudaStreamSynchronize(st));
+        JTB_OK(cudaMemcpyAsync(flag.data(), d_flag, n_reads * 4, cudaMemcpyDeviceToHost, st));
+        JTB_OK(cudaStreamSynchronize(st));
         std::vector<int> flagged;
         for (int64_t r = 0; r < n_reads; ++r) if (flag[r] & 1) flagged.push_back((int)r);
         if (!flagged.empty()) {
-            SFK(cudaMemcpyAsync(d_flagged, flagged.data(), flagged.size() * 4, cudaMemcpyHostToDevice, st));
+            JTB_OK(cudaMemcpyAsync(d_flagged, flagged.data(), flagged.size() * 4, cudaMemcpyHostToDevice, st));
             sf_count_dups<<<(unsigned)flagged.size(), 128, 0, st>>>(d_reads, d_flagged, (int)flagged.size(), d_shards, d_lut, d_sorted, d_payload, d_acc);
-            SFK(cudaGetLastError());
+            JTB_OK(cudaGetLastError());
             ++launches;
         }
     }
     if (n_elems > 0) {
         sf_classify<<<(unsigned)((n_elems + 255) / 256), 256, 0, st>>>(d_reads, d_shards, d_elems, d_acc, n_elems, d_elem_shard,
                                                                       d_outcome, d_lat, d_dup, d_id, d_tally);
-        SFK(cudaGetLastError());
+        JTB_OK(cudaGetLastError());
         ++launches;
     }
-    SFK(cudaEventRecord(e1, st));
+    JTB_OK(cudaEventRecord(e1, st));
     std::vector<SfShardOut> tally(n_shards);
-    SFK(cudaMemcpyAsync(tally.data(), d_tally, n_shards * sizeof(SfShardOut), cudaMemcpyDeviceToHost, st));
+    JTB_OK(cudaMemcpyAsync(tally.data(), d_tally, n_shards * sizeof(SfShardOut), cudaMemcpyDeviceToHost, st));
     if (out->elem_capacity > 0 && n_elems > 0) {
-        SFK(cudaMemcpyAsync(out->elem_outcome, d_outcome, n_elems, cudaMemcpyDeviceToHost, st));
-        SFK(cudaMemcpyAsync(out->elem_latency_ms, d_lat, n_elems * 8, cudaMemcpyDeviceToHost, st));
-        SFK(cudaMemcpyAsync(out->elem_dup_count, d_dup, n_elems * 4, cudaMemcpyDeviceToHost, st));
-        SFK(cudaMemcpyAsync(out->elem_id, d_id, n_elems * 4, cudaMemcpyDeviceToHost, st));
+        JTB_OK(cudaMemcpyAsync(out->elem_outcome, d_outcome, n_elems, cudaMemcpyDeviceToHost, st));
+        JTB_OK(cudaMemcpyAsync(out->elem_latency_ms, d_lat, n_elems * 8, cudaMemcpyDeviceToHost, st));
+        JTB_OK(cudaMemcpyAsync(out->elem_dup_count, d_dup, n_elems * 4, cudaMemcpyDeviceToHost, st));
+        JTB_OK(cudaMemcpyAsync(out->elem_id, d_id, n_elems * 4, cudaMemcpyDeviceToHost, st));
     }
     std::vector<int> h_missing((size_t)n_reads, 0);
-    if (n_reads > 0) SFK(cudaMemcpyAsync(h_missing.data(), d_missing, n_reads * 4, cudaMemcpyDeviceToHost, st));
-    SFK(cudaStreamSynchronize(st));
+    if (n_reads > 0) JTB_OK(cudaMemcpyAsync(h_missing.data(), d_missing, n_reads * 4, cudaMemcpyDeviceToHost, st));
+    JTB_OK(cudaStreamSynchronize(st));
     float ms = 0;
-    SFK(cudaEventElapsedTime(&ms, e0, e1));
+    JTB_OK(cudaEventElapsedTime(&ms, e0, e1));
     // ids that were never :add-invoked in their key but occur twice in one read: jepsen counts (frequencies v) over
     // every value of a read, so they are :duplicated too.  Such reads are flagged by stage A (never in a healthy
     // history); their id lists are counted here.
@@ -551,7 +547,7 @@ inline int run_set_full(cudaStream_t st, cudaEvent_t e0, cudaEvent_t e1, SfBuffe
                 }
                 const SfShard& sd = shards[s];
                 rowbits.resize(sd.words_per_row);
-                SFK(cudaMemcpy(rowbits.data(), d_bits + sd.bits_off + (r - sd.read_off) * (int64_t)sd.words_per_row,
+                JTB_OK(cudaMemcpy(rowbits.data(), d_bits + sd.bits_off + (r - sd.read_off) * (int64_t)sd.words_per_row,
                                (size_t)sd.words_per_row * 4, cudaMemcpyDeviceToHost));
                 out->suspect_shard[out->n_suspect] = s;
                 out->suspect_index[out->n_suspect] = reads[r].ok_idx;
@@ -596,18 +592,6 @@ inline int run_set_full(cudaStream_t st, cudaEvent_t e0, cudaEvent_t e1, SfBuffe
     }
     return 0;
 }
-#undef SFK
-
-#define SCK(call)                                                                  \
-    do {                                                                           \
-        cudaError_t e_ = (call);                                                   \
-        if (e_ != cudaSuccess) {                                                   \
-            err = std::string(#call) + ": " + cudaGetErrorString(e_);              \
-            cleanup();                                                             \
-            return -1;                                                             \
-        }                                                                          \
-    } while (0)
-
 // =================================================================================================
 // bank totals
 // =================================================================================================
@@ -688,40 +672,37 @@ inline int run_bank_totals(cudaStream_t st, cudaEvent_t e0, cudaEvent_t e1, cons
         reads.push_back(BkRead{h->payload_off[e], std::max(0, (int)h->payload_len[e]), h->index[e]});
     }
     const int64_t n = (int64_t)reads.size();
-    BkRead* d_reads = nullptr; int32_t* d_payload = nullptr; uint8_t* d_type = nullptr; BkAgg* d_agg = nullptr;
-    auto cleanup = [&]() { cudaFree(d_reads); cudaFree(d_payload); cudaFree(d_type); cudaFree(d_agg); };
-    auto nz = [](size_t b) { return b ? b : (size_t)16; };
-    SCK(cudaMalloc(&d_reads, nz(n * sizeof(BkRead))));
-    SCK(cudaMalloc(&d_payload, nz((size_t)h->n_payload * 4)));
-    SCK(cudaMalloc(&d_type, nz(n)));
-    SCK(cudaMalloc(&d_agg, sizeof(BkAgg)));
+    CallAllocs A;
+    const BkRead* d_reads; const int32_t* d_payload; uint8_t* d_type; BkAgg* d_agg;
+    JTB_OK(A.put(&d_reads, reads, st));
+    JTB_OK(A.put(&d_payload, h->payload, (size_t)h->n_payload, st));
+    JTB_OK(A.alloc(&d_type, (size_t)n));
+    JTB_OK(A.alloc(&d_agg, 1));
     BkAgg init;
     std::memset(&init, 0, sizeof init);
     for (int t = 0; t < 5; ++t) { init.first_idx[t] = 0x7fffffff; init.last_idx[t] = -1; init.worst_idx[t] = 0x7fffffff; }
     init.lowest = INT64_MAX; init.highest = INT64_MIN;
     init.lowest_idx = init.highest_idx = init.first_error_idx = 0x7fffffff;
-    SCK(cudaMemcpyAsync(d_reads, reads.data(), n * sizeof(BkRead), cudaMemcpyHostToDevice, st));
-    SCK(cudaMemcpyAsync(d_payload, h->payload, (size_t)h->n_payload * 4, cudaMemcpyHostToDevice, st));
-    SCK(cudaMemcpyAsync(d_agg, &init, sizeof init, cudaMemcpyHostToDevice, st));
+    JTB_OK(cudaMemcpyAsync(d_agg, &init, sizeof init, cudaMemcpyHostToDevice, st));
     int ids[8] = {0, 0, 0, 0, 0, 0, 0, 0};
     for (int i = 0; i < m->n_accounts && i < 8; ++i) ids[i] = m->account_ids[i];
     const int4 lo = make_int4(ids[0], ids[1], ids[2], ids[3]), hi = make_int4(ids[4], ids[5], ids[6], ids[7]);
-    SCK(cudaEventRecord(e0, st));
+    JTB_OK(cudaEventRecord(e0, st));
     if (n > 0) {
         for (int pass = 0; pass < 2; ++pass) {
             bk_scan<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d_reads, n, d_payload, m->n_accounts, lo, hi, total_amount,
                                                                  m->negative_balances_ok, pass, d_type, d_agg);
-            SCK(cudaGetLastError());
+            JTB_OK(cudaGetLastError());
         }
     }
-    SCK(cudaEventRecord(e1, st));
+    JTB_OK(cudaEventRecord(e1, st));
     BkAgg agg;
-    SCK(cudaMemcpyAsync(&agg, d_agg, sizeof agg, cudaMemcpyDeviceToHost, st));
+    JTB_OK(cudaMemcpyAsync(&agg, d_agg, sizeof agg, cudaMemcpyDeviceToHost, st));
     std::vector<uint8_t> types((size_t)n);
-    SCK(cudaMemcpyAsync(types.data(), d_type, n, cudaMemcpyDeviceToHost, st));
-    SCK(cudaStreamSynchronize(st));
+    JTB_OK(cudaMemcpyAsync(types.data(), d_type, n, cudaMemcpyDeviceToHost, st));
+    JTB_OK(cudaStreamSynchronize(st));
     float ms = 0;
-    SCK(cudaEventElapsedTime(&ms, e0, e1));
+    JTB_OK(cudaEventElapsedTime(&ms, e0, e1));
     std::memset(out, 0, sizeof *out);
     out->read_count = n;
     out->first_error_index = -1;
@@ -749,7 +730,6 @@ inline int run_bank_totals(cudaStream_t st, cudaEvent_t e0, cudaEvent_t e1, cons
         out->reference_throws = 1;
         out->valid = JTB_UNKNOWN;
     }
-    cleanup();
     out->seconds_kernel = ms * 1e-3;
     out->seconds_total = std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count() - t_start;
     return 0;

@@ -32,6 +32,7 @@
 #include <cuda_runtime.h>
 
 #include "../../include/jtb_check.h"
+#include "jtb_call.cuh"
 #include "jtb_monotonic.cuh"
 
 namespace jtb {
@@ -114,10 +115,6 @@ struct TlDev {
     unsigned long long* wop = nullptr;    // [n_shards] (completion << 32 | op), op = lookup or 0x80000000 | read
 };
 
-__device__ __forceinline__ int64_t tl_id(const int32_t* r) {
-    return (int64_t)(((uint64_t)(uint32_t)r[1] << 32) | (uint32_t)r[0]);
-}
-
 // sorted slot of id in shard s, -1 when no transfer invoke carries it
 __device__ __forceinline__ int32_t tl_find(const TlDev& d, int32_t s, uint64_t idu) {
     int32_t a = d.t_off[s], b = d.t_off[s + 1];
@@ -131,7 +128,7 @@ __device__ __forceinline__ int32_t tl_find(const TlDev& d, int32_t s, uint64_t i
 // column of key in shard s's key table, -1 when no read observes it
 __device__ __forceinline__ int32_t tl_col(const TlDev& d, int32_t s, int64_t key) {
     const int32_t* kt = d.keys + d.key_off[s];
-    int32_t a = 0, b = d.n_keys[s];
+    int32_t a = 0, b = d.n_keys[s];   // mono_col's search for an int64 key: 2 * account + 1 may leave the int32 range
     while (a < b) {
         const int32_t c = (a + b) >> 1;
         if (kt[c] < key) a = c + 1; else b = c;
@@ -171,7 +168,7 @@ __global__ void tl_records(TlDev d, TlRKey* __restrict__ rkey, int32_t* __restri
     if (g >= d.n_rec) return;
     const int32_t l = tl_lookup_of(d, g), s = d.l_shard[l];
     const int32_t* r = tl_rec(d, l, g);
-    const uint64_t idu = (uint64_t)tl_id(r) ^ TL_SIGN;
+    const uint64_t idu = (uint64_t)mono_join(r[0], r[1]) ^ TL_SIGN;
     const int32_t slot = tl_find(d, s, idu);
     d.rec_slot[g] = slot;
     rkey[g] = TlRKey{(uint32_t)l, idu};
@@ -288,10 +285,6 @@ __device__ __forceinline__ void tl_span(const TlDev& d, int32_t r, int32_t s, in
     ja = a;
 }
 
-__device__ __forceinline__ int64_t tl_value(const int32_t* p) {
-    return (int64_t)(((uint64_t)(uint32_t)p[2] << 32) | (uint32_t)p[1]);
-}
-
 // warp per read, lane per triple: BELOW against P of the last lookup completed before it, ABOVE against N of the
 // first lookup invoked after it
 __global__ void tl_reads(TlDev d) {
@@ -307,7 +300,7 @@ __global__ void tl_reads(TlDev d) {
     unsigned below = 0, above = 0;
     for (int32_t j = lane; j < nt; j += 32) {
         const int32_t col = tl_col(d, s, p[3 * j]);
-        const int64_t v = tl_value(p + 3 * j);
+        const int64_t v = mono_join(p[3 * j + 1], p[3 * j + 2]);
         below += nb > 0 && v < d.P[prow + col];
         above += ja < d.ib_off[s + 1] && v > d.N[nrow + col];
     }
@@ -356,7 +349,7 @@ __global__ void tl_explain(TlDev d, int32_t n_shards, TlWitness* __restrict__ ou
     int32_t bcol = INT_MAX, acol = INT_MAX;
     for (int32_t j = 0; j < d.ntrip[r]; ++j) {
         const int32_t col = tl_col(d, s, p[3 * j]);
-        const int64_t v = tl_value(p + 3 * j);
+        const int64_t v = mono_join(p[3 * j + 1], p[3 * j + 2]);
         if (nb > 0 && v < d.P[prow + col]) bcol = min(bcol, col);
         if (ja < d.ib_off[s + 1] && v > d.N[nrow + col]) acol = min(acol, col);
     }
@@ -364,7 +357,7 @@ __global__ void tl_explain(TlDev d, int32_t n_shards, TlWitness* __restrict__ ou
     const int32_t col = below ? bcol : acol, key = d.keys[d.key_off[s] + col];
     int64_t v = 0;
     for (int32_t j = 0; j < d.ntrip[r]; ++j)
-        if (p[3 * j] == key) v = tl_value(p + 3 * j);
+        if (p[3 * j] == key) v = mono_join(p[3 * j + 1], p[3 * j + 2]);
     o.kind = below ? JTB_TL_READ_BELOW_LOOKUP : JTB_TL_READ_ABOVE_LOOKUP;
     o.key = key;
     o.value = v;
@@ -423,13 +416,6 @@ struct TlHost {
     std::vector<int32_t> ib, ib_inv, ib_off;
 };
 
-inline int tl_fail(std::string& err, const char* what, int32_t index, long long x = 0) {
-    char buf[256];
-    snprintf(buf, sizeof buf, what, index, x);
-    err = buf;
-    return -2;
-}
-
 // Pair every transfer micro-op with the next event of its process and every :ok lookup with the latest invoke of its
 // process, validate them, and lay out the transfer table and the lookups' record offsets.
 inline int tl_host_pass(const jtb_history* h, TlHost& T, std::string& err) {
@@ -464,22 +450,23 @@ inline int tl_host_pass(const jtb_history* h, TlHost& T, std::string& err) {
             if (h->type[e] == JTB_T_INVOKE) {
                 last_inv[p] = pos;
                 if (h->f[e] != JTB_F_TRANSFER) continue;
-                if (len <= 0) return tl_fail(err, "transfer at :index %d: an invoke without ids", h->index[e]);
+                if (len <= 0) return input_error(err, "transfer at :index %d: an invoke without ids", h->index[e]);
                 if (len % 5 != 0)
-                    return tl_fail(err, "transfer at :index %d: payload length %lld is not a multiple of 5", h->index[e],
-                                   len);
+                    return input_error(err, "transfer at :index %d: payload length %d is not a multiple of 5",
+                                       h->index[e], len);
                 if (off < 0 || off + len > h->n_payload)
-                    return tl_fail(err, "transfer at :index %d: payload out of range", h->index[e]);
+                    return input_error(err, "transfer at :index %d: payload out of range", h->index[e]);
                 const size_t first = T.t_id.size();
                 for (int32_t j = 0; j < len; j += 5) {
                     const int32_t* r = h->payload + off + j;
-                    if (r[4] < 0) return tl_fail(err, "transfer at :index %d: negative amount %lld", h->index[e], r[4]);
+                    if (r[4] < 0)
+                        return input_error(err, "transfer at :index %d: negative amount %d", h->index[e], r[4]);
                     if (r[2] < 0 || r[2] >= (1 << 30) || r[3] < 0 || r[3] >= (1 << 30))
-                        return tl_fail(err, "transfer at :index %d: account outside [0, 2^30)", h->index[e]);
-                    const int64_t id = (int64_t)(((uint64_t)(uint32_t)r[1] << 32) | (uint32_t)r[0]);
+                        return input_error(err, "transfer at :index %d: account outside [0, 2^30)", h->index[e]);
+                    const int64_t id = mono_join(r[0], r[1]);
                     if (!ids.insert(id).second)
-                        return tl_fail(err, "transfer at :index %d: id %lld is carried by two transfer invokes",
-                                       h->index[e], id);
+                        return input_error(err, "transfer at :index %d: id %lld is carried by two transfer invokes",
+                                           h->index[e], (long long)id);
                     if (T.t_id.size() >= (size_t)INT_MAX) { err = "more than 2^31-1 transfers"; return -2; }
                     T.t_shard.push_back(s);
                     T.t_id.push_back(id);
@@ -495,9 +482,10 @@ inline int tl_host_pass(const jtb_history* h, TlHost& T, std::string& err) {
             }
             if (h->type[e] != JTB_T_OK || h->f[e] != JTB_F_LOOKUP || len < 0) continue;
             if (len % 5 != 0)
-                return tl_fail(err, "lookup at :index %d: payload length %lld is not a multiple of 5", h->index[e], len);
+                return input_error(err, "lookup at :index %d: payload length %d is not a multiple of 5", h->index[e],
+                                   len);
             if (off < 0 || off + len > h->n_payload)
-                return tl_fail(err, "lookup at :index %d: payload out of range", h->index[e]);
+                return input_error(err, "lookup at :index %d: payload out of range", h->index[e]);
             if (T.rec_base.back() + len / 5 > INT_MAX) { err = "more than 2^31-1 lookup records"; return -2; }
             auto it = last_inv.find(p);
             T.l_shard.push_back(s);
@@ -520,23 +508,12 @@ inline int tl_host_pass(const jtb_history* h, TlHost& T, std::string& err) {
     return 0;
 }
 
-#define TLOK(call)                                                                                        \
-    do {                                                                                                  \
-        cudaError_t e_ = (call);                                                                          \
-        if (e_ != cudaSuccess) { err = std::string(#call) + ": " + cudaGetErrorString(e_); return -1; }  \
-    } while (0)
-
 inline int run_transfer_lookups(cudaStream_t st, cudaEvent_t ev0, cudaEvent_t ev1, const jtb_history* h,
                                 int32_t flags, jtb_tl_shard* shards, jtb_tl_result* out, std::string& err) {
     const auto t0 = std::chrono::steady_clock::now();
     if (!h || !shards || !out) { err = "null argument"; return -2; }
     if (flags != 0) { err = "flags must be 0 (reserved)"; return -2; }
-    if (h->n_events < 0 || h->n_shards < 0 || (h->n_events > 0 && (!h->type || !h->f || !h->process || !h->index ||
-                                                                  !h->payload_off || !h->payload_len)) ||
-        !h->shard_off || (h->n_payload > 0 && !h->payload)) {
-        err = "malformed jtb_history";
-        return -2;
-    }
+    if (int rc = check_history(h, false, err)) return rc;
     const int32_t S = h->n_shards;
     MonoHost H;
     if (int rc = mono_host_pass(h, H, err)) return rc;
@@ -570,153 +547,109 @@ inline int run_transfer_lookups(cudaStream_t st, cudaEvent_t ev0, cudaEvent_t ev
     const int64_t nR = T.rec_base.back();
     float ms = 0;
     if (nL > 0) {   // without an :ok lookup nothing can be violated
-        MonoAllocs A;
+        CallAllocs A;
         const size_t slots = H.keys.size();
         std::vector<int32_t> slot_shard(slots), r_cidx(m);
         for (int32_t s = 0; s < S; ++s)
             for (int64_t q = H.key_off[s]; q < H.key_off[s + 1]; ++q) slot_shard[q] = s;
         for (int32_t r = 0; r < m; ++r) r_cidx[r] = h->index[H.r_ev[r]];
-        void *p_payload, *p_poff, *p_ntrip, *p_rshard, *p_rinv, *p_rcomp, *p_rcidx, *p_nk, *p_koff, *p_keys, *p_sshard;
-        void *p_tshard, *p_tid, *p_trec, *p_tinv, *p_tok, *p_tfate, *p_tiidx, *p_tcidx, *p_toff, *p_tk0, *p_tk,
-            *p_tid0, *p_tperm;
-        void *p_lshard, *p_linv, *p_lcomp, *p_lcidx, *p_lpoff, *p_rbase, *p_lkoff, *p_ib, *p_ibinv, *p_iboff, *p_sbase,
-            *p_ibase;
-        void *p_rslot, *p_rk0, *p_rk, *p_rv0, *p_rv, *p_mlk, *p_mv, *p_mfrom, *p_mk0, *p_mk, *p_have, *p_wid,
-            *p_lcode, *p_S, *p_P, *p_N, *p_count, *p_wop, *p_wit, *p_mid, *p_tmp;
-        TLOK(A.get(&p_payload, (size_t)h->n_payload * 4));
-        TLOK(A.get(&p_poff, (size_t)m * 8)); TLOK(A.get(&p_ntrip, (size_t)m * 4)); TLOK(A.get(&p_rshard, (size_t)m * 4));
-        TLOK(A.get(&p_rinv, (size_t)m * 4)); TLOK(A.get(&p_rcomp, (size_t)m * 4)); TLOK(A.get(&p_rcidx, (size_t)m * 4));
-        TLOK(A.get(&p_nk, (size_t)S * 4)); TLOK(A.get(&p_koff, ((size_t)S + 1) * 8)); TLOK(A.get(&p_keys, slots * 4));
-        TLOK(A.get(&p_sshard, slots * 4));
-        TLOK(A.get(&p_tshard, (size_t)nT * 4)); TLOK(A.get(&p_tid, (size_t)nT * 8)); TLOK(A.get(&p_trec, (size_t)nT * 12));
-        TLOK(A.get(&p_tinv, (size_t)nT * 4)); TLOK(A.get(&p_tok, (size_t)nT * 4)); TLOK(A.get(&p_tfate, (size_t)nT * 4));
-        TLOK(A.get(&p_tiidx, (size_t)nT * 4)); TLOK(A.get(&p_tcidx, (size_t)nT * 4));
-        TLOK(A.get(&p_toff, ((size_t)S + 1) * 4));
-        TLOK(A.get(&p_tk0, (size_t)nT * sizeof(TlTKey))); TLOK(A.get(&p_tk, (size_t)nT * sizeof(TlTKey)));
-        TLOK(A.get(&p_tid0, (size_t)nT * 4)); TLOK(A.get(&p_tperm, (size_t)nT * 4));
-        TLOK(A.get(&p_lshard, (size_t)nL * 4)); TLOK(A.get(&p_linv, (size_t)nL * 4)); TLOK(A.get(&p_lcomp, (size_t)nL * 4));
-        TLOK(A.get(&p_lcidx, (size_t)nL * 4)); TLOK(A.get(&p_lpoff, (size_t)nL * 8));
-        TLOK(A.get(&p_rbase, ((size_t)nL + 1) * 8)); TLOK(A.get(&p_lkoff, ((size_t)S + 1) * 4));
-        TLOK(A.get(&p_ib, T.ib.size() * 4)); TLOK(A.get(&p_ibinv, T.ib.size() * 4));
-        TLOK(A.get(&p_iboff, ((size_t)S + 1) * 4)); TLOK(A.get(&p_sbase, (size_t)S * 8));
-        TLOK(A.get(&p_ibase, (size_t)S * 8));
-        TLOK(A.get(&p_rslot, (size_t)nR * 4));
-        TLOK(A.get(&p_rk0, (size_t)nR * sizeof(TlRKey))); TLOK(A.get(&p_rk, (size_t)nR * sizeof(TlRKey)));
-        TLOK(A.get(&p_rv0, (size_t)nR * 4)); TLOK(A.get(&p_rv, (size_t)nR * 4));
-        TLOK(A.get(&p_mlk, (size_t)nT * 4)); TLOK(A.get(&p_mv, (size_t)nT * 4)); TLOK(A.get(&p_mfrom, (size_t)nT * 4));
-        TLOK(A.get(&p_mk0, (size_t)nT * 8)); TLOK(A.get(&p_mk, (size_t)nT * 8));
-        TLOK(A.get(&p_have, (size_t)nL * 16)); TLOK(A.get(&p_wid, (size_t)nL * 40)); TLOK(A.get(&p_lcode, (size_t)nL * 4));
-        if (A.get(&p_S, (size_t)s_rows * 8) != cudaSuccess || A.get(&p_P, (size_t)s_rows * 8) != cudaSuccess ||
-            A.get(&p_N, (size_t)i_rows * 8) != cudaSuccess) {
-            char buf[160];
-            snprintf(buf, sizeof buf, "the S matrix (%lld lookup x observed-key sums) does not fit on the device",
-                     (long long)s_rows);
-            err = buf;
-            return -2;
-        }
-        TLOK(A.get(&p_count, (size_t)S * JTB_TL_KINDS * 8)); TLOK(A.get(&p_wop, (size_t)S * 8));
-        TLOK(A.get(&p_wit, (size_t)S * sizeof(TlWitness))); TLOK(A.get(&p_mid, (size_t)S * 8));
+        TlDev d;
+        d.n_t = nT;
+        d.n_l = nL;
+        d.m = m;
+        d.n_rec = nR;
+        const int32_t* sshard;
+        const int64_t* tid;
+        TlTKey *tk0, *tk;
+        TlRKey *rk0, *rk;
+        int32_t *tid0, *tperm, *rv0, *rv;
+        uint64_t *mk0, *mk;
+        TlWitness* wit;
+        unsigned long long* mid;
+        uint8_t* tmp;
+        JTB_OK(A.put(&d.payload, h->payload, (size_t)h->n_payload, st));
+        JTB_OK(A.put(&d.poff, H.r_poff, st)); JTB_OK(A.put(&d.ntrip, H.r_ntrip, st)); JTB_OK(A.put(&d.r_shard, H.r_shard, st));
+        JTB_OK(A.put(&d.r_inv, H.r_inv, st)); JTB_OK(A.put(&d.r_comp, H.r_comp, st)); JTB_OK(A.put(&d.r_cidx, r_cidx, st));
+        JTB_OK(A.put(&d.n_keys, H.n_keys, st)); JTB_OK(A.put(&d.key_off, H.key_off, st)); JTB_OK(A.put(&d.keys, H.keys, st));
+        JTB_OK(A.put(&sshard, slot_shard, st));
+        JTB_OK(A.put(&d.t_shard, T.t_shard, st)); JTB_OK(A.put(&tid, T.t_id, st)); JTB_OK(A.put(&d.t_rec, T.t_rec, st));
+        JTB_OK(A.put(&d.t_inv, T.t_inv, st)); JTB_OK(A.put(&d.t_okcomp, T.t_okcomp, st));
+        JTB_OK(A.put(&d.t_fate, T.t_fate, st)); JTB_OK(A.put(&d.t_iidx, T.t_iidx, st));
+        JTB_OK(A.put(&d.t_cidx, T.t_cidx, st)); JTB_OK(A.put(&d.t_off, T.t_off, st));
+        JTB_OK(A.alloc(&tk0, nT)); JTB_OK(A.alloc(&tk, nT));
+        JTB_OK(A.alloc(&tid0, nT)); JTB_OK(A.alloc(&tperm, nT));
+        JTB_OK(A.put(&d.l_shard, T.l_shard, st)); JTB_OK(A.put(&d.l_inv, T.l_inv, st)); JTB_OK(A.put(&d.l_comp, T.l_comp, st));
+        JTB_OK(A.put(&d.l_cidx, T.l_cidx, st)); JTB_OK(A.put(&d.l_poff, T.l_poff, st));
+        JTB_OK(A.put(&d.rec_base, T.rec_base, st)); JTB_OK(A.put(&d.lk_off, T.lk_off, st));
+        JTB_OK(A.put(&d.ib, T.ib, st)); JTB_OK(A.put(&d.ib_inv, T.ib_inv, st));
+        JTB_OK(A.put(&d.ib_off, T.ib_off, st)); JTB_OK(A.put(&d.s_base, s_base, st));
+        JTB_OK(A.put(&d.i_base, i_base, st));
+        JTB_OK(A.alloc(&d.rec_slot, nR));
+        JTB_OK(A.alloc(&rk0, nR)); JTB_OK(A.alloc(&rk, nR));
+        JTB_OK(A.alloc(&rv0, nR)); JTB_OK(A.alloc(&rv, nR));
+        JTB_OK(A.alloc(&d.mlk, nT)); JTB_OK(A.alloc(&d.mv, nT)); JTB_OK(A.alloc(&d.mfrom, nT));
+        JTB_OK(A.alloc(&mk0, nT)); JTB_OK(A.alloc(&mk, nT));
+        JTB_OK(A.alloc(&d.have, (size_t)nL * 2)); JTB_OK(A.alloc(&d.wid, (size_t)nL * 5)); JTB_OK(A.alloc(&d.lk_code, nL));
+        if (A.alloc(&d.S, (size_t)s_rows) != cudaSuccess || A.alloc(&d.P, (size_t)s_rows) != cudaSuccess ||
+            A.alloc(&d.N, (size_t)i_rows) != cudaSuccess)
+            return input_error(err, "the S matrix (%lld lookup x observed-key sums) does not fit on the device",
+                               (long long)s_rows);
+        JTB_OK(A.alloc(&d.count, (size_t)S * JTB_TL_KINDS)); JTB_OK(A.alloc(&d.wop, S));
+        JTB_OK(A.alloc(&wit, S)); JTB_OK(A.alloc(&mid, S));
+        d.tkey = tk; d.tperm = tperm;
+        d.rkey = rk; d.rval = rv;
+        d.msort = mk;
         size_t tmp_t = 0, tmp_r = 0, tmp_m = 0;
         if (nT > 0) {
-            TLOK(cub::DeviceRadixSort::SortPairs(nullptr, tmp_t, (TlTKey*)p_tk0, (TlTKey*)p_tk, (int32_t*)p_tid0,
-                                                 (int32_t*)p_tperm, nT, TlTKeyDecomposer{}, st));
-            TLOK(cub::DeviceRadixSort::SortKeys(nullptr, tmp_m, (uint64_t*)p_mk0, (uint64_t*)p_mk, nT, 0, 64, st));
+            JTB_OK(cub::DeviceRadixSort::SortPairs(nullptr, tmp_t, tk0, tk, tid0, tperm, nT, TlTKeyDecomposer{}, st));
+            JTB_OK(cub::DeviceRadixSort::SortKeys(nullptr, tmp_m, mk0, mk, nT, 0, 64, st));
         }
         if (nR > 0)
-            TLOK(cub::DeviceRadixSort::SortPairs(nullptr, tmp_r, (TlRKey*)p_rk0, (TlRKey*)p_rk, (int32_t*)p_rv0,
-                                                 (int32_t*)p_rv, (int)nR, TlRKeyDecomposer{}, st));
+            JTB_OK(cub::DeviceRadixSort::SortPairs(nullptr, tmp_r, rk0, rk, rv0, rv, (int)nR, TlRKeyDecomposer{}, st));
         const size_t tmp_bytes = std::max({tmp_t, tmp_r, tmp_m});
-        TLOK(A.get(&p_tmp, tmp_bytes));
-        auto up = [&](void* dst, const void* src, size_t bytes) {
-            return bytes ? cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, st) : cudaSuccess;
-        };
-        TLOK(up(p_payload, h->payload, (size_t)h->n_payload * 4));
-        TLOK(up(p_poff, H.r_poff.data(), (size_t)m * 8)); TLOK(up(p_ntrip, H.r_ntrip.data(), (size_t)m * 4));
-        TLOK(up(p_rshard, H.r_shard.data(), (size_t)m * 4)); TLOK(up(p_rinv, H.r_inv.data(), (size_t)m * 4));
-        TLOK(up(p_rcomp, H.r_comp.data(), (size_t)m * 4)); TLOK(up(p_rcidx, r_cidx.data(), (size_t)m * 4));
-        TLOK(up(p_nk, H.n_keys.data(), (size_t)S * 4)); TLOK(up(p_koff, H.key_off.data(), ((size_t)S + 1) * 8));
-        TLOK(up(p_keys, H.keys.data(), slots * 4)); TLOK(up(p_sshard, slot_shard.data(), slots * 4));
-        TLOK(up(p_tshard, T.t_shard.data(), (size_t)nT * 4)); TLOK(up(p_tid, T.t_id.data(), (size_t)nT * 8));
-        TLOK(up(p_trec, T.t_rec.data(), (size_t)nT * 12)); TLOK(up(p_tinv, T.t_inv.data(), (size_t)nT * 4));
-        TLOK(up(p_tok, T.t_okcomp.data(), (size_t)nT * 4)); TLOK(up(p_tfate, T.t_fate.data(), (size_t)nT * 4));
-        TLOK(up(p_tiidx, T.t_iidx.data(), (size_t)nT * 4)); TLOK(up(p_tcidx, T.t_cidx.data(), (size_t)nT * 4));
-        TLOK(up(p_toff, T.t_off.data(), ((size_t)S + 1) * 4));
-        TLOK(up(p_lshard, T.l_shard.data(), (size_t)nL * 4)); TLOK(up(p_linv, T.l_inv.data(), (size_t)nL * 4));
-        TLOK(up(p_lcomp, T.l_comp.data(), (size_t)nL * 4)); TLOK(up(p_lcidx, T.l_cidx.data(), (size_t)nL * 4));
-        TLOK(up(p_lpoff, T.l_poff.data(), (size_t)nL * 8)); TLOK(up(p_rbase, T.rec_base.data(), ((size_t)nL + 1) * 8));
-        TLOK(up(p_lkoff, T.lk_off.data(), ((size_t)S + 1) * 4));
-        TLOK(up(p_ib, T.ib.data(), T.ib.size() * 4)); TLOK(up(p_ibinv, T.ib_inv.data(), T.ib.size() * 4));
-        TLOK(up(p_iboff, T.ib_off.data(), ((size_t)S + 1) * 4));
-        TLOK(up(p_sbase, s_base.data(), (size_t)S * 8)); TLOK(up(p_ibase, i_base.data(), (size_t)S * 8));
-
-        TlDev d;
-        d.payload = (const int32_t*)p_payload;
-        d.n_t = nT;
-        d.tkey = (const TlTKey*)p_tk; d.tperm = (const int32_t*)p_tperm; d.t_shard = (const int32_t*)p_tshard;
-        d.t_rec = (const int32_t*)p_trec; d.t_inv = (const int32_t*)p_tinv; d.t_okcomp = (const int32_t*)p_tok;
-        d.t_fate = (const int32_t*)p_tfate; d.t_iidx = (const int32_t*)p_tiidx; d.t_cidx = (const int32_t*)p_tcidx;
-        d.t_off = (const int32_t*)p_toff;
-        d.n_l = nL;
-        d.l_shard = (const int32_t*)p_lshard; d.l_inv = (const int32_t*)p_linv; d.l_comp = (const int32_t*)p_lcomp;
-        d.l_cidx = (const int32_t*)p_lcidx; d.l_poff = (const int64_t*)p_lpoff; d.rec_base = (const int64_t*)p_rbase;
-        d.lk_off = (const int32_t*)p_lkoff; d.ib = (const int32_t*)p_ib; d.ib_inv = (const int32_t*)p_ibinv;
-        d.ib_off = (const int32_t*)p_iboff; d.s_base = (const int64_t*)p_sbase; d.i_base = (const int64_t*)p_ibase;
-        d.n_keys = (const int32_t*)p_nk; d.key_off = (const int64_t*)p_koff; d.keys = (const int32_t*)p_keys;
-        d.m = m;
-        d.poff = (const int64_t*)p_poff; d.ntrip = (const int32_t*)p_ntrip; d.r_shard = (const int32_t*)p_rshard;
-        d.r_inv = (const int32_t*)p_rinv; d.r_comp = (const int32_t*)p_rcomp; d.r_cidx = (const int32_t*)p_rcidx;
-        d.n_rec = nR;
-        d.rec_slot = (int32_t*)p_rslot; d.rkey = (const TlRKey*)p_rk; d.rval = (const int32_t*)p_rv;
-        d.mlk = (int32_t*)p_mlk; d.mv = (int32_t*)p_mv; d.mfrom = (int32_t*)p_mfrom; d.msort = (const uint64_t*)p_mk;
-        d.have = (unsigned long long*)p_have; d.wid = (unsigned long long*)p_wid; d.lk_code = (int32_t*)p_lcode;
-        d.S = (unsigned long long*)p_S; d.P = (int64_t*)p_P; d.N = (int64_t*)p_N;
-        d.count = (unsigned long long*)p_count; d.wop = (unsigned long long*)p_wop;
+        JTB_OK(A.alloc(&tmp, tmp_bytes));
         auto grid = [](int64_t n, int per) { return (unsigned)((n + per - 1) / per); };
 
-        TLOK(cudaEventRecord(ev0, st));
-        TLOK(cudaMemsetAsync(p_mlk, 0x7f, (size_t)nT * 4, st));   // 0x7f7f7f7f > any lookup id: "none"
-        TLOK(cudaMemsetAsync(p_have, 0, (size_t)nL * 16, st));
-        TLOK(cudaMemsetAsync(p_wid, 0xff, (size_t)nL * 40, st));
-        TLOK(cudaMemsetAsync(p_S, 0, (size_t)s_rows * 8, st));
-        TLOK(cudaMemsetAsync(p_count, 0, (size_t)S * JTB_TL_KINDS * 8, st));
-        TLOK(cudaMemsetAsync(p_wop, 0xff, (size_t)S * 8, st));
-        TLOK(cudaMemsetAsync(p_mid, 0xff, (size_t)S * 8, st));
+        JTB_OK(cudaEventRecord(ev0, st));
+        JTB_OK(cudaMemsetAsync(d.mlk, 0x7f, (size_t)nT * 4, st));   // 0x7f7f7f7f > any lookup id: "none"
+        JTB_OK(cudaMemsetAsync(d.have, 0, (size_t)nL * 16, st));
+        JTB_OK(cudaMemsetAsync(d.wid, 0xff, (size_t)nL * 40, st));
+        JTB_OK(cudaMemsetAsync(d.S, 0, (size_t)s_rows * 8, st));
+        JTB_OK(cudaMemsetAsync(d.count, 0, (size_t)S * JTB_TL_KINDS * 8, st));
+        JTB_OK(cudaMemsetAsync(d.wop, 0xff, (size_t)S * 8, st));
+        JTB_OK(cudaMemsetAsync(mid, 0xff, (size_t)S * 8, st));
         size_t tb;
         if (nT > 0) {
-            tl_tkeys<<<grid(nT, 256), 256, 0, st>>>(nT, (const int32_t*)p_tshard, (const int64_t*)p_tid, (TlTKey*)p_tk0,
-                                                     (int32_t*)p_tid0);
+            tl_tkeys<<<grid(nT, 256), 256, 0, st>>>(nT, d.t_shard, tid, tk0, tid0);
             tb = tmp_bytes;
-            TLOK(cub::DeviceRadixSort::SortPairs(p_tmp, tb, (TlTKey*)p_tk0, (TlTKey*)p_tk, (int32_t*)p_tid0,
-                                                 (int32_t*)p_tperm, nT, TlTKeyDecomposer{}, st));
+            JTB_OK(cub::DeviceRadixSort::SortPairs(tmp, tb, tk0, tk, tid0, tperm, nT, TlTKeyDecomposer{}, st));
         }
         if (nR > 0) {
-            tl_records<<<grid(nR, 256), 256, 0, st>>>(d, (TlRKey*)p_rk0, (int32_t*)p_rv0);
+            tl_records<<<grid(nR, 256), 256, 0, st>>>(d, rk0, rv0);
             tb = tmp_bytes;
-            TLOK(cub::DeviceRadixSort::SortPairs(p_tmp, tb, (TlRKey*)p_rk0, (TlRKey*)p_rk, (int32_t*)p_rv0,
-                                                 (int32_t*)p_rv, (int)nR, TlRKeyDecomposer{}, st));
+            JTB_OK(cub::DeviceRadixSort::SortPairs(tmp, tb, rk0, rk, rv0, rv, (int)nR, TlRKeyDecomposer{}, st));
         }
         if (nT > 0) {
-            tl_mval<<<grid(nT, 256), 256, 0, st>>>(d, (uint64_t*)p_mk0);
+            tl_mval<<<grid(nT, 256), 256, 0, st>>>(d, mk0);
             tb = tmp_bytes;
-            TLOK(cub::DeviceRadixSort::SortKeys(p_tmp, tb, (uint64_t*)p_mk0, (uint64_t*)p_mk, nT, 0, 64, st));
+            JTB_OK(cub::DeviceRadixSort::SortKeys(tmp, tb, mk0, mk, nT, 0, 64, st));
         }
         if (nR > 0) tl_distinct<<<grid(nR, 256), 256, 0, st>>>(d);
         tl_need<<<grid(nL, 128), 128, 0, st>>>(d);
-        if (slots > 0) tl_extremes<<<grid((int64_t)slots, 128), 128, 0, st>>>(d, (int32_t)slots,
-                                                                               (const int32_t*)p_sshard);
+        if (slots > 0) tl_extremes<<<grid((int64_t)slots, 128), 128, 0, st>>>(d, (int32_t)slots, sshard);
         if (m > 0) tl_reads<<<grid((int64_t)m * 32, 256), 256, 0, st>>>(d);
-        tl_explain<<<grid(S, 128), 128, 0, st>>>(d, S, (TlWitness*)p_wit);
-        if (nT > 0) tl_missing<<<grid(nT, 256), 256, 0, st>>>(d, (const TlWitness*)p_wit, (unsigned long long*)p_mid);
-        tl_missing_related<<<grid(S, 128), 128, 0, st>>>(d, S, (const unsigned long long*)p_mid, (TlWitness*)p_wit);
-        TLOK(cudaGetLastError());
-        TLOK(cudaEventRecord(ev1, st));
+        tl_explain<<<grid(S, 128), 128, 0, st>>>(d, S, wit);
+        if (nT > 0) tl_missing<<<grid(nT, 256), 256, 0, st>>>(d, wit, mid);
+        tl_missing_related<<<grid(S, 128), 128, 0, st>>>(d, S, mid, wit);
+        JTB_OK(cudaGetLastError());
+        JTB_OK(cudaEventRecord(ev1, st));
         std::vector<unsigned long long> count((size_t)S * JTB_TL_KINDS), wop(S);
-        std::vector<TlWitness> wit(S);
-        TLOK(cudaMemcpyAsync(count.data(), p_count, count.size() * 8, cudaMemcpyDeviceToHost, st));
-        TLOK(cudaMemcpyAsync(wop.data(), p_wop, (size_t)S * 8, cudaMemcpyDeviceToHost, st));
-        TLOK(cudaMemcpyAsync(wit.data(), p_wit, (size_t)S * sizeof(TlWitness), cudaMemcpyDeviceToHost, st));
-        TLOK(cudaStreamSynchronize(st));
-        TLOK(cudaEventElapsedTime(&ms, ev0, ev1));
+        std::vector<TlWitness> wit_h(S);
+        JTB_OK(cudaMemcpyAsync(count.data(), d.count, count.size() * 8, cudaMemcpyDeviceToHost, st));
+        JTB_OK(cudaMemcpyAsync(wop.data(), d.wop, (size_t)S * 8, cudaMemcpyDeviceToHost, st));
+        JTB_OK(cudaMemcpyAsync(wit_h.data(), wit, (size_t)S * sizeof(TlWitness), cudaMemcpyDeviceToHost, st));
+        JTB_OK(cudaStreamSynchronize(st));
+        JTB_OK(cudaEventElapsedTime(&ms, ev0, ev1));
         for (int32_t s = 0; s < S; ++s) {
             jtb_tl_shard& o = shards[s];
             for (int k = 0; k < JTB_TL_KINDS; ++k) {
@@ -724,7 +657,7 @@ inline int run_transfer_lookups(cudaStream_t st, cudaEvent_t ev0, cudaEvent_t ev
                 out->n_violations += o.count_by_kind[k];
             }
             if (wop[s] == ~0ull) continue;
-            const TlWitness& w = wit[s];
+            const TlWitness& w = wit_h[s];
             o.valid = JTB_INVALID;
             o.witness_index = w.op_cidx;
             o.kind = w.kind;
@@ -735,14 +668,8 @@ inline int run_transfer_lookups(cudaStream_t st, cudaEvent_t ev0, cudaEvent_t ev
             o.bound = w.bound;
         }
     }
-    for (int32_t s = 0; s < S; ++s) {
-        out->valid = std::max(out->valid, shards[s].valid);
-        if (shards[s].valid != JTB_VALID) out->n_failures++;
-    }
-    out->seconds_kernel = ms * 1e-3;
-    out->seconds_total = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+    roll_up(out, shards, S, ms, t0);
     return 0;
 }
-#undef TLOK
 
 }  // namespace jtb

@@ -19,7 +19,7 @@ CSRC = os.path.join(_HERE, "csrc")
 _SOURCES = ["jtb_abi.cu", "jtb_prep.cpp", "jtb_multi.cpp"]
 _DEPS = _SOURCES + ["jtb_prep.h", "jtb_expand.h", "jtb_wgl.cuh", "jtb_scout.cuh", "jtb_scans.cuh",
                     "jtb_table_bench.cuh", "jtb_level.cuh", "jtb_partition.cuh", "jtb_monotonic.cuh",
-                    "jtb_counter_bounds.cuh", "jtb_transfer_lookups.cuh"]
+                    "jtb_counter_bounds.cuh", "jtb_transfer_lookups.cuh", "jtb_call.cuh"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared", "-ldl"]
 
