@@ -441,6 +441,35 @@
                                                           :bound (at (+ s 20)))
                                        (<= 0 rel)  (assoc :related (by-index rel)))))))))
 
+;; ---- read explanations -------------------------------------------------------------------------------------
+(def ^:private rx-kind {1 :key 2 :joint})
+
+(defn read-explanation-checker
+  "Whether one set of transfers explains every counter each :ok read shows, on the GPU: the transfers that must be in
+  the read, the ones that cannot be and the ones that may be, and a budgeted search for a subset of the last that
+  closes every counter at once.  :key errors have a counter no subset closes (lost, phantom, duplicated or corrupt
+  amounts), :joint errors close each counter alone but not all at once (torn or fractured transfers).  A read the
+  budget ({:max-nodes n}) does not decide makes the verdict :unknown.  Add it to the compose map at
+  tests/ledger.clj:363-367 as `:read-explanations (read-explanation-checker {})`.
+  Result: {:valid? :read-count :transfer-count :explained-count :undecided-count :error-count :errors [:op :error]}."
+  [opts]
+  (reify checker/Checker
+    (check [_ _test history _opts]
+      (let [{:keys [arrays by-index]} (flatten-history :ledger-lookups history)
+            res    (Native/checkReadExplanations @ctx arrays (long (:max-nodes opts 0)))
+            at     (fn [i] (aget res (int i)))
+            s      11                                     ; shard 0: valid reads transfers witness explained undecided ...
+            errors (into {} (for [k (range 2) :let [n (at (+ s 6 k))] :when (pos? n)] [(rx-kind (inc k)) n]))
+            kind   (at (+ s 9))
+            key    (at (+ s 10))]
+        (cond-> {:valid? (verdict (at s)) :read-count (at (+ s 1)) :transfer-count (at (+ s 2))
+                 :explained-count (at (+ s 4)) :undecided-count (at (+ s 5)) :error-count (reduce + (vals errors))
+                 :errors errors}
+          (= 2 (at s)) (assoc :op    (by-index (at (+ s 3)))
+                              :error (cond-> {:type (rx-kind kind) :must-count (at (+ s 11)) :may-count (at (+ s 12))}
+                                       (<= 0 key) (assoc :key [(quot key 2) (counter-field (rem key 2))])
+                                       (= 1 kind) (assoc :value (at (+ s 13)) :must-sum (at (+ s 14))))))))))
+
 ;; ---- independent ----------------------------------------------------------------------------------------------
 (defn independent-checker
   "Like (independent/checker (checker/compose checkers)) for a map {name checker-kind} built from THIS namespace's

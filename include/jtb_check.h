@@ -24,7 +24,7 @@
 extern "C" {
 #endif
 
-#define JTB_ABI_VERSION 5
+#define JTB_ABI_VERSION 6
 
 /* ---- verdict lattice (jepsen.checker/merge-valid) ------------------------------------------- */
 #define JTB_VALID   0
@@ -373,6 +373,58 @@ typedef struct jtb_tl_result {
     double  seconds_total;      /* host wall time of the call incl. the host pass, H2D, D2H                           */
 } jtb_tl_result;
 
+/* ---- read-explanation check (DESIGN.md "K10 read-explanation check") -------------------------------------------------
+ * Input: the ledger-lookups form, read exactly as the transfer-lookup check reads it.  Every [:t ...] micro-op is one
+ * transfer with its txn's interval and fate; it adds its amount to key 2*debit+0 and key 2*credit+1.  With M(t) and the
+ * lookups as in K9, and A(t) = the latest invocation of an :ok lookup whose records lack t (-1 when none), every
+ * transfer t of the shard of an :ok read r (invocation iv, completion cp) is in exactly one class:
+ *   must    M(t) < iv (t was :ok, or returned by an :ok lookup, before r was invoked)
+ *   cannot  otherwise, when t's fate is :fail, t was invoked after cp, or A(t) > cp
+ *   may     every other transfer with a nonzero amount on a key r observes
+ * With d_k = v_k(r) - (the must transfers' sum on k), r is explained when some subset X of its "may" transfers has sum
+ * d_k on every key k it observes.  The decision is budgeted, and the budget is deterministic: a read observing more than
+ * JTB_RX_MAX_KEYS keys or with more than JTB_RX_MAX_GATHER "may" transfers, one with more than JTB_RX_MAX_FREE of them
+ * left after the root pruning, and one whose canonical search visits more than max_nodes nodes are UNDECIDED.  A shard
+ * is JTB_INVALID when some read is not explained, else JTB_UNKNOWN when some read is undecided, else JTB_VALID. */
+#define JTB_RX_KEY   1 /* some single observed key has no subset of the "may" transfers summing to d_k             */
+#define JTB_RX_JOINT 2 /* every key alone has one, but no one subset closes all of them (torn / fractured transfers) */
+#define JTB_RX_MAX_KEYS   256
+#define JTB_RX_MAX_GATHER 128
+#define JTB_RX_MAX_FREE   64
+#define JTB_RX_DEFAULT_MAX_NODES 4096 /* max_nodes <= 0 */
+
+typedef struct jtb_rx_shard {
+    int32_t valid;              /* JTB_VALID / JTB_UNKNOWN / JTB_INVALID                                              */
+    int32_t n_reads;            /* :ok reads of the shard                                                             */
+    int32_t n_transfers;        /* transfer micro-ops of the shard (every fate)                                       */
+    int32_t witness_index;      /* completion :index of the earliest-completing unexplained read, -1                  */
+    int64_t n_explained;        /* reads explained                                                                    */
+    int64_t n_undecided;        /* reads left undecided by the budget                                                 */
+    int64_t count_by_kind[2];   /* [kind - 1]: unexplained reads of that kind                                         */
+    int64_t nodes;              /* search nodes over the shard's reads, the per-key searches of unexplained reads
+                                   included                                                                           */
+    int32_t kind;               /* JTB_RX_KEY / JTB_RX_JOINT, 0 when no read is unexplained                           */
+    int32_t key;                /* KEY: the smallest key without a subset; JOINT: the smallest key the root pruning
+                                   found unreachable, -1 when only the search refuted the read                        */
+    int32_t n_must;             /* |must| of the witness read: must transfers on a key it observes                    */
+    int32_t n_may;              /* "may" transfers of the witness read the root pruning did not drop                  */
+    int64_t value;              /* KEY: the witness read's value of key                                               */
+    int64_t must_sum;           /* KEY: the must transfers' sum on key                                                */
+} jtb_rx_shard;
+
+typedef struct jtb_rx_result {
+    int32_t valid;              /* merge-valid over shards                                                            */
+    int32_t n_failures;         /* shards that are not VALID                                                          */
+    int64_t n_reads;            /* :ok reads                                                                          */
+    int64_t n_transfers;        /* transfer micro-ops                                                                 */
+    int64_t n_explained;
+    int64_t n_unexplained;
+    int64_t n_undecided;
+    int64_t nodes;
+    double  seconds_kernel;     /* device time (CUDA events)                                                          */
+    double  seconds_total;      /* host wall time of the call incl. the host pass, H2D, D2H                           */
+} jtb_rx_result;
+
 typedef struct jtb_ctx jtb_ctx;
 
 /* ---- lifecycle -------------------------------------------------------------------------------- */
@@ -380,7 +432,7 @@ int         jtb_abi_version(void);
 /* sizeof of the ABI structs as this library was compiled, for binding self-checks:
  * 0 jtb_history, 1 jtb_model, 2 jtb_opts, 3 jtb_lin_shard, 4 jtb_lin_result, 5 jtb_setfull_shard,
  * 6 jtb_setfull_out, 7 jtb_bank_result, 8 jtb_final_config, 9 jtb_mono_shard, 10 jtb_mono_result, 11 jtb_cb_shard,
- * 12 jtb_cb_result, 13 jtb_tl_shard, 14 jtb_tl_result; -1 otherwise */
+ * 12 jtb_cb_result, 13 jtb_tl_shard, 14 jtb_tl_result, 15 jtb_rx_shard, 16 jtb_rx_result; -1 otherwise */
 long        jtb_struct_size(int which);
 int         jtb_device_count(void);                 /* number of CUDA devices, <0 on error          */
 jtb_ctx*    jtb_create(const jtb_opts* opts);       /* NULL on failure (no CUDA device etc.)        */
@@ -446,6 +498,13 @@ int jtb_check_counter_bounds(jtb_ctx* ctx, const jtb_history* h, int32_t flags, 
  * cannot hold, flags != 0, or a device allocation failure (jtb_last_error says which; the context stays usable). */
 int jtb_check_transfer_lookups(jtb_ctx* ctx, const jtb_history* h, int32_t flags, jtb_tl_shard* shards,
                                jtb_tl_result* out);
+
+/* ---- read-explanation check (see jtb_rx_shard above) ------------------------------------------------------------ *
+ * shards[n_shards] is caller-allocated; max_nodes <= 0 means JTB_RX_DEFAULT_MAX_NODES; flags is reserved and must be 0.
+ * Returns 0 on success, <0 on the transfer-lookup check's input errors, flags != 0, or a device allocation failure
+ * (jtb_last_error says which; the context stays usable). */
+int jtb_check_read_explanations(jtb_ctx* ctx, const jtb_history* h, int64_t max_nodes, int32_t flags,
+                                jtb_rx_shard* shards, jtb_rx_result* out);
 
 /* ---- multi-GPU fan-out inside the library (SURVEY §8(b) `n_gpus`, §8(e)) ----------------------------------- *
  * What `independent/checker` (set_full.clj:155) does over JVM threads, done over the GPUs of one box for a host

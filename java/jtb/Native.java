@@ -107,4 +107,14 @@ public final class Native {
      *     by kind, {@code witnessIndex, kind, transferId, key, relatedIndex, value, bound}
      */
     public static native long[] checkTransferLookups(long ctx, Object[] history);
+
+    /**
+     * {@code jtb_check_read_explanations}: whether one set of transfers explains every counter each :ok read shows.
+     * Input: the ledger-lookups form.  {@code maxNodes <= 0} is the default per-read search budget.
+     *
+     * @return {@code [valid, nFailures, nReads, nTransfers, nExplained, nUnexplained, nUndecided, nodes, kernelNs,
+     *     totalNs, nShards]} followed by 15 longs per shard: {@code valid, nReads, nTransfers, witnessIndex,
+     *     nExplained, nUndecided, nKey, nJoint, nodes, kind, key, nMust, nMay, value, mustSum}
+     */
+    public static native long[] checkReadExplanations(long ctx, Object[] history, long maxNodes);
 }

@@ -5,7 +5,7 @@ import ctypes as C
 
 from .history import MAX_ACCOUNTS
 
-ABI_VERSION = 5
+ABI_VERSION = 6
 OPT_NO_EAGER_READS = 1
 OPT_NO_SCOUTS = 2
 OPT_ENGINE_LEVEL = 4
@@ -22,6 +22,9 @@ CB_BELOW, CB_ABOVE = 1, 2
 TL_KINDS = 9
 TL_KIND_NAME = {1: "phantom", 2: "mismatch", 3: "failed-visible", 4: "future", 5: "duplicate", 6: "lost",
                 7: "vanished", 8: "read-below-lookup", 9: "read-above-lookup"}
+RX_KEY, RX_JOINT = 1, 2
+RX_KIND_NAME = {1: "key", 2: "joint"}
+RX_MAX_KEYS, RX_MAX_GATHER, RX_MAX_FREE, RX_DEFAULT_MAX_NODES = 256, 128, 64, 4096
 SF_NEVER_READ, SF_STABLE, SF_LOST = 0, 1, 2
 BANK_OK, BANK_UNEXPECTED_KEY, BANK_NIL_BALANCE, BANK_WRONG_TOTAL, BANK_NEGATIVE_VALUE = range(5)
 BANK_ERR_NAME = {1: "unexpected-key", 2: "nil-balance", 3: "wrong-total", 4: "negative-value"}
@@ -216,5 +219,34 @@ def tl_to_dict(res, shards) -> dict:
         "n_transfers": res.n_transfers, "n_reads": res.n_reads, "n_violations": res.n_violations,
         "seconds_kernel": res.seconds_kernel, "seconds_total": res.seconds_total,
         "shards": [{f: (list(s.count_by_kind) if f == "count_by_kind" else getattr(s, f)) for f in TL_SHARD_FIELDS}
+                   for s in shards],
+    }
+
+
+class CRxShard(C.Structure):
+    """jtb_rx_shard: the read-explanation verdict of one shard."""
+    _fields_ = [("valid", C.c_int32), ("n_reads", C.c_int32), ("n_transfers", C.c_int32), ("witness_index", C.c_int32),
+                ("n_explained", C.c_int64), ("n_undecided", C.c_int64), ("count_by_kind", C.c_int64 * 2),
+                ("nodes", C.c_int64), ("kind", C.c_int32), ("key", C.c_int32), ("n_must", C.c_int32),
+                ("n_may", C.c_int32), ("value", C.c_int64), ("must_sum", C.c_int64)]
+
+
+class CRxResult(C.Structure):
+    _fields_ = [("valid", C.c_int32), ("n_failures", C.c_int32), ("n_reads", C.c_int64), ("n_transfers", C.c_int64),
+                ("n_explained", C.c_int64), ("n_unexplained", C.c_int64), ("n_undecided", C.c_int64),
+                ("nodes", C.c_int64), ("seconds_kernel", C.c_double), ("seconds_total", C.c_double)]
+
+
+RX_SHARD_FIELDS = ("valid", "n_reads", "n_transfers", "witness_index", "n_explained", "n_undecided", "count_by_kind",
+                   "nodes", "kind", "key", "n_must", "n_may", "value", "must_sum")
+
+
+def rx_to_dict(res, shards) -> dict:
+    """One result dict for the library and the oracle (count_by_kind as a list indexed by kind - 1)."""
+    return {
+        "valid": res.valid, "n_failures": res.n_failures, "n_reads": res.n_reads, "n_transfers": res.n_transfers,
+        "n_explained": res.n_explained, "n_unexplained": res.n_unexplained, "n_undecided": res.n_undecided,
+        "nodes": res.nodes, "seconds_kernel": res.seconds_kernel, "seconds_total": res.seconds_total,
+        "shards": [{f: (list(s.count_by_kind) if f == "count_by_kind" else getattr(s, f)) for f in RX_SHARD_FIELDS}
                    for s in shards],
     }

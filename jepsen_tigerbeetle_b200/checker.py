@@ -410,6 +410,59 @@ class TransferLookups(Checker, _Native):
         return out
 
 
+class ReadExplanations(Checker, _Native):
+    """Whether one set of transfers explains every counter a ledger :ok read shows, on the GPU (K10).
+
+    Reads the ledger-lookups form.  For each read, the transfers that must be in it (:ok, or returned by an :ok lookup,
+    before it was invoked), the ones that cannot be (:fail, invoked after it completed, or absent from an :ok lookup
+    invoked after it completed) and the rest, which may be; a read is explained when some subset of the last closes
+    every counter it observes at once.  A read for which no single counter has such a subset is a "key" error (lost,
+    phantom, duplicated or corrupt amounts), one for which each counter has one but no one subset closes all of them a
+    "joint" error (torn or fractured transfers).  The search is budgeted (max-nodes, default 4096): a read it does not
+    decide makes the verdict :unknown, never false.  Result: {valid?, read-count, transfer-count, explained-count,
+    undecided-count, error-count, errors {kind count}, [op, error]}."""
+
+    def __init__(self, checker_opts: Mapping[str, Any] | None = None, ctx: Context | None = None,
+                 **ctx_opts) -> None:
+        _Native.__init__(self, ctx, **ctx_opts)
+        self.max_nodes = int((checker_opts or {}).get("max-nodes", 0))
+
+    def _shard_map(self, s: dict) -> dict:
+        errors = {abi.RX_KIND_NAME[k + 1]: n for k, n in enumerate(s["count_by_kind"]) if n}
+        m: dict[str, Any] = {"valid?": VERDICT_NAME[s["valid"]], "read-count": s["n_reads"],
+                             "transfer-count": s["n_transfers"], "explained-count": s["n_explained"],
+                             "undecided-count": s["n_undecided"], "error-count": sum(errors.values()),
+                             "errors": errors}
+        if s["valid"] == INVALID:
+            m["op"] = {"index": s["witness_index"]}
+            err: dict[str, Any] = {"type": abi.RX_KIND_NAME[s["kind"]], "must-count": s["n_must"],
+                                   "may-count": s["n_may"]}
+            k = s["key"]
+            if k >= 0:
+                err["key"] = [k >> 1, COUNTER_FIELDS[k & 1]]
+            if s["kind"] == abi.RX_KEY:
+                err.update({"value": s["value"], "must-sum": s["must_sum"]})
+            m["error"] = err
+        return m
+
+    def check_flat(self, test, h: FlatHistory) -> tuple[dict, list[dict]]:
+        r = self.ctx.check_read_explanations(h, self.max_nodes)
+        top = {"valid?": VERDICT_NAME[r["valid"]], "read-count": r["n_reads"], "transfer-count": r["n_transfers"],
+               "explained-count": r["n_explained"], "undecided-count": r["n_undecided"],
+               "error-count": r["n_unexplained"], "nodes": r["nodes"], "seconds-kernel": r["seconds_kernel"],
+               "seconds-total": r["seconds_total"]}
+        return top, [self._shard_map(s) for s in r["shards"]]
+
+    def check(self, test, history, opts=None) -> dict:
+        h = _flat(history, "ledger-lookups")
+        if h.n_shards != 1:
+            raise ValueError("history has independent keys: wrap with independent_checker(...)")
+        top, per = self.check_flat(test, h)
+        out = dict(per[0])
+        out.update({k: v for k, v in top.items() if k.startswith("seconds-") or k == "nodes"})
+        return out
+
+
 class Compose(Checker):
     """`(checker/compose {name checker ...})`: run each, `:valid?` = merge-valid of the results."""
 
@@ -442,13 +495,13 @@ class Independent(Checker):
             return c.model
         if isinstance(c, (MonotonicKeys, CounterBounds)):
             return "ledger-counters"
-        if isinstance(c, TransferLookups):
+        if isinstance(c, (TransferLookups, ReadExplanations)):
             return "ledger-lookups"
         return "set"
 
     def _per_key(self, checker: Checker, test, h: FlatHistory, opts) -> list[dict]:
         if isinstance(checker, (Linearizable, SetFull, ReadAllInvokedAdds, MonotonicKeys, CounterBounds,
-                                TransferLookups)):
+                                TransferLookups, ReadExplanations)):
             try:
                 return checker.check_flat(test, h)[1]
             except Exception:  # noqa: BLE001
@@ -511,6 +564,12 @@ def counter_bounds_checker(opts: Mapping[str, Any] | None = None, **kw) -> Count
 def transfer_lookup_checker(opts: Mapping[str, Any] | None = None, **kw) -> TransferLookups:
     """The looked-up transfer records against the transfers clients issued and the counters reads show (K9)."""
     return TransferLookups(opts, **kw)
+
+
+def read_explanation_checker(opts: Mapping[str, Any] | None = None, **kw) -> ReadExplanations:
+    """Whether one set of transfers explains every counter each ledger read shows (K10); {"max-nodes": n} sets the
+    per-read search budget."""
+    return ReadExplanations(opts, **kw)
 
 
 def compose(checkers: Mapping[str, Checker]) -> Compose:
@@ -680,12 +739,13 @@ def final_reads() -> FinalReads:
 
 def ledger_checker(checker_opts: Mapping[str, Any] | None = None, ctx: Context | None = None,
                    linear: bool = True, monotonic: bool = False, counter_bounds: bool = False,
-                   transfer_lookups: bool = False) -> Compose:
+                   transfer_lookups: bool = False, read_explanations: bool = False) -> Compose:
     """The ledger test's checker (tests/ledger.clj:363-367) minus the gnuplot plotter, plus the
     linearizability search the north-star adds and, with monotonic=True, the monotonic-key check, with
-    counter_bounds=True, the counter-bounds check and, with transfer_lookups=True, the transfer-lookup check:
+    counter_bounds=True, the counter-bounds check, with transfer_lookups=True, the transfer-lookup check and, with
+    read_explanations=True, the read-explanation check:
         {:SI (checker opts) :lookup-transfers ... :final-reads ... :unexpected-ops ... [:linear ...] [:monotonic ...]
-         [:counter-bounds ...] [:transfer-lookups ...]}"""
+         [:counter-bounds ...] [:transfer-lookups ...] [:read-explanations ...]}"""
     cs: dict[str, Checker] = {"SI": bank_checker(checker_opts, ctx=ctx),
                               "lookup-transfers": lookup_all_invoked_transfers(),
                               "final-reads": final_reads(), "unexpected-ops": unexpected_ops()}
@@ -697,4 +757,6 @@ def ledger_checker(checker_opts: Mapping[str, Any] | None = None, ctx: Context |
         cs["counter-bounds"] = counter_bounds_checker(ctx=ctx)
     if transfer_lookups:
         cs["transfer-lookups"] = transfer_lookup_checker(ctx=ctx)
+    if read_explanations:
+        cs["read-explanations"] = read_explanation_checker(ctx=ctx)
     return compose(cs)

@@ -20,6 +20,7 @@
 #include "jtb_monotonic.cuh"
 #include "jtb_counter_bounds.cuh"
 #include "jtb_transfer_lookups.cuh"
+#include "jtb_read_explanations.cuh"
 
 using namespace jtb;
 
@@ -729,6 +730,8 @@ long jtb_struct_size(int which) {
     case 12: return sizeof(jtb_cb_result);
     case 13: return sizeof(jtb_tl_shard);
     case 14: return sizeof(jtb_tl_result);
+    case 15: return sizeof(jtb_rx_shard);
+    case 16: return sizeof(jtb_rx_result);
     }
     return -1;
 }
@@ -1128,6 +1131,16 @@ int jtb_check_transfer_lookups(jtb_ctx* ctx, const jtb_history* h, int32_t flags
     if (cudaSetDevice(ctx->device) != cudaSuccess) { ctx->err = "cudaSetDevice failed"; return -1; }
     ctx->fc.valid = false;
     return run_transfer_lookups(ctx->stream, ctx->ev0, ctx->ev1, h, flags, shards, out, ctx->err);
+}
+
+// K10: the read-explanation check (csrc/jtb_read_explanations.cuh)
+int jtb_check_read_explanations(jtb_ctx* ctx, const jtb_history* h, int64_t max_nodes, int32_t flags,
+                                jtb_rx_shard* shards, jtb_rx_result* out) {
+    if (!ctx) return -1;
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    if (cudaSetDevice(ctx->device) != cudaSuccess) { ctx->err = "cudaSetDevice failed"; return -1; }
+    ctx->fc.valid = false;
+    return run_read_explanations(ctx->stream, ctx->ev0, ctx->ev1, h, max_nodes, flags, shards, out, ctx->err);
 }
 
 // SURVEY 8(f) N2: the step before the checkers (independent/subhistory, ledger->bank) on the device

@@ -108,7 +108,8 @@ def generate_ledger_counters(spec: SynthSpec, fractured: bool = False, lost_tran
 
 def generate_ledger_lookups(spec: SynthSpec, p_lookup: float = 0.0, lost_transfer: bool = False,
                             phantom_record: bool = False, mismatched_record: bool = False,
-                            vanished_record: bool = False, inflated_read: bool = False) -> FlatHistory:
+                            vanished_record: bool = False, inflated_read: bool = False, torn_transfer: bool = False,
+                            torn_pair: bool = False, split_amount: bool = False) -> FlatHistory:
     """The ledger-lookups form of a one-key bank `spec` (what flatten_ops(..., "ledger-lookups") makes of a ledger
     history): the events of generate_ledger_counters(spec), every transfer invoke carrying its record (id, debit,
     credit, amount) with ids 1, 2, ... in invocation order, then one quiesced :final? lookup per client, one after
@@ -124,7 +125,13 @@ def generate_ledger_lookups(spec: SynthSpec, p_lookup: float = 0.0, lost_transfe
                          read, which completes first, now lies above that lookup's sums; needs p_info > 0 and two
                          clients)
       inflated_read      the final read's first counter is one more than it was (READ_ABOVE_LOOKUP; needs
-                         spec.final_reads)"""
+                         spec.final_reads)
+    Read mutations for the read-explanation check (the first non-final :ok read, from the middle of the history on,
+    that has what the mutation needs among the :ok transfers concurrent with it; meta["torn_read_index"] is its :index):
+      torn_transfer      the read shows only the debit half of one concurrent transfer
+      torn_pair          two concurrent transfers of equal amount on four distinct accounts: the read shows the debit
+                         half of the first and the credit half of the second, so the totals still hold
+      split_amount       the read shows amount - 1 of a concurrent transfer (amount >= 2) on both sides"""
     if spec.model != "bank" or spec.n_keys != 1:
         raise ValueError("the ledger-lookups form needs a one-key bank spec")
     if inflated_read and not spec.final_reads:
@@ -202,6 +209,9 @@ def generate_ledger_lookups(spec: SynthSpec, p_lookup: float = 0.0, lost_transfe
     if inflated_read:
         e = np.nonzero((base.flags & FLAG_FINAL).astype(bool) & (base.type == T_OK) & (base.f == F_READ))[0][0]
         payload[poff_pre[e] + 1] += 1
+    torn_at = -1
+    for kind in [k for k, on in (("transfer", torn_transfer), ("pair", torn_pair), ("split", split_amount)) if on]:
+        torn_at = _tear_read(kind, base, ops, op_ev, ex["mutated_transfer"], payload, poff_pre)
     lt = np.array([x for lk in lookups for x in lk[:2]], np.int64)
     time_pre = np.concatenate([base.time_ns, lt])
     order = np.argsort(time_pre, kind="stable")
@@ -215,11 +225,63 @@ def generate_ledger_lookups(spec: SynthSpec, p_lookup: float = 0.0, lost_transfe
              np.arange(n + 2 * L, dtype=np.int32))
     meta = dict(base.meta, model="ledger-lookups", n_ops=base.meta["n_ops"] + L, multi_transfer_txns=0,
                 n_lookups=L)
+    if torn_transfer or torn_pair or split_amount:
+        meta["torn_read_index"] = int(index[np.nonzero(order == torn_at)[0][0]])
     h = FlatHistory(typ, f, flags, proc, index.astype(np.int32), time_pre[order], cat(base.a, zeros),
                     cat(base.b, zeros), cat(base.c, zeros), poff_pre[order], plen_pre[order], payload,
                     np.array([0, n + 2 * L], np.int64), base.key_ids.copy(), meta)
     h.validate()
     return h
+
+
+def _tear_read(kind: str, base: FlatHistory, ops: list, op_ev: np.ndarray, skip: int, payload: np.ndarray,
+               poff: np.ndarray) -> int:
+    """One read mutation of generate_ledger_lookups (no random draws) on the payload of the lookups form; returns the
+    base event of the read.  A read's payload is (2a, debits, 0, 2a + 1, credits, 0) per account a = 1, 2, ..."""
+    reads = np.nonzero((base.f == F_READ) & (base.type == T_OK) & ~(base.flags & FLAG_FINAL).astype(bool))[0]
+    reads = np.concatenate([reads[len(reads) // 2:], reads[:len(reads) // 2]])
+    tr = [i for i, o in enumerate(ops) if o[6] == F_TRANSFER and o[10] == 0 and i != skip]
+    t_inv = np.array([ops[i][0] for i in tr], np.int64)
+    t_ret = np.array([ops[i][1] for i in tr], np.int64)
+
+    def add(e: int, acct: int, field: int, x: int) -> None:
+        payload[poff[e] + 6 * (acct - 1) + 3 * field + 1] += x
+
+    for e in reads:
+        r = ops[op_ev[e]]
+        conc = [tr[j] for j in np.nonzero((t_inv < r[1]) & (t_ret > r[0]))[0]]
+        seen = lambda i: ops[i][2] < r[2]   # noqa: E731  (linearized before the read)
+        if kind == "transfer" and conc:
+            t = ops[conc[0]]
+            if seen(conc[0]):
+                add(e, t[9], 1, -t[7])
+            else:
+                add(e, t[8], 0, t[7])
+            return int(e)
+        if kind == "split":
+            big = [i for i in conc if ops[i][7] >= 2]
+            if big:
+                t = ops[big[0]]
+                x = -1 if seen(big[0]) else t[7] - 1
+                add(e, t[8], 0, x)
+                add(e, t[9], 1, x)
+                return int(e)
+        if kind == "pair":
+            for a in range(len(conc)):
+                for b in range(a + 1, len(conc)):
+                    t1, t2 = ops[conc[a]], ops[conc[b]]
+                    if t1[7] != t2[7] or {t1[8], t1[9]} & {t2[8], t2[9]}:
+                        continue
+                    if seen(conc[a]):
+                        add(e, t1[9], 1, -t1[7])
+                    else:
+                        add(e, t1[8], 0, t1[7])
+                    if seen(conc[b]):
+                        add(e, t2[8], 0, -t2[7])
+                    else:
+                        add(e, t2[9], 1, t2[7])
+                    return int(e)
+    raise ValueError(f"no read has what the {kind} mutation needs")
 
 
 def _generate(spec: SynthSpec, counters: bool = False, fracture: bool = False, lost: bool = False,

@@ -5,7 +5,8 @@ MONO_GRAPH builds Elle's monotonic-key graph literally (plus real-time edges) an
 for 2-cycles by brute force.  See mono_oracle.cpp.  CB_LITERAL sums every transfer for every (read, key); CB_SWEEP
 keeps running sums over one walk of the events.  See counter_bounds.cpp.  TL_LITERAL checks every (lookup, transfer)
 pair and every (read, key, lookup) triple; TL_SWEEP walks with hash maps, sorted M lists, prefix maxima and suffix
-minima.  See transfer_lookups.cpp."""
+minima.  See transfer_lookups.cpp.  RX_BRUTE enumerates every subset of a read's "may" transfers; RX_SEARCH is the
+library's budgeted pruning and depth-first search over a sweep.  See read_explanations.cpp."""
 from __future__ import annotations
 
 import ctypes as C
@@ -19,6 +20,7 @@ from jepsen_tigerbeetle_b200.history import FlatHistory, as_c_history
 MONO_GRAPH, MONO_PAIRS = 0, 1
 CB_LITERAL, CB_SWEEP = 0, 1
 TL_LITERAL, TL_SWEEP = 0, 1
+RX_BRUTE, RX_SEARCH = 0, 1
 DECIDE_PARTIAL = 1 << 16   # decide shards with partial reads instead of reporting them UNKNOWN
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB = None
@@ -28,7 +30,8 @@ def build(force: bool = False) -> str:
     """The library in mono_oracle/, rebuilt when stale; when the directory is read-only a rebuild goes to a fresh
     temporary directory instead."""
     so = os.path.join(_HERE, "libjtb_mono_oracle.so")
-    srcs = [os.path.join(_HERE, f) for f in ("mono_oracle.cpp", "counter_bounds.cpp", "transfer_lookups.cpp", "Makefile")]
+    srcs = [os.path.join(_HERE, f) for f in ("mono_oracle.cpp", "counter_bounds.cpp", "transfer_lookups.cpp",
+                                                "read_explanations.cpp", "Makefile")]
     srcs.append(os.path.join(_HERE, "..", "include", "jtb_check.h"))
     stale = not os.path.exists(so) or any(os.path.getmtime(s) > os.path.getmtime(so) for s in srcs)
     if force or stale:
@@ -50,6 +53,9 @@ def lib() -> C.CDLL:
         _LIB.jtbm_check_counter_bounds.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
         _LIB.jtbm_tl_last_error.restype = C.c_char_p
         _LIB.jtbm_check_transfer_lookups.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
+        _LIB.jtbm_rx_last_error.restype = C.c_char_p
+        _LIB.jtbm_check_read_explanations.argtypes = [C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_void_p,
+                                                      C.c_void_p, C.c_void_p]
     return _LIB
 
 
@@ -86,3 +92,23 @@ def check_transfer_lookups(h: FlatHistory, algo: int = TL_SWEEP, flags: int = 0)
     if rc != 0:
         raise RuntimeError(lib().jtbm_tl_last_error().decode())
     return abi.tl_to_dict(res, shards[:h.n_shards])
+
+
+def check_read_explanations(h: FlatHistory, algo: int = RX_SEARCH, max_nodes: int = 0, flags: int = 0,
+                            per_read: bool = False) -> dict:
+    """Twin of `jtb_check_read_explanations` (same result dict as `native.Context.check_read_explanations`).
+    per_read=True adds "per_read": one code per :ok read in shard-major completion order (0 explained, 1 KEY, 2 JOINT,
+    3 undecided)."""
+    import numpy as np
+    ch = as_c_history(h)
+    shards = (abi.CRxShard * max(1, h.n_shards))()
+    res = abi.CRxResult()
+    codes = np.zeros(max(1, int(np.count_nonzero(h.f == 0))), np.int8)
+    rc = lib().jtbm_check_read_explanations(C.addressof(ch), max_nodes, flags, algo, C.addressof(shards),
+                                            C.addressof(res), codes.ctypes.data if per_read else None)
+    if rc != 0:
+        raise RuntimeError(lib().jtbm_rx_last_error().decode())
+    out = abi.rx_to_dict(res, shards[:h.n_shards])
+    if per_read:
+        out["per_read"] = codes[:res.n_reads].tolist()
+    return out
