@@ -470,6 +470,40 @@
                                        (<= 0 key) (assoc :key [(quot key 2) (counter-field (rem key 2))])
                                        (= 1 kind) (assoc :value (at (+ s 13)) :must-sum (at (+ s 14))))))))))
 
+;; ---- read gaps ----------------------------------------------------------------------------------------------------
+(def ^:private rg-kind {1 :key 2 :joint 3 :double})
+
+(defn read-gap-checker
+  "Whether the transfers committed between two successive :ok reads explain what changed, on the GPU: the reads of a
+  shard in the monotonic-key order (by the sum of their values, then invocation), and for each gap between neighbours a
+  budgeted search for a subset of the transfers that may have committed inside it summing to the change of every
+  counter.  :key errors have a counter that goes down or that no subset closes, :joint errors close each counter alone
+  but not all at once, :double errors name a transfer two gaps both need.  A gap the budget ({:max-nodes n}) does not
+  decide, and a shard with a partial read, make the verdict :unknown.  Add it to the compose map at
+  tests/ledger.clj:363-367 as `:read-gaps (read-gap-checker {})`.
+  Result: {:valid? :read-count :transfer-count :explained-count :undecided-count :error-count :errors
+  [:op :lower-op :error]}."
+  [opts]
+  (reify checker/Checker
+    (check [_ _test history _opts]
+      (let [{:keys [arrays by-index]} (flatten-history :ledger-lookups history)
+            res    (Native/checkReadGaps @ctx arrays (long (:max-nodes opts 0)))
+            at     (fn [i] (aget res (int i)))
+            s      12                                     ; shard 0: valid cause reads transfers explained undecided ...
+            errors (into {} (for [k (range 3) :let [n (at (+ s 6 k))] :when (pos? n)] [(rg-kind (inc k)) n]))
+            kind   (at (+ s 12))
+            key    (at (+ s 13))]
+        (cond-> {:valid? (verdict (at s)) :read-count (at (+ s 2)) :transfer-count (at (+ s 3))
+                 :explained-count (at (+ s 4)) :undecided-count (at (+ s 5)) :error-count (reduce + (vals errors))
+                 :errors errors}
+          (= 2 (at s)) (assoc :op    (by-index (at (+ s 10)))
+                              :error (cond-> {:type (rg-kind kind) :eligible-count (at (+ s 17))}
+                                       (<= 0 key)  (assoc :key [(quot key 2) (counter-field (rem key 2))])
+                                       (= 1 kind)  (assoc :delta (at (+ s 14)))
+                                       (= 3 kind)  (assoc :transfer-id (at (+ s 15))
+                                                          :other-op (by-index (at (+ s 16))))))
+          (and (= 2 (at s)) (<= 0 (at (+ s 11)))) (assoc :lower-op (by-index (at (+ s 11)))))))))
+
 ;; ---- independent ----------------------------------------------------------------------------------------------
 (defn independent-checker
   "Like (independent/checker (checker/compose checkers)) for a map {name checker-kind} built from THIS namespace's

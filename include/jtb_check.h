@@ -24,7 +24,7 @@
 extern "C" {
 #endif
 
-#define JTB_ABI_VERSION 6
+#define JTB_ABI_VERSION 7
 
 /* ---- verdict lattice (jepsen.checker/merge-valid) ------------------------------------------- */
 #define JTB_VALID   0
@@ -425,6 +425,65 @@ typedef struct jtb_rx_result {
     double  seconds_total;      /* host wall time of the call incl. the host pass, H2D, D2H                           */
 } jtb_rx_result;
 
+/* ---- read-gap check (DESIGN.md "K11 read-gap check") ----------------------------------------------------------------
+ * Input: the ledger-lookups form, read as the read-explanation check reads it (M(t), A(t) and the fates are K10's).  A
+ * shard whose :ok reads do not all observe every key of the shard is JTB_UNKNOWN with JTB_CAUSE_PARTIAL_READ.  On the
+ * others the :ok reads are ordered as the monotonic-key check orders them, by (S = the sum of the values, invocation
+ * position), r_1 ... r_n, and each read closes one gap: gap 0 from the zero state to r_1, gap i from r_i to r_{i+1},
+ * with Delta_k = v_k(r_{i+1}) - v_k(r_i).  A transfer is eligible for gap i unless its fate is :fail, it was invoked
+ * after r_{i+1} completed, A(t) > cp(r_{i+1}), or (i >= 1) M(t) < iv(r_i); transfers with a zero amount on every
+ * observed key are ignored, and so are those whose amount exceeds Delta_k on one of their keys (no subset summing to
+ * Delta holds them).  A gap with some Delta_k < 0 is unexplained (KEY: the two reads form a monotonic-key 2-cycle);
+ * Delta = 0 is explained; otherwise the gap is explained when a subset of its eligible transfers sums to Delta_k on
+ * every key, decided with the read-explanation check's caps (the gather cap after the amount filter), pruning,
+ * canonical search and node budget.
+ * A transfer the root pruning forces into two gaps is DOUBLE: the differences between successive read states are
+ * disjoint.  A shard is JTB_INVALID when some gap is unexplained or some transfer DOUBLE, else JTB_UNKNOWN when some
+ * gap is undecided, else JTB_VALID. */
+#define JTB_RG_KEY    1 /* some Delta_k < 0, or some key alone has no subset of the eligible transfers that fit under
+                           Delta (amount <= Delta on each of its observed keys) summing to Delta_k                  */
+#define JTB_RG_JOINT  2 /* every key alone has one, but no one subset closes all of them                              */
+#define JTB_RG_DOUBLE 3 /* a transfer the root pruning forces into this gap and into an earlier one                   */
+#define JTB_RG_MAX_KEYS   256
+#define JTB_RG_MAX_GATHER 128
+#define JTB_RG_MAX_FREE   64
+#define JTB_RG_DEFAULT_MAX_NODES 4096 /* max_nodes <= 0 */
+
+typedef struct jtb_rg_shard {
+    int32_t valid;              /* JTB_VALID / JTB_UNKNOWN / JTB_INVALID                                              */
+    int32_t cause;              /* JTB_CAUSE_PARTIAL_READ when a partial read makes the shard UNKNOWN, else 0         */
+    int32_t n_reads;            /* :ok reads of the shard; a full-key shard has as many gaps                          */
+    int32_t n_transfers;        /* transfer micro-ops of the shard (every fate)                                       */
+    int64_t n_explained;        /* gaps explained                                                                     */
+    int64_t n_undecided;        /* gaps left undecided by the budget                                                  */
+    int64_t count_by_kind[3];   /* unexplained gaps of kind KEY, of kind JOINT, and DOUBLE transfers                  */
+    int64_t nodes;              /* search nodes over the shard's gaps, the per-key searches of unexplained gaps
+                                   included                                                                           */
+    int32_t witness_index;      /* completion :index of r_{i+1} of the first violating gap in the order, -1          */
+    int32_t lower_index;        /* completion :index of r_i, -1 for gap 0 or no witness                               */
+    int32_t kind;               /* JTB_RG_KEY / JOINT / DOUBLE (the smallest at the witness gap), 0 without one       */
+    int32_t key;                /* KEY: the smallest refuted key; JOINT: the smallest key the root pruning found
+                                   unreachable, -1 when only the search refuted the gap; DOUBLE: -1                   */
+    int64_t delta;              /* KEY: Delta_k of key                                                                */
+    int64_t transfer_id;        /* DOUBLE: the transfer's id (the smallest at the witness gap)                        */
+    int32_t other_index;        /* DOUBLE: completion :index of the upper read of the earlier gap, -1                 */
+    int32_t n_eligible;         /* eligible transfers of the witness gap the root pruning did not drop                */
+} jtb_rg_shard;
+
+typedef struct jtb_rg_result {
+    int32_t valid;              /* merge-valid over shards                                                            */
+    int32_t n_failures;         /* shards that are not VALID                                                          */
+    int64_t n_reads;            /* :ok reads                                                                          */
+    int64_t n_transfers;        /* transfer micro-ops                                                                 */
+    int64_t n_explained;        /* gaps explained                                                                     */
+    int64_t n_unexplained;      /* gaps unexplained (KEY + JOINT)                                                     */
+    int64_t n_double;           /* DOUBLE transfers                                                                   */
+    int64_t n_undecided;        /* gaps undecided                                                                     */
+    int64_t nodes;
+    double  seconds_kernel;     /* device time (CUDA events)                                                          */
+    double  seconds_total;      /* host wall time of the call incl. the host pass, H2D, D2H                           */
+} jtb_rg_result;
+
 typedef struct jtb_ctx jtb_ctx;
 
 /* ---- lifecycle -------------------------------------------------------------------------------- */
@@ -432,7 +491,8 @@ int         jtb_abi_version(void);
 /* sizeof of the ABI structs as this library was compiled, for binding self-checks:
  * 0 jtb_history, 1 jtb_model, 2 jtb_opts, 3 jtb_lin_shard, 4 jtb_lin_result, 5 jtb_setfull_shard,
  * 6 jtb_setfull_out, 7 jtb_bank_result, 8 jtb_final_config, 9 jtb_mono_shard, 10 jtb_mono_result, 11 jtb_cb_shard,
- * 12 jtb_cb_result, 13 jtb_tl_shard, 14 jtb_tl_result, 15 jtb_rx_shard, 16 jtb_rx_result; -1 otherwise */
+ * 12 jtb_cb_result, 13 jtb_tl_shard, 14 jtb_tl_result, 15 jtb_rx_shard, 16 jtb_rx_result, 17 jtb_rg_shard,
+ * 18 jtb_rg_result; -1 otherwise */
 long        jtb_struct_size(int which);
 int         jtb_device_count(void);                 /* number of CUDA devices, <0 on error          */
 jtb_ctx*    jtb_create(const jtb_opts* opts);       /* NULL on failure (no CUDA device etc.)        */
@@ -505,6 +565,14 @@ int jtb_check_transfer_lookups(jtb_ctx* ctx, const jtb_history* h, int32_t flags
  * (jtb_last_error says which; the context stays usable). */
 int jtb_check_read_explanations(jtb_ctx* ctx, const jtb_history* h, int64_t max_nodes, int32_t flags,
                                 jtb_rx_shard* shards, jtb_rx_result* out);
+
+/* ---- read-gap check (see jtb_rg_shard above) -------------------------------------------------------------------- *
+ * shards[n_shards] is caller-allocated; max_nodes <= 0 means JTB_RG_DEFAULT_MAX_NODES; flags is reserved and must be 0.
+ * Returns 0 on success, <0 on the read-explanation check's input errors, flags != 0, a dense value matrix (reads x
+ * keys of the full-key shards) the device cannot hold, or a device allocation failure (jtb_last_error says which; the
+ * context stays usable). */
+int jtb_check_read_gaps(jtb_ctx* ctx, const jtb_history* h, int64_t max_nodes, int32_t flags, jtb_rg_shard* shards,
+                        jtb_rg_result* out);
 
 /* ---- multi-GPU fan-out inside the library (SURVEY §8(b) `n_gpus`, §8(e)) ----------------------------------- *
  * What `independent/checker` (set_full.clj:155) does over JVM threads, done over the GPUs of one box for a host

@@ -117,4 +117,15 @@ public final class Native {
      *     nExplained, nUndecided, nKey, nJoint, nodes, kind, key, nMust, nMay, value, mustSum}
      */
     public static native long[] checkReadExplanations(long ctx, Object[] history, long maxNodes);
+
+    /**
+     * {@code jtb_check_read_gaps}: whether the transfers committed between two successive :ok reads explain what
+     * changed.  Input: the ledger-lookups form.  {@code maxNodes <= 0} is the default per-gap search budget.
+     *
+     * @return {@code [valid, nFailures, nReads, nTransfers, nExplained, nUnexplained, nDouble, nUndecided, nodes,
+     *     kernelNs, totalNs, nShards]} followed by 18 longs per shard: {@code valid, cause, nReads, nTransfers,
+     *     nExplained, nUndecided, nKey, nJoint, nDouble, nodes, witnessIndex, lowerIndex, kind, key, delta,
+     *     transferId, otherIndex, nEligible}
+     */
+    public static native long[] checkReadGaps(long ctx, Object[] history, long maxNodes);
 }

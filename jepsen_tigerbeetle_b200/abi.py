@@ -5,7 +5,7 @@ import ctypes as C
 
 from .history import MAX_ACCOUNTS
 
-ABI_VERSION = 6
+ABI_VERSION = 7
 OPT_NO_EAGER_READS = 1
 OPT_NO_SCOUTS = 2
 OPT_ENGINE_LEVEL = 4
@@ -25,6 +25,9 @@ TL_KIND_NAME = {1: "phantom", 2: "mismatch", 3: "failed-visible", 4: "future", 5
 RX_KEY, RX_JOINT = 1, 2
 RX_KIND_NAME = {1: "key", 2: "joint"}
 RX_MAX_KEYS, RX_MAX_GATHER, RX_MAX_FREE, RX_DEFAULT_MAX_NODES = 256, 128, 64, 4096
+RG_KEY, RG_JOINT, RG_DOUBLE = 1, 2, 3
+RG_KIND_NAME = {1: "key", 2: "joint", 3: "double"}
+RG_MAX_KEYS, RG_MAX_GATHER, RG_MAX_FREE, RG_DEFAULT_MAX_NODES = 256, 128, 64, 4096
 SF_NEVER_READ, SF_STABLE, SF_LOST = 0, 1, 2
 BANK_OK, BANK_UNEXPECTED_KEY, BANK_NIL_BALANCE, BANK_WRONG_TOTAL, BANK_NEGATIVE_VALUE = range(5)
 BANK_ERR_NAME = {1: "unexpected-key", 2: "nil-balance", 3: "wrong-total", 4: "negative-value"}
@@ -248,5 +251,37 @@ def rx_to_dict(res, shards) -> dict:
         "n_explained": res.n_explained, "n_unexplained": res.n_unexplained, "n_undecided": res.n_undecided,
         "nodes": res.nodes, "seconds_kernel": res.seconds_kernel, "seconds_total": res.seconds_total,
         "shards": [{f: (list(s.count_by_kind) if f == "count_by_kind" else getattr(s, f)) for f in RX_SHARD_FIELDS}
+                   for s in shards],
+    }
+
+
+class CRgShard(C.Structure):
+    """jtb_rg_shard: the read-gap verdict of one shard."""
+    _fields_ = [("valid", C.c_int32), ("cause", C.c_int32), ("n_reads", C.c_int32), ("n_transfers", C.c_int32),
+                ("n_explained", C.c_int64), ("n_undecided", C.c_int64), ("count_by_kind", C.c_int64 * 3),
+                ("nodes", C.c_int64), ("witness_index", C.c_int32), ("lower_index", C.c_int32), ("kind", C.c_int32),
+                ("key", C.c_int32), ("delta", C.c_int64), ("transfer_id", C.c_int64), ("other_index", C.c_int32),
+                ("n_eligible", C.c_int32)]
+
+
+class CRgResult(C.Structure):
+    _fields_ = [("valid", C.c_int32), ("n_failures", C.c_int32), ("n_reads", C.c_int64), ("n_transfers", C.c_int64),
+                ("n_explained", C.c_int64), ("n_unexplained", C.c_int64), ("n_double", C.c_int64),
+                ("n_undecided", C.c_int64), ("nodes", C.c_int64), ("seconds_kernel", C.c_double),
+                ("seconds_total", C.c_double)]
+
+
+RG_SHARD_FIELDS = ("valid", "cause", "n_reads", "n_transfers", "n_explained", "n_undecided", "count_by_kind", "nodes",
+                   "witness_index", "lower_index", "kind", "key", "delta", "transfer_id", "other_index", "n_eligible")
+
+
+def rg_to_dict(res, shards) -> dict:
+    """One result dict for the library and the oracle (count_by_kind as a list indexed by kind - 1)."""
+    return {
+        "valid": res.valid, "n_failures": res.n_failures, "n_reads": res.n_reads, "n_transfers": res.n_transfers,
+        "n_explained": res.n_explained, "n_unexplained": res.n_unexplained, "n_double": res.n_double,
+        "n_undecided": res.n_undecided, "nodes": res.nodes, "seconds_kernel": res.seconds_kernel,
+        "seconds_total": res.seconds_total,
+        "shards": [{f: (list(s.count_by_kind) if f == "count_by_kind" else getattr(s, f)) for f in RG_SHARD_FIELDS}
                    for s in shards],
     }

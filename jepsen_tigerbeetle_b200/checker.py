@@ -463,6 +463,65 @@ class ReadExplanations(Checker, _Native):
         return out
 
 
+class ReadGaps(Checker, _Native):
+    """Whether the transfers committed between two successive ledger reads explain what changed, on the GPU (K11).
+
+    Reads the ledger-lookups form.  The :ok reads of a shard whose reads all observe every key are ordered as the
+    monotonic-key check orders them (by the sum of their values, then invocation); each read closes the gap from the
+    read before it (the zero state for the first).  A gap is explained when some subset of the transfers that may have
+    committed inside it sums to the gap's change on every counter.  A gap with a counter going down, or whose change no
+    single counter's subset produces, is a "key" error; one whose counters each close alone but not all at once a
+    "joint" error; a transfer that two gaps both need is a "double" error.  Shards with a partial read are :unknown.
+    The search is budgeted (max-nodes, default 4096): a gap it does not decide makes the verdict :unknown, never false.
+    Result: {valid?, read-count, transfer-count, explained-count, undecided-count, error-count, errors {kind count},
+    [op, lower-op, error]}."""
+
+    def __init__(self, checker_opts: Mapping[str, Any] | None = None, ctx: Context | None = None,
+                 **ctx_opts) -> None:
+        _Native.__init__(self, ctx, **ctx_opts)
+        self.max_nodes = int((checker_opts or {}).get("max-nodes", 0))
+
+    def _shard_map(self, s: dict) -> dict:
+        errors = {abi.RG_KIND_NAME[k + 1]: n for k, n in enumerate(s["count_by_kind"]) if n}
+        m: dict[str, Any] = {"valid?": VERDICT_NAME[s["valid"]], "read-count": s["n_reads"],
+                             "transfer-count": s["n_transfers"], "explained-count": s["n_explained"],
+                             "undecided-count": s["n_undecided"], "error-count": sum(errors.values()),
+                             "errors": errors}
+        if s["cause"]:
+            m["cause"] = abi.CAUSE_NAME.get(s["cause"], "unknown")
+        if s["valid"] == INVALID:
+            m["op"] = {"index": s["witness_index"]}
+            if s["lower_index"] >= 0:
+                m["lower-op"] = {"index": s["lower_index"]}
+            err: dict[str, Any] = {"type": abi.RG_KIND_NAME[s["kind"]], "eligible-count": s["n_eligible"]}
+            k = s["key"]
+            if k >= 0:
+                err["key"] = [k >> 1, COUNTER_FIELDS[k & 1]]
+            if s["kind"] == abi.RG_KEY:
+                err["delta"] = s["delta"]
+            if s["kind"] == abi.RG_DOUBLE:
+                err.update({"transfer-id": s["transfer_id"], "other-op": {"index": s["other_index"]}})
+            m["error"] = err
+        return m
+
+    def check_flat(self, test, h: FlatHistory) -> tuple[dict, list[dict]]:
+        r = self.ctx.check_read_gaps(h, self.max_nodes)
+        top = {"valid?": VERDICT_NAME[r["valid"]], "read-count": r["n_reads"], "transfer-count": r["n_transfers"],
+               "explained-count": r["n_explained"], "undecided-count": r["n_undecided"],
+               "error-count": r["n_unexplained"] + r["n_double"], "nodes": r["nodes"],
+               "seconds-kernel": r["seconds_kernel"], "seconds-total": r["seconds_total"]}
+        return top, [self._shard_map(s) for s in r["shards"]]
+
+    def check(self, test, history, opts=None) -> dict:
+        h = _flat(history, "ledger-lookups")
+        if h.n_shards != 1:
+            raise ValueError("history has independent keys: wrap with independent_checker(...)")
+        top, per = self.check_flat(test, h)
+        out = dict(per[0])
+        out.update({k: v for k, v in top.items() if k.startswith("seconds-") or k == "nodes"})
+        return out
+
+
 class Compose(Checker):
     """`(checker/compose {name checker ...})`: run each, `:valid?` = merge-valid of the results."""
 
@@ -495,13 +554,13 @@ class Independent(Checker):
             return c.model
         if isinstance(c, (MonotonicKeys, CounterBounds)):
             return "ledger-counters"
-        if isinstance(c, (TransferLookups, ReadExplanations)):
+        if isinstance(c, (TransferLookups, ReadExplanations, ReadGaps)):
             return "ledger-lookups"
         return "set"
 
     def _per_key(self, checker: Checker, test, h: FlatHistory, opts) -> list[dict]:
         if isinstance(checker, (Linearizable, SetFull, ReadAllInvokedAdds, MonotonicKeys, CounterBounds,
-                                TransferLookups, ReadExplanations)):
+                                TransferLookups, ReadExplanations, ReadGaps)):
             try:
                 return checker.check_flat(test, h)[1]
             except Exception:  # noqa: BLE001
@@ -570,6 +629,12 @@ def read_explanation_checker(opts: Mapping[str, Any] | None = None, **kw) -> Rea
     """Whether one set of transfers explains every counter each ledger read shows (K10); {"max-nodes": n} sets the
     per-read search budget."""
     return ReadExplanations(opts, **kw)
+
+
+def read_gap_checker(opts: Mapping[str, Any] | None = None, **kw) -> ReadGaps:
+    """Whether the transfers committed between two successive ledger reads explain what changed (K11);
+    {"max-nodes": n} sets the per-gap search budget."""
+    return ReadGaps(opts, **kw)
 
 
 def compose(checkers: Mapping[str, Checker]) -> Compose:
@@ -739,13 +804,14 @@ def final_reads() -> FinalReads:
 
 def ledger_checker(checker_opts: Mapping[str, Any] | None = None, ctx: Context | None = None,
                    linear: bool = True, monotonic: bool = False, counter_bounds: bool = False,
-                   transfer_lookups: bool = False, read_explanations: bool = False) -> Compose:
+                   transfer_lookups: bool = False, read_explanations: bool = False,
+                   read_gaps: bool = False) -> Compose:
     """The ledger test's checker (tests/ledger.clj:363-367) minus the gnuplot plotter, plus the
     linearizability search the north-star adds and, with monotonic=True, the monotonic-key check, with
-    counter_bounds=True, the counter-bounds check, with transfer_lookups=True, the transfer-lookup check and, with
-    read_explanations=True, the read-explanation check:
+    counter_bounds=True, the counter-bounds check, with transfer_lookups=True, the transfer-lookup check, with
+    read_explanations=True, the read-explanation check and, with read_gaps=True, the read-gap check:
         {:SI (checker opts) :lookup-transfers ... :final-reads ... :unexpected-ops ... [:linear ...] [:monotonic ...]
-         [:counter-bounds ...] [:transfer-lookups ...] [:read-explanations ...]}"""
+         [:counter-bounds ...] [:transfer-lookups ...] [:read-explanations ...] [:read-gaps ...]}"""
     cs: dict[str, Checker] = {"SI": bank_checker(checker_opts, ctx=ctx),
                               "lookup-transfers": lookup_all_invoked_transfers(),
                               "final-reads": final_reads(), "unexpected-ops": unexpected_ops()}
@@ -759,4 +825,6 @@ def ledger_checker(checker_opts: Mapping[str, Any] | None = None, ctx: Context |
         cs["transfer-lookups"] = transfer_lookup_checker(ctx=ctx)
     if read_explanations:
         cs["read-explanations"] = read_explanation_checker(ctx=ctx)
+    if read_gaps:
+        cs["read-gaps"] = read_gap_checker(ctx=ctx)
     return compose(cs)

@@ -21,6 +21,7 @@
 #include "jtb_counter_bounds.cuh"
 #include "jtb_transfer_lookups.cuh"
 #include "jtb_read_explanations.cuh"
+#include "jtb_read_gaps.cuh"
 
 using namespace jtb;
 
@@ -732,6 +733,8 @@ long jtb_struct_size(int which) {
     case 14: return sizeof(jtb_tl_result);
     case 15: return sizeof(jtb_rx_shard);
     case 16: return sizeof(jtb_rx_result);
+    case 17: return sizeof(jtb_rg_shard);
+    case 18: return sizeof(jtb_rg_result);
     }
     return -1;
 }
@@ -1141,6 +1144,16 @@ int jtb_check_read_explanations(jtb_ctx* ctx, const jtb_history* h, int64_t max_
     if (cudaSetDevice(ctx->device) != cudaSuccess) { ctx->err = "cudaSetDevice failed"; return -1; }
     ctx->fc.valid = false;
     return run_read_explanations(ctx->stream, ctx->ev0, ctx->ev1, h, max_nodes, flags, shards, out, ctx->err);
+}
+
+// K11: the read-gap check (csrc/jtb_read_gaps.cuh)
+int jtb_check_read_gaps(jtb_ctx* ctx, const jtb_history* h, int64_t max_nodes, int32_t flags, jtb_rg_shard* shards,
+                        jtb_rg_result* out) {
+    if (!ctx) return -1;
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    if (cudaSetDevice(ctx->device) != cudaSuccess) { ctx->err = "cudaSetDevice failed"; return -1; }
+    ctx->fc.valid = false;
+    return run_read_gaps(ctx->stream, ctx->ev0, ctx->ev1, h, max_nodes, flags, shards, out, ctx->err);
 }
 
 // SURVEY 8(f) N2: the step before the checkers (independent/subhistory, ledger->bank) on the device

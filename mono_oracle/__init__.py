@@ -6,7 +6,9 @@ for 2-cycles by brute force.  See mono_oracle.cpp.  CB_LITERAL sums every transf
 keeps running sums over one walk of the events.  See counter_bounds.cpp.  TL_LITERAL checks every (lookup, transfer)
 pair and every (read, key, lookup) triple; TL_SWEEP walks with hash maps, sorted M lists, prefix maxima and suffix
 minima.  See transfer_lookups.cpp.  RX_BRUTE enumerates every subset of a read's "may" transfers; RX_SEARCH is the
-library's budgeted pruning and depth-first search over a sweep.  See read_explanations.cpp."""
+library's budgeted pruning and depth-first search over a sweep.  See read_explanations.cpp.  RG_BRUTE enumerates every
+subset of a gap's eligible transfers; RG_SEARCH is the library's amount filter, caps and search per gap.  See
+read_gaps.cpp."""
 from __future__ import annotations
 
 import ctypes as C
@@ -21,6 +23,7 @@ MONO_GRAPH, MONO_PAIRS = 0, 1
 CB_LITERAL, CB_SWEEP = 0, 1
 TL_LITERAL, TL_SWEEP = 0, 1
 RX_BRUTE, RX_SEARCH = 0, 1
+RG_BRUTE, RG_SEARCH = 0, 1
 DECIDE_PARTIAL = 1 << 16   # decide shards with partial reads instead of reporting them UNKNOWN
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB = None
@@ -31,7 +34,7 @@ def build(force: bool = False) -> str:
     temporary directory instead."""
     so = os.path.join(_HERE, "libjtb_mono_oracle.so")
     srcs = [os.path.join(_HERE, f) for f in ("mono_oracle.cpp", "counter_bounds.cpp", "transfer_lookups.cpp",
-                                                "read_explanations.cpp", "Makefile")]
+                                                "read_explanations.cpp", "read_gaps.cpp", "Makefile")]
     srcs.append(os.path.join(_HERE, "..", "include", "jtb_check.h"))
     stale = not os.path.exists(so) or any(os.path.getmtime(s) > os.path.getmtime(so) for s in srcs)
     if force or stale:
@@ -56,6 +59,9 @@ def lib() -> C.CDLL:
         _LIB.jtbm_rx_last_error.restype = C.c_char_p
         _LIB.jtbm_check_read_explanations.argtypes = [C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_void_p,
                                                       C.c_void_p, C.c_void_p]
+        _LIB.jtbm_rg_last_error.restype = C.c_char_p
+        _LIB.jtbm_check_read_gaps.argtypes = [C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                                              C.c_void_p]
     return _LIB
 
 
@@ -111,4 +117,24 @@ def check_read_explanations(h: FlatHistory, algo: int = RX_SEARCH, max_nodes: in
     out = abi.rx_to_dict(res, shards[:h.n_shards])
     if per_read:
         out["per_read"] = codes[:res.n_reads].tolist()
+    return out
+
+
+def check_read_gaps(h: FlatHistory, algo: int = RG_SEARCH, max_nodes: int = 0, flags: int = 0,
+                    per_gap: bool = False) -> dict:
+    """Twin of `jtb_check_read_gaps` (same result dict as `native.Context.check_read_gaps`).  per_gap=True adds
+    "per_gap": one code per :ok read in shard-major order, a full-key shard's gaps in gap order (0 explained, 1 KEY,
+    2 JOINT, 3 undecided; 3 for every read of a partial-read shard)."""
+    import numpy as np
+    ch = as_c_history(h)
+    shards = (abi.CRgShard * max(1, h.n_shards))()
+    res = abi.CRgResult()
+    codes = np.zeros(max(1, int(np.count_nonzero(h.f == 0))), np.int8)
+    rc = lib().jtbm_check_read_gaps(C.addressof(ch), max_nodes, flags, algo, C.addressof(shards), C.addressof(res),
+                                    codes.ctypes.data if per_gap else None)
+    if rc != 0:
+        raise RuntimeError(lib().jtbm_rg_last_error().decode())
+    out = abi.rg_to_dict(res, shards[:h.n_shards])
+    if per_gap:
+        out["per_gap"] = codes[:res.n_reads].tolist()
     return out
