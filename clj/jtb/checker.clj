@@ -504,6 +504,40 @@
                                                           :other-op (by-index (at (+ s 16))))))
           (and (= 2 (at s)) (<= 0 (at (+ s 11)))) (assoc :lower-op (by-index (at (+ s 11)))))))))
 
+;; ---- transfer placement -------------------------------------------------------------------------------------------
+(def ^:private tp-kind {1 :key 2 :joint 3 :double 4 :lost})
+
+(defn transfer-placement-checker
+  "The read-gap check with located transfers carried across gaps, on the GPU: a transfer one gap's search proves it
+  holds, or that only one gap of its window can still hold, is placed there and leaves the other gaps, which are
+  searched again without it until nothing moves ({:max-rounds n}, default 64).  Besides the read-gap errors, :lost
+  errors name a transfer known to be committed before some read that no gap can hold.  A gap the budget
+  ({:max-nodes n}) does not decide, and a shard with a partial read, make the verdict :unknown.  Add it to the compose
+  map at tests/ledger.clj:363-367 as `:transfer-placement (transfer-placement-checker {})`.
+  Result: {:valid? :read-count :transfer-count :explained-count :undecided-count :error-count :errors :placed-count
+  :rounds [:op :lower-op :error]}."
+  [opts]
+  (reify checker/Checker
+    (check [_ _test history _opts]
+      (let [{:keys [arrays by-index]} (flatten-history :ledger-lookups history)
+            res    (Native/checkTransferPlacement @ctx arrays (long (:max-nodes opts 0)) (int (:max-rounds opts 0)))
+            at     (fn [i] (aget res (int i)))
+            s      15                                     ; shard 0: valid cause reads transfers explained undecided ...
+            errors (into {} (for [k (range 4) :let [n (at (+ s 6 k))] :when (pos? n)] [(tp-kind (inc k)) n]))
+            kind   (at (+ s 15))
+            key    (at (+ s 16))]
+        (cond-> {:valid? (verdict (at s)) :read-count (at (+ s 2)) :transfer-count (at (+ s 3))
+                 :explained-count (at (+ s 4)) :undecided-count (at (+ s 5)) :error-count (reduce + (vals errors))
+                 :errors errors :placed-count (at (+ s 10)) :rounds (at (+ s 12))}
+          (= 2 (at s)) (assoc :op    (by-index (at (+ s 13)))
+                              :error (cond-> {:type (tp-kind kind) :round (at (+ s 17))
+                                              :eligible-count (at (+ s 21))}
+                                       (<= 0 key)       (assoc :key [(quot key 2) (counter-field (rem key 2))])
+                                       (= 1 kind)       (assoc :delta (at (+ s 18)))
+                                       (#{3 4} kind)    (assoc :transfer-id (at (+ s 19))
+                                                               :other-op (by-index (at (+ s 20))))))
+          (and (= 2 (at s)) (<= 0 (at (+ s 14)))) (assoc :lower-op (by-index (at (+ s 14)))))))))
+
 ;; ---- independent ----------------------------------------------------------------------------------------------
 (defn independent-checker
   "Like (independent/checker (checker/compose checkers)) for a map {name checker-kind} built from THIS namespace's

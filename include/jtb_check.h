@@ -24,7 +24,7 @@
 extern "C" {
 #endif
 
-#define JTB_ABI_VERSION 7
+#define JTB_ABI_VERSION 8
 
 /* ---- verdict lattice (jepsen.checker/merge-valid) ------------------------------------------- */
 #define JTB_VALID   0
@@ -484,6 +484,75 @@ typedef struct jtb_rg_result {
     double  seconds_total;      /* host wall time of the call incl. the host pass, H2D, D2H                           */
 } jtb_rg_result;
 
+/* ---- transfer-placement check (DESIGN.md "K12 transfer-placement check") --------------------------------------------
+ * Input, shards, reads, their order r_1 ... r_n, the gaps, Delta, M(t) and A(t): the read-gap check's.  Every transfer
+ * that is not :fail, has a positive amount and touches a key the shard observes gets a window of gaps [lo, hi]: t is in
+ * no gap before lo (some read at or before lo in the order completed before t was invoked, or A(t) > its completion),
+ * and a "must" transfer (M(t) < the invocation of some read) is in exactly one gap at or before hi, the gap of the first
+ * such read; a "may" transfer has hi = the last gap and may lie in none.  Then rounds (Jacobi: each reads only the state
+ * the previous one left):
+ *   - round 0 is the read-gap check, gap for gap (gather, caps, pruning, search, nodes, DOUBLE);
+ *   - after every round, per transfer: one the root pruning forced into exactly one gap this round is owned by it
+ *     (into two: DOUBLE); a must transfer with exactly one possible gap (gathered, and not pruned out there) left in its
+ *     window is owned by it (PLACE); one with none is LOST.  PLACE and LOST need every gap of the window complete
+ *     (not past the gather cap, at most JTB_TP_MAX_KEYS keys);
+ *   - round 1 re-runs every gap, round r >= 2 the gaps in the window of a transfer whose owner changed in round r - 1;
+ *     a re-run gap uses Delta' = Delta - the amounts of the transfers it owns (a negative component is KEY) and gathers
+ *     only the in-window transfers no gap owns;
+ *   - the rounds stop after a round r >= 1 that changes no owner, or after max_rounds.
+ * Anomalies latch (a gap unexplained in some round stays so, with its first kind).  A shard is JTB_INVALID on an
+ * unexplained gap, a DOUBLE or a LOST transfer, else JTB_UNKNOWN when a gap is undecided in the last round that ran it,
+ * else JTB_VALID. */
+#define JTB_TP_KEY    1 /* a gap with some Delta'_k < 0, or a key alone no subset of the gathered transfers closes    */
+#define JTB_TP_JOINT  2 /* every key alone closes, but no one subset closes all of them                               */
+#define JTB_TP_DOUBLE 3 /* a transfer the root pruning forces into two gaps in one round                              */
+#define JTB_TP_LOST   4 /* a must transfer with no possible gap left in its window                                    */
+#define JTB_TP_MAX_KEYS   JTB_RG_MAX_KEYS
+#define JTB_TP_MAX_GATHER JTB_RG_MAX_GATHER
+#define JTB_TP_MAX_FREE   JTB_RG_MAX_FREE
+#define JTB_TP_DEFAULT_MAX_NODES  JTB_RG_DEFAULT_MAX_NODES /* max_nodes <= 0 */
+#define JTB_TP_DEFAULT_MAX_ROUNDS 64                       /* max_rounds <= 0 */
+
+typedef struct jtb_tp_shard {
+    int32_t valid;              /* JTB_VALID / JTB_UNKNOWN / JTB_INVALID                                              */
+    int32_t cause;              /* JTB_CAUSE_PARTIAL_READ when a partial read makes the shard UNKNOWN, else 0         */
+    int32_t n_reads;            /* :ok reads of the shard; a full-key shard has as many gaps                          */
+    int32_t n_transfers;        /* transfer micro-ops of the shard (every fate)                                       */
+    int64_t n_explained;        /* gaps explained in the last round that ran them and never unexplained               */
+    int64_t n_undecided;        /* gaps undecided in the last round that ran them and never unexplained               */
+    int64_t count_by_kind[4];   /* unexplained gaps of kind KEY, of kind JOINT, DOUBLE transfers, LOST transfers      */
+    int64_t n_placed;           /* transfers owned by a gap at the fixpoint                                           */
+    int64_t nodes;              /* search nodes over every round                                                      */
+    int32_t rounds;             /* rounds that ran a gap of the shard                                                 */
+    int32_t witness_index;      /* completion :index of the read closing the witness gap (LOST: r at hi(t)), -1       */
+    int32_t lower_index;        /* completion :index of the read before it in the order, -1                           */
+    int32_t kind;               /* JTB_TP_KEY / JOINT / DOUBLE / LOST (the smallest at the witness gap), 0 without one */
+    int32_t key;                /* KEY / JOINT: as jtb_rg_shard.key; DOUBLE / LOST: -1                                */
+    int32_t round;              /* the round that found the witness, -1 without one                                   */
+    int64_t delta;              /* KEY: Delta'_k of key in that round                                                 */
+    int64_t transfer_id;        /* DOUBLE / LOST: the transfer's id (the smallest at the witness gap)                 */
+    int32_t other_index;        /* DOUBLE: completion :index of the read closing the other gap; LOST: the :index of
+                                   the event that fixes M(t); -1                                                      */
+    int32_t n_eligible;         /* transfers of the witness gap the root pruning kept in the last round that ran it   */
+} jtb_tp_shard;
+
+typedef struct jtb_tp_result {
+    int32_t valid;              /* merge-valid over shards                                                            */
+    int32_t n_failures;         /* shards that are not VALID                                                          */
+    int64_t n_reads;            /* :ok reads                                                                          */
+    int64_t n_transfers;        /* transfer micro-ops                                                                 */
+    int64_t n_explained;        /* gaps explained                                                                     */
+    int64_t n_unexplained;      /* gaps unexplained (KEY + JOINT)                                                     */
+    int64_t n_double;           /* DOUBLE transfers                                                                   */
+    int64_t n_lost;             /* LOST transfers                                                                     */
+    int64_t n_undecided;        /* gaps undecided                                                                     */
+    int64_t n_placed;           /* transfers owned at the fixpoint                                                    */
+    int64_t nodes;
+    int64_t rounds;             /* the most rounds of any shard                                                       */
+    double  seconds_kernel;     /* device time (CUDA events)                                                          */
+    double  seconds_total;      /* host wall time of the call incl. the host pass, H2D, D2H                           */
+} jtb_tp_result;
+
 typedef struct jtb_ctx jtb_ctx;
 
 /* ---- lifecycle -------------------------------------------------------------------------------- */
@@ -492,7 +561,7 @@ int         jtb_abi_version(void);
  * 0 jtb_history, 1 jtb_model, 2 jtb_opts, 3 jtb_lin_shard, 4 jtb_lin_result, 5 jtb_setfull_shard,
  * 6 jtb_setfull_out, 7 jtb_bank_result, 8 jtb_final_config, 9 jtb_mono_shard, 10 jtb_mono_result, 11 jtb_cb_shard,
  * 12 jtb_cb_result, 13 jtb_tl_shard, 14 jtb_tl_result, 15 jtb_rx_shard, 16 jtb_rx_result, 17 jtb_rg_shard,
- * 18 jtb_rg_result; -1 otherwise */
+ * 18 jtb_rg_result, 19 jtb_tp_shard, 20 jtb_tp_result; -1 otherwise */
 long        jtb_struct_size(int which);
 int         jtb_device_count(void);                 /* number of CUDA devices, <0 on error          */
 jtb_ctx*    jtb_create(const jtb_opts* opts);       /* NULL on failure (no CUDA device etc.)        */
@@ -573,6 +642,13 @@ int jtb_check_read_explanations(jtb_ctx* ctx, const jtb_history* h, int64_t max_
  * context stays usable). */
 int jtb_check_read_gaps(jtb_ctx* ctx, const jtb_history* h, int64_t max_nodes, int32_t flags, jtb_rg_shard* shards,
                         jtb_rg_result* out);
+
+/* ---- transfer-placement check (see jtb_tp_shard above) -------------------------------------------------------- *
+ * shards[n_shards] is caller-allocated; max_nodes <= 0 means JTB_TP_DEFAULT_MAX_NODES, max_rounds <= 0
+ * JTB_TP_DEFAULT_MAX_ROUNDS; flags is reserved and must be 0.  Returns 0 on success, <0 on the read-gap check's errors
+ * (jtb_last_error says which; the context stays usable). */
+int jtb_check_transfer_placement(jtb_ctx* ctx, const jtb_history* h, int64_t max_nodes, int32_t max_rounds,
+                                 int32_t flags, jtb_tp_shard* shards, jtb_tp_result* out);
 
 /* ---- multi-GPU fan-out inside the library (SURVEY §8(b) `n_gpus`, §8(e)) ----------------------------------- *
  * What `independent/checker` (set_full.clj:155) does over JVM threads, done over the GPUs of one box for a host

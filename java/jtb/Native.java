@@ -128,4 +128,15 @@ public final class Native {
      *     transferId, otherIndex, nEligible}
      */
     public static native long[] checkReadGaps(long ctx, Object[] history, long maxNodes);
+
+    /**
+     * {@code jtb_check_transfer_placement}: the read-gap check with located transfers carried across gaps to a
+     * fixpoint.  Input: the ledger-lookups form.  {@code maxNodes <= 0} and {@code maxRounds <= 0} are the defaults.
+     *
+     * @return {@code [valid, nFailures, nReads, nTransfers, nExplained, nUnexplained, nDouble, nLost, nUndecided,
+     *     nPlaced, nodes, rounds, kernelNs, totalNs, nShards]} followed by 22 longs per shard: {@code valid, cause,
+     *     nReads, nTransfers, nExplained, nUndecided, nKey, nJoint, nDouble, nLost, nPlaced, nodes, rounds,
+     *     witnessIndex, lowerIndex, kind, key, round, delta, transferId, otherIndex, nEligible}
+     */
+    public static native long[] checkTransferPlacement(long ctx, Object[] history, long maxNodes, int maxRounds);
 }

@@ -5,7 +5,7 @@ import ctypes as C
 
 from .history import MAX_ACCOUNTS
 
-ABI_VERSION = 7
+ABI_VERSION = 8
 OPT_NO_EAGER_READS = 1
 OPT_NO_SCOUTS = 2
 OPT_ENGINE_LEVEL = 4
@@ -28,6 +28,10 @@ RX_MAX_KEYS, RX_MAX_GATHER, RX_MAX_FREE, RX_DEFAULT_MAX_NODES = 256, 128, 64, 40
 RG_KEY, RG_JOINT, RG_DOUBLE = 1, 2, 3
 RG_KIND_NAME = {1: "key", 2: "joint", 3: "double"}
 RG_MAX_KEYS, RG_MAX_GATHER, RG_MAX_FREE, RG_DEFAULT_MAX_NODES = 256, 128, 64, 4096
+TP_KEY, TP_JOINT, TP_DOUBLE, TP_LOST = 1, 2, 3, 4
+TP_KIND_NAME = {1: "key", 2: "joint", 3: "double", 4: "lost"}
+TP_MAX_KEYS, TP_MAX_GATHER, TP_MAX_FREE, TP_DEFAULT_MAX_NODES = RG_MAX_KEYS, RG_MAX_GATHER, RG_MAX_FREE, 4096
+TP_DEFAULT_MAX_ROUNDS = 64
 SF_NEVER_READ, SF_STABLE, SF_LOST = 0, 1, 2
 BANK_OK, BANK_UNEXPECTED_KEY, BANK_NIL_BALANCE, BANK_WRONG_TOTAL, BANK_NEGATIVE_VALUE = range(5)
 BANK_ERR_NAME = {1: "unexpected-key", 2: "nil-balance", 3: "wrong-total", 4: "negative-value"}
@@ -283,5 +287,39 @@ def rg_to_dict(res, shards) -> dict:
         "n_undecided": res.n_undecided, "nodes": res.nodes, "seconds_kernel": res.seconds_kernel,
         "seconds_total": res.seconds_total,
         "shards": [{f: (list(s.count_by_kind) if f == "count_by_kind" else getattr(s, f)) for f in RG_SHARD_FIELDS}
+                   for s in shards],
+    }
+
+
+class CTpShard(C.Structure):
+    """jtb_tp_shard: the transfer-placement verdict of one shard."""
+    _fields_ = [("valid", C.c_int32), ("cause", C.c_int32), ("n_reads", C.c_int32), ("n_transfers", C.c_int32),
+                ("n_explained", C.c_int64), ("n_undecided", C.c_int64), ("count_by_kind", C.c_int64 * 4),
+                ("n_placed", C.c_int64), ("nodes", C.c_int64), ("rounds", C.c_int32), ("witness_index", C.c_int32),
+                ("lower_index", C.c_int32), ("kind", C.c_int32), ("key", C.c_int32), ("round", C.c_int32),
+                ("delta", C.c_int64), ("transfer_id", C.c_int64), ("other_index", C.c_int32),
+                ("n_eligible", C.c_int32)]
+
+
+class CTpResult(C.Structure):
+    _fields_ = [("valid", C.c_int32), ("n_failures", C.c_int32), ("n_reads", C.c_int64), ("n_transfers", C.c_int64),
+                ("n_explained", C.c_int64), ("n_unexplained", C.c_int64), ("n_double", C.c_int64),
+                ("n_lost", C.c_int64), ("n_undecided", C.c_int64), ("n_placed", C.c_int64), ("nodes", C.c_int64),
+                ("rounds", C.c_int64), ("seconds_kernel", C.c_double), ("seconds_total", C.c_double)]
+
+
+TP_SHARD_FIELDS = ("valid", "cause", "n_reads", "n_transfers", "n_explained", "n_undecided", "count_by_kind",
+                   "n_placed", "nodes", "rounds", "witness_index", "lower_index", "kind", "key", "round", "delta",
+                   "transfer_id", "other_index", "n_eligible")
+
+
+def tp_to_dict(res, shards) -> dict:
+    """One result dict for the library and the oracle (count_by_kind as a list indexed by kind - 1)."""
+    return {
+        "valid": res.valid, "n_failures": res.n_failures, "n_reads": res.n_reads, "n_transfers": res.n_transfers,
+        "n_explained": res.n_explained, "n_unexplained": res.n_unexplained, "n_double": res.n_double,
+        "n_lost": res.n_lost, "n_undecided": res.n_undecided, "n_placed": res.n_placed, "nodes": res.nodes,
+        "rounds": res.rounds, "seconds_kernel": res.seconds_kernel, "seconds_total": res.seconds_total,
+        "shards": [{f: (list(s.count_by_kind) if f == "count_by_kind" else getattr(s, f)) for f in TP_SHARD_FIELDS}
                    for s in shards],
     }

@@ -522,6 +522,67 @@ class ReadGaps(Checker, _Native):
         return out
 
 
+class TransferPlacement(Checker, _Native):
+    """The read-gap check with located transfers carried across gaps, on the GPU (K12).
+
+    Reads the ledger-lookups form and orders and gaps the reads as the read-gap check does.  A transfer that one gap's
+    search proves it must hold, or that only one gap of its window can still hold, is placed there and leaves every
+    other gap, which is then searched again without it, round after round until nothing moves (max-rounds, default
+    64).  Besides the read-gap errors ("key", "joint", "double") a transfer known to be committed before some read that
+    no gap can hold is a "lost" error.  Shards with a partial read are :unknown; a gap the budget (max-nodes, default
+    4096) does not decide makes the verdict :unknown, never false.
+    Result: {valid?, read-count, transfer-count, explained-count, undecided-count, error-count, errors {kind count},
+    placed-count, rounds, [op, lower-op, error]}."""
+
+    def __init__(self, checker_opts: Mapping[str, Any] | None = None, ctx: Context | None = None,
+                 **ctx_opts) -> None:
+        _Native.__init__(self, ctx, **ctx_opts)
+        self.max_nodes = int((checker_opts or {}).get("max-nodes", 0))
+        self.max_rounds = int((checker_opts or {}).get("max-rounds", 0))
+
+    def _shard_map(self, s: dict) -> dict:
+        errors = {abi.TP_KIND_NAME[k + 1]: n for k, n in enumerate(s["count_by_kind"]) if n}
+        m: dict[str, Any] = {"valid?": VERDICT_NAME[s["valid"]], "read-count": s["n_reads"],
+                             "transfer-count": s["n_transfers"], "explained-count": s["n_explained"],
+                             "undecided-count": s["n_undecided"], "error-count": sum(errors.values()),
+                             "errors": errors, "placed-count": s["n_placed"], "rounds": s["rounds"]}
+        if s["cause"]:
+            m["cause"] = abi.CAUSE_NAME.get(s["cause"], "unknown")
+        if s["valid"] == INVALID:
+            m["op"] = {"index": s["witness_index"]}
+            if s["lower_index"] >= 0:
+                m["lower-op"] = {"index": s["lower_index"]}
+            err: dict[str, Any] = {"type": abi.TP_KIND_NAME[s["kind"]], "round": s["round"],
+                                   "eligible-count": s["n_eligible"]}
+            k = s["key"]
+            if k >= 0:
+                err["key"] = [k >> 1, COUNTER_FIELDS[k & 1]]
+            if s["kind"] == abi.TP_KEY:
+                err["delta"] = s["delta"]
+            if s["kind"] in (abi.TP_DOUBLE, abi.TP_LOST):
+                err.update({"transfer-id": s["transfer_id"], "other-op": {"index": s["other_index"]}})
+            m["error"] = err
+        return m
+
+    def check_flat(self, test, h: FlatHistory) -> tuple[dict, list[dict]]:
+        r = self.ctx.check_transfer_placement(h, self.max_nodes, self.max_rounds)
+        top = {"valid?": VERDICT_NAME[r["valid"]], "read-count": r["n_reads"], "transfer-count": r["n_transfers"],
+               "explained-count": r["n_explained"], "undecided-count": r["n_undecided"],
+               "error-count": r["n_unexplained"] + r["n_double"] + r["n_lost"], "placed-count": r["n_placed"],
+               "rounds": r["rounds"], "nodes": r["nodes"], "seconds-kernel": r["seconds_kernel"],
+               "seconds-total": r["seconds_total"]}
+        return top, [self._shard_map(s) for s in r["shards"]]
+
+    def check(self, test, history, opts=None) -> dict:
+        h = _flat(history, "ledger-lookups")
+        if h.n_shards != 1:
+            raise ValueError("history has independent keys: wrap with independent_checker(...)")
+        top, per = self.check_flat(test, h)
+        out = dict(per[0])
+        out.update({k: v for k, v in top.items() if k.startswith("seconds-") or k == "nodes"})
+        return out
+
+
 class Compose(Checker):
     """`(checker/compose {name checker ...})`: run each, `:valid?` = merge-valid of the results."""
 
@@ -554,13 +615,13 @@ class Independent(Checker):
             return c.model
         if isinstance(c, (MonotonicKeys, CounterBounds)):
             return "ledger-counters"
-        if isinstance(c, (TransferLookups, ReadExplanations, ReadGaps)):
+        if isinstance(c, (TransferLookups, ReadExplanations, ReadGaps, TransferPlacement)):
             return "ledger-lookups"
         return "set"
 
     def _per_key(self, checker: Checker, test, h: FlatHistory, opts) -> list[dict]:
         if isinstance(checker, (Linearizable, SetFull, ReadAllInvokedAdds, MonotonicKeys, CounterBounds,
-                                TransferLookups, ReadExplanations, ReadGaps)):
+                                TransferLookups, ReadExplanations, ReadGaps, TransferPlacement)):
             try:
                 return checker.check_flat(test, h)[1]
             except Exception:  # noqa: BLE001
@@ -635,6 +696,12 @@ def read_gap_checker(opts: Mapping[str, Any] | None = None, **kw) -> ReadGaps:
     """Whether the transfers committed between two successive ledger reads explain what changed (K11);
     {"max-nodes": n} sets the per-gap search budget."""
     return ReadGaps(opts, **kw)
+
+
+def transfer_placement_checker(opts: Mapping[str, Any] | None = None, **kw) -> TransferPlacement:
+    """The read-gap check with located transfers carried across gaps to a fixpoint (K12); {"max-nodes": n} sets the
+    per-gap search budget and {"max-rounds": n} the number of rounds."""
+    return TransferPlacement(opts, **kw)
 
 
 def compose(checkers: Mapping[str, Checker]) -> Compose:
@@ -805,13 +872,15 @@ def final_reads() -> FinalReads:
 def ledger_checker(checker_opts: Mapping[str, Any] | None = None, ctx: Context | None = None,
                    linear: bool = True, monotonic: bool = False, counter_bounds: bool = False,
                    transfer_lookups: bool = False, read_explanations: bool = False,
-                   read_gaps: bool = False) -> Compose:
+                   read_gaps: bool = False, transfer_placement: bool = False) -> Compose:
     """The ledger test's checker (tests/ledger.clj:363-367) minus the gnuplot plotter, plus the
     linearizability search the north-star adds and, with monotonic=True, the monotonic-key check, with
     counter_bounds=True, the counter-bounds check, with transfer_lookups=True, the transfer-lookup check, with
-    read_explanations=True, the read-explanation check and, with read_gaps=True, the read-gap check:
+    read_explanations=True, the read-explanation check, with read_gaps=True, the read-gap check and, with
+    transfer_placement=True, the transfer-placement check:
         {:SI (checker opts) :lookup-transfers ... :final-reads ... :unexpected-ops ... [:linear ...] [:monotonic ...]
-         [:counter-bounds ...] [:transfer-lookups ...] [:read-explanations ...] [:read-gaps ...]}"""
+         [:counter-bounds ...] [:transfer-lookups ...] [:read-explanations ...] [:read-gaps ...]
+         [:transfer-placement ...]}"""
     cs: dict[str, Checker] = {"SI": bank_checker(checker_opts, ctx=ctx),
                               "lookup-transfers": lookup_all_invoked_transfers(),
                               "final-reads": final_reads(), "unexpected-ops": unexpected_ops()}
@@ -827,4 +896,6 @@ def ledger_checker(checker_opts: Mapping[str, Any] | None = None, ctx: Context |
         cs["read-explanations"] = read_explanation_checker(ctx=ctx)
     if read_gaps:
         cs["read-gaps"] = read_gap_checker(ctx=ctx)
+    if transfer_placement:
+        cs["transfer-placement"] = transfer_placement_checker(ctx=ctx)
     return compose(cs)

@@ -22,6 +22,7 @@
 #include "jtb_transfer_lookups.cuh"
 #include "jtb_read_explanations.cuh"
 #include "jtb_read_gaps.cuh"
+#include "jtb_transfer_placement.cuh"
 
 using namespace jtb;
 
@@ -735,6 +736,8 @@ long jtb_struct_size(int which) {
     case 16: return sizeof(jtb_rx_result);
     case 17: return sizeof(jtb_rg_shard);
     case 18: return sizeof(jtb_rg_result);
+    case 19: return sizeof(jtb_tp_shard);
+    case 20: return sizeof(jtb_tp_result);
     }
     return -1;
 }
@@ -1154,6 +1157,17 @@ int jtb_check_read_gaps(jtb_ctx* ctx, const jtb_history* h, int64_t max_nodes, i
     if (cudaSetDevice(ctx->device) != cudaSuccess) { ctx->err = "cudaSetDevice failed"; return -1; }
     ctx->fc.valid = false;
     return run_read_gaps(ctx->stream, ctx->ev0, ctx->ev1, h, max_nodes, flags, shards, out, ctx->err);
+}
+
+// K12: the transfer-placement check (csrc/jtb_transfer_placement.cuh)
+int jtb_check_transfer_placement(jtb_ctx* ctx, const jtb_history* h, int64_t max_nodes, int32_t max_rounds,
+                                 int32_t flags, jtb_tp_shard* shards, jtb_tp_result* out) {
+    if (!ctx) return -1;
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    if (cudaSetDevice(ctx->device) != cudaSuccess) { ctx->err = "cudaSetDevice failed"; return -1; }
+    ctx->fc.valid = false;
+    return run_transfer_placement(ctx->stream, ctx->ev0, ctx->ev1, h, max_nodes, max_rounds, flags, shards, out,
+                                  ctx->err);
 }
 
 // SURVEY 8(f) N2: the step before the checkers (independent/subhistory, ledger->bank) on the device

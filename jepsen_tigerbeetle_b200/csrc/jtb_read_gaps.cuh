@@ -91,6 +91,66 @@ struct RgWarp {
     int32_t ct[JTB_RG_MAX_GATHER];
 };
 
+// The gather of the gap closed by a read completed at cp over the previous read invoked at ivl (-1 for gap 0), Delta
+// and the keys in W: the shard's eligible transfers that fit under Delta and pass extra(t), into the candidate arrays
+// of W and G.ct.  Returns how many there are; more than JTB_RG_MAX_GATHER means the gap has too many (the arrays hold
+// the first ones).
+template <class Extra>
+__device__ __forceinline__ int32_t rg_gather(const RgDev& d, RgWarp& G, int32_t s, int32_t K, int32_t cp, int32_t ivl,
+                                             int lane, Extra extra) {
+    RxWarp& W = G.x;
+    int32_t n = 0;
+    auto find = [&](int64_t k) {
+        int32_t a = 0, b = K;
+        while (a < b) {
+            const int32_t c = (a + b) >> 1;
+            if (W.key[c] < k) a = c + 1; else b = c;
+        }
+        return (int16_t)(a < K && W.key[a] == k ? a : -1);
+    };
+    auto take = [&](bool valid, int32_t t) {
+        int16_t jd = -1, jc = -1;
+        int32_t a = 0;
+        if (valid) {
+            const int32_t* q = d.t_rec + 3 * (int64_t)t;
+            a = q[2];
+            valid = !(d.t_M[t] < ivl) && d.t_A[t] < cp && a > 0 && extra(t);
+            if (valid) {
+                jd = find(2 * (int64_t)q[0]);
+                jc = find(2 * (int64_t)q[1] + 1);
+                valid = (jd >= 0 || jc >= 0) && (jd < 0 || a <= W.d[jd]) && (jc < 0 || a <= W.d[jc]);
+            }
+        }
+        const unsigned bal = __ballot_sync(0xffffffffu, valid);
+        const int32_t at = n + __popc(bal & ((1u << lane) - 1));
+        if (valid && at < JTB_RG_MAX_GATHER) {
+            W.cid[at] = d.t_id[t];
+            W.ca[at] = a;
+            W.cjd[at] = jd;
+            W.cjc[at] = jc;
+            G.ct[at] = t;
+        }
+        n += __popc(bal);
+    };
+    const int32_t olo = d.ok_off[s], b = rx_lower(d.ok_inv, olo, d.ok_off[s + 1], cp);
+    for (int32_t base = b - 1; base >= olo && n <= JTB_RG_MAX_GATHER; base -= 32) {
+        const int32_t j = base - lane;
+        const bool valid = j >= olo && d.ok_pmax[j] >= ivl;
+        if (!__any_sync(0xffffffffu, valid)) break;
+        take(valid, valid ? d.ok_t[j] : 0);
+    }
+    for (int32_t c = 0; c < K && n <= JTB_RG_MAX_GATHER; ++c) {
+        if (W.d[c] <= 0) continue;   // a crashed transfer anchored at c needs its amount <= Delta_c
+        const int64_t slot = d.key_off[s] + c;
+        const int32_t clo = d.cr_off[slot], bc = rx_lower(d.cr_inv, clo, d.cr_off[slot + 1], cp);
+        for (int32_t base = clo; base < bc && n <= JTB_RG_MAX_GATHER; base += 32) {
+            const int32_t j = base + lane;
+            take(j < bc, j < bc ? d.cr_t[j] : 0);
+        }
+    }
+    return n;
+}
+
 // warp per gap
 __global__ void __launch_bounds__(RG_WARPS * 32) rg_gaps(RgDev d) {
     __shared__ RgWarp smem[RG_WARPS];
@@ -129,55 +189,7 @@ __global__ void __launch_bounds__(RG_WARPS * 32) rg_gaps(RgDev d) {
             code = RX_EXPLAINED;
         } else {
             // gather the eligible transfers that fit under Delta; n > cap = too many
-            int32_t n = 0;
-            auto find = [&](int64_t k) {
-                int32_t a = 0, b = K;
-                while (a < b) {
-                    const int32_t c = (a + b) >> 1;
-                    if (W.key[c] < k) a = c + 1; else b = c;
-                }
-                return (int16_t)(a < K && W.key[a] == k ? a : -1);
-            };
-            auto take = [&](bool valid, int32_t t) {
-                int16_t jd = -1, jc = -1;
-                int32_t a = 0;
-                if (valid) {
-                    const int32_t* q = d.t_rec + 3 * (int64_t)t;
-                    a = q[2];
-                    valid = !(d.t_M[t] < ivl) && d.t_A[t] < cp && a > 0;
-                    if (valid) {
-                        jd = find(2 * (int64_t)q[0]);
-                        jc = find(2 * (int64_t)q[1] + 1);
-                        valid = (jd >= 0 || jc >= 0) && (jd < 0 || a <= W.d[jd]) && (jc < 0 || a <= W.d[jc]);
-                    }
-                }
-                const unsigned bal = __ballot_sync(0xffffffffu, valid);
-                const int32_t at = n + __popc(bal & ((1u << lane) - 1));
-                if (valid && at < JTB_RG_MAX_GATHER) {
-                    W.cid[at] = d.t_id[t];
-                    W.ca[at] = a;
-                    W.cjd[at] = jd;
-                    W.cjc[at] = jc;
-                    G.ct[at] = t;
-                }
-                n += __popc(bal);
-            };
-            const int32_t olo = d.ok_off[s], b = rx_lower(d.ok_inv, olo, d.ok_off[s + 1], cp);
-            for (int32_t base = b - 1; base >= olo && n <= JTB_RG_MAX_GATHER; base -= 32) {
-                const int32_t j = base - lane;
-                const bool valid = j >= olo && d.ok_pmax[j] >= ivl;
-                if (!__any_sync(0xffffffffu, valid)) break;
-                take(valid, valid ? d.ok_t[j] : 0);
-            }
-            for (int32_t c = 0; c < K && n <= JTB_RG_MAX_GATHER; ++c) {
-                if (W.d[c] <= 0) continue;   // a crashed transfer anchored at c needs its amount <= Delta_c
-                const int64_t slot = d.key_off[s] + c;
-                const int32_t clo = d.cr_off[slot], bc = rx_lower(d.cr_inv, clo, d.cr_off[slot + 1], cp);
-                for (int32_t base = clo; base < bc && n <= JTB_RG_MAX_GATHER; base += 32) {
-                    const int32_t j = base + lane;
-                    take(j < bc, j < bc ? d.cr_t[j] : 0);
-                }
-            }
+            const int32_t n = rg_gather(d, G, s, K, cp, ivl, lane, [](int32_t) { return true; });
             __syncwarp();
             if (n <= JTB_RG_MAX_GATHER) {
                 // the root pruning once more, as rx_search starts, to record the transfers it forces in

@@ -20,14 +20,14 @@ _SOURCES = ["jtb_abi.cu", "jtb_prep.cpp", "jtb_multi.cpp"]
 _DEPS = _SOURCES + ["jtb_prep.h", "jtb_expand.h", "jtb_wgl.cuh", "jtb_scout.cuh", "jtb_scans.cuh",
                     "jtb_table_bench.cuh", "jtb_level.cuh", "jtb_partition.cuh", "jtb_monotonic.cuh",
                     "jtb_counter_bounds.cuh", "jtb_transfer_lookups.cuh", "jtb_read_explanations.cuh",
-                    "jtb_read_gaps.cuh", "jtb_call.cuh"]
+                    "jtb_read_gaps.cuh", "jtb_transfer_placement.cuh", "jtb_call.cuh"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared", "-ldl"]
 
 EXPORTS = ["jtb_abi_version", "jtb_device_count", "jtb_create", "jtb_destroy", "jtb_last_error",
            "jtb_check_linearizable", "jtb_check_set_full", "jtb_check_bank_totals", "jtb_check_monotonic_keys",
            "jtb_check_counter_bounds", "jtb_check_transfer_lookups", "jtb_check_read_explanations",
-           "jtb_check_read_gaps",
+           "jtb_check_read_gaps", "jtb_check_transfer_placement",
            "jtb_table_bench", "jtb_get_stats", "jtb_struct_size", "jtb_prepare_seconds", "jtb_prepare_info",
            "jtb_final_configs", "jtb_gather_bench", "jtb_host_alloc", "jtb_host_free", "jtb_partition_by_key", "jtb_ledger_balances", "jtb_multi_create", "jtb_multi_create_error", "jtb_multi_destroy", "jtb_multi_n_gpus",
            "jtb_multi_last_error", "jtb_multi_check_linearizable", "jtb_multi_check_set_full"]
@@ -82,6 +82,8 @@ def lib() -> C.CDLL:
             L.jtb_check_read_explanations.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p,
                                                       C.c_void_p]
             L.jtb_check_read_gaps.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p]
+            L.jtb_check_transfer_placement.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_int32,
+                                                       C.c_void_p, C.c_void_p]
             L.jtb_table_bench.argtypes = [C.c_void_p, C.c_uint64, C.c_int, C.c_int, C.c_void_p,
                                           C.c_void_p, C.c_void_p]
             L.jtb_gather_bench.argtypes = [C.c_void_p, C.c_uint64, C.c_int, C.c_int, C.c_uint32, C.c_int, C.c_int,
@@ -262,6 +264,25 @@ class Context:
         if rc != 0:
             raise NativeError(f"jtb_check_read_gaps rc={rc}: {self._err()}")
         return abi.rg_to_dict(res, shards[:h.n_shards])
+
+    # ---- K12: transfer-placement check ---------------------------------------------------------------------------
+    def check_transfer_placement(self, h: FlatHistory, max_nodes: int = 0, max_rounds: int = 0) -> dict:
+        """The read-gap check, with every transfer a gap's root pruning locates (or that only one gap of its window
+        can still hold) carried into the other gaps, round after round to a fixpoint; a transfer known to be committed
+        that no gap of its window can hold is LOST (input: the ledger-lookups form; max_nodes <= 0 and max_rounds <= 0
+        are the defaults).  {"valid", "n_failures", "n_reads", "n_transfers", "n_explained", "n_unexplained",
+        "n_double", "n_lost", "n_undecided", "n_placed", "nodes", "rounds", "seconds_kernel", "seconds_total",
+        "shards": [{"valid", "cause", "n_reads", "n_transfers", "n_explained", "n_undecided", "count_by_kind",
+        "n_placed", "nodes", "rounds", "witness_index", "lower_index", "kind", "key", "round", "delta", "transfer_id",
+        "other_index", "n_eligible"}]}; count_by_kind[kind - 1]."""
+        ch = as_c_history(h)
+        shards = (abi.CTpShard * max(1, h.n_shards))()
+        res = abi.CTpResult()
+        rc = lib().jtb_check_transfer_placement(self._h, C.addressof(ch), max_nodes, max_rounds, 0,
+                                                C.addressof(shards), C.addressof(res))
+        if rc != 0:
+            raise NativeError(f"jtb_check_transfer_placement rc={rc}: {self._err()}")
+        return abi.tp_to_dict(res, shards[:h.n_shards])
 
     def final_configs(self, h: FlatHistory, model: CModel, shard: int = 0, cap: int = 10) -> dict:
         """knossos' :configs of an INVALID shard (`jtb_final_configs`): call directly after `check_linearizable`

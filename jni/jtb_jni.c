@@ -541,3 +541,46 @@ JNIEXPORT jlongArray JNICALL Java_jtb_Native_checkReadGaps(JNIEnv* env, jclass c
     free(shards);
     return out;
 }
+
+/* ---- K12: transfer-placement check ------------------------------------------------------------------------------ */
+JNIEXPORT jlongArray JNICALL Java_jtb_Native_checkTransferPlacement(JNIEnv* env, jclass cls, jlong handle,
+                                                                    jobjectArray history, jlong max_nodes,
+                                                                    jint max_rounds) {
+    (void)cls;
+    jtb_history hist;
+    hist_pins pins;
+    if (pin_history(env, history, &hist, &pins)) return NULL;
+    const int ns = hist.n_shards;
+    jtb_tp_shard* shards = (jtb_tp_shard*)calloc(ns > 0 ? (size_t)ns : 1, sizeof *shards);
+    jtb_tp_result r;
+    memset(&r, 0, sizeof r);
+    const int rc = jtb_check_transfer_placement((jtb_ctx*)(intptr_t)handle, &hist, (int64_t)max_nodes,
+                                                (int32_t)max_rounds, 0, shards, &r);
+    unpin_history(env, &pins);
+    if (rc != 0) {
+        free(shards);
+        throw_rt(env, jtb_last_error((jtb_ctx*)(intptr_t)handle));
+        return NULL;
+    }
+    const int64_t total = 15 + 22ll * ns;
+    jlong* v = (jlong*)calloc((size_t)total, sizeof *v);
+    int64_t k = 0;
+    v[k++] = r.valid; v[k++] = r.n_failures; v[k++] = r.n_reads; v[k++] = r.n_transfers; v[k++] = r.n_explained;
+    v[k++] = r.n_unexplained; v[k++] = r.n_double; v[k++] = r.n_lost; v[k++] = r.n_undecided; v[k++] = r.n_placed;
+    v[k++] = r.nodes; v[k++] = r.rounds; v[k++] = ns_of(r.seconds_kernel); v[k++] = ns_of(r.seconds_total);
+    v[k++] = ns;
+    for (int s = 0; s < ns; ++s) {
+        const jtb_tp_shard* q = &shards[s];
+        v[k++] = q->valid; v[k++] = q->cause; v[k++] = q->n_reads; v[k++] = q->n_transfers; v[k++] = q->n_explained;
+        v[k++] = q->n_undecided; v[k++] = q->count_by_kind[0]; v[k++] = q->count_by_kind[1];
+        v[k++] = q->count_by_kind[2]; v[k++] = q->count_by_kind[3]; v[k++] = q->n_placed; v[k++] = q->nodes;
+        v[k++] = q->rounds; v[k++] = q->witness_index; v[k++] = q->lower_index; v[k++] = q->kind; v[k++] = q->key;
+        v[k++] = q->round; v[k++] = q->delta; v[k++] = q->transfer_id; v[k++] = q->other_index;
+        v[k++] = q->n_eligible;
+    }
+    jlongArray out = (*env)->NewLongArray(env, (jsize)k);
+    if (out) (*env)->SetLongArrayRegion(env, out, 0, (jsize)k, v);
+    free(v);
+    free(shards);
+    return out;
+}

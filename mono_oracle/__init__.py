@@ -8,7 +8,8 @@ pair and every (read, key, lookup) triple; TL_SWEEP walks with hash maps, sorted
 minima.  See transfer_lookups.cpp.  RX_BRUTE enumerates every subset of a read's "may" transfers; RX_SEARCH is the
 library's budgeted pruning and depth-first search over a sweep.  See read_explanations.cpp.  RG_BRUTE enumerates every
 subset of a gap's eligible transfers; RG_SEARCH is the library's amount filter, caps and search per gap.  See
-read_gaps.cpp."""
+read_gaps.cpp.  TP_BRUTE enumerates every placement of each transfer in a gap of its window; TP_SEARCH is the
+library's rounds of per-gap searches with owned transfers carried between gaps.  See transfer_placement.cpp."""
 from __future__ import annotations
 
 import ctypes as C
@@ -24,6 +25,7 @@ CB_LITERAL, CB_SWEEP = 0, 1
 TL_LITERAL, TL_SWEEP = 0, 1
 RX_BRUTE, RX_SEARCH = 0, 1
 RG_BRUTE, RG_SEARCH = 0, 1
+TP_BRUTE, TP_SEARCH = 0, 1
 DECIDE_PARTIAL = 1 << 16   # decide shards with partial reads instead of reporting them UNKNOWN
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB = None
@@ -34,7 +36,8 @@ def build(force: bool = False) -> str:
     temporary directory instead."""
     so = os.path.join(_HERE, "libjtb_mono_oracle.so")
     srcs = [os.path.join(_HERE, f) for f in ("mono_oracle.cpp", "counter_bounds.cpp", "transfer_lookups.cpp",
-                                                "read_explanations.cpp", "read_gaps.cpp", "Makefile")]
+                                                "read_explanations.cpp", "read_gaps.cpp", "transfer_placement.cpp",
+                                                "gaps_common.h", "Makefile")]
     srcs.append(os.path.join(_HERE, "..", "include", "jtb_check.h"))
     stale = not os.path.exists(so) or any(os.path.getmtime(s) > os.path.getmtime(so) for s in srcs)
     if force or stale:
@@ -62,6 +65,9 @@ def lib() -> C.CDLL:
         _LIB.jtbm_rg_last_error.restype = C.c_char_p
         _LIB.jtbm_check_read_gaps.argtypes = [C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
                                               C.c_void_p]
+        _LIB.jtbm_tp_last_error.restype = C.c_char_p
+        _LIB.jtbm_check_transfer_placement.argtypes = [C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_int32,
+                                                       C.c_void_p, C.c_void_p]
     return _LIB
 
 
@@ -138,3 +144,17 @@ def check_read_gaps(h: FlatHistory, algo: int = RG_SEARCH, max_nodes: int = 0, f
     if per_gap:
         out["per_gap"] = codes[:res.n_reads].tolist()
     return out
+
+
+def check_transfer_placement(h: FlatHistory, algo: int = TP_SEARCH, max_nodes: int = 0, max_rounds: int = 0,
+                             flags: int = 0) -> dict:
+    """Twin of `jtb_check_transfer_placement` (same result dict as `native.Context.check_transfer_placement`).
+    TP_BRUTE fills only the verdict, the cause and the read and transfer counts."""
+    ch = as_c_history(h)
+    shards = (abi.CTpShard * max(1, h.n_shards))()
+    res = abi.CTpResult()
+    rc = lib().jtbm_check_transfer_placement(C.addressof(ch), max_nodes, max_rounds, flags, algo,
+                                             C.addressof(shards), C.addressof(res))
+    if rc != 0:
+        raise RuntimeError(lib().jtbm_tp_last_error().decode())
+    return abi.tp_to_dict(res, shards[:h.n_shards])

@@ -1,0 +1,331 @@
+// gaps_common.h — what the CPU oracles of the read-gap and the transfer-placement checks share (TEST INFRASTRUCTURE
+// ONLY): the shard parse, M(t) and A(t), a gap's subset-sum problem, its brute force, the library's search and the
+// sweep structures of the gather.  Its anonymous namespace gives each oracle a copy of its own.
+#pragma once
+#include <algorithm>
+#include <climits>
+#include <cstdint>
+#include <cstdio>
+#include <string>
+#include <unordered_map>
+#include <unordered_set>
+#include <utility>
+#include <vector>
+
+#include "../include/jtb_check.h"
+
+namespace {
+
+constexpr int RG_BRUTE = 0, RG_SEARCH = 1;
+constexpr int32_t NONE = INT_MAX;
+// per-gap codes of the optional per-gap output
+constexpr int8_t G_EXPLAINED = 0, G_UNDECIDED = 3;
+
+thread_local std::string g_err;
+
+struct XRead {
+    int32_t inv, comp, comp_index;
+    std::vector<std::pair<int32_t, int64_t>> kv;   // sorted by key
+};
+
+struct XTransfer {
+    int64_t id;
+    int32_t debit, credit, amount, inv;
+    int32_t fate = -1, okcomp = NONE;
+    int32_t M = NONE, A = -1;
+};
+
+struct XLookup {
+    int32_t inv, comp;
+    std::unordered_set<int64_t> ids;
+};
+
+struct Shard {
+    std::vector<XRead> R;
+    std::vector<XTransfer> T;
+    std::vector<XLookup> L;
+};
+
+inline int64_t rec_id(const int32_t* r) { return (int64_t)(((uint64_t)(uint32_t)r[1] << 32) | (uint32_t)r[0]); }
+
+int fail(const char* fmt, int32_t index, int64_t x = 0) {
+    char buf[256];
+    snprintf(buf, sizeof buf, fmt, index, (long long)x);
+    g_err = buf;
+    return -2;
+}
+
+int parse_shard(const jtb_history* h, int32_t s, Shard& S, int64_t& n_records) {
+    const int64_t lo = h->shard_off[s], hi = h->shard_off[s + 1];
+    std::unordered_map<int32_t, int32_t> last_inv;
+    std::unordered_map<int32_t, std::vector<size_t>> open;
+    std::unordered_set<int64_t> ids;
+    for (int64_t e = lo; e < hi; ++e) {
+        const int32_t p = h->process[e], pos = (int32_t)(e - lo);
+        if (p < 0) continue;
+        auto ot = open.find(p);
+        if (ot != open.end()) {
+            if (h->type[e] != JTB_T_INVOKE)
+                for (size_t t : ot->second) {
+                    S.T[t].fate = h->type[e];
+                    if (h->type[e] == JTB_T_OK) S.T[t].okcomp = pos;
+                }
+            open.erase(ot);
+        }
+        const int32_t len = h->payload_len[e];
+        const int64_t off = h->payload_off[e];
+        if (h->type[e] == JTB_T_INVOKE) {
+            last_inv[p] = pos;
+            if (h->f[e] != JTB_F_TRANSFER) continue;
+            if (len <= 0) return fail("transfer at :index %d: an invoke without ids", h->index[e]);
+            if (len % 5 != 0) return fail("transfer at :index %d: payload length %lld is not a multiple of 5",
+                                          h->index[e], len);
+            if (off < 0 || off + len > h->n_payload) return fail("transfer at :index %d: payload out of range",
+                                                                h->index[e]);
+            auto& o = open[p];
+            for (int32_t j = 0; j < len; j += 5) {
+                const int32_t* r = h->payload + off + j;
+                if (r[4] < 0) return fail("transfer at :index %d: negative amount %lld", h->index[e], r[4]);
+                if (r[2] < 0 || r[2] >= (1 << 30) || r[3] < 0 || r[3] >= (1 << 30))
+                    return fail("transfer at :index %d: account outside [0, 2^30)", h->index[e]);
+                const int64_t id = rec_id(r);
+                if (!ids.insert(id).second)
+                    return fail("transfer at :index %d: id %lld is carried by two transfer invokes", h->index[e], id);
+                XTransfer t;
+                t.id = id; t.debit = r[2]; t.credit = r[3]; t.amount = r[4]; t.inv = pos;
+                o.push_back(S.T.size());
+                S.T.push_back(t);
+            }
+            continue;
+        }
+        if (h->type[e] != JTB_T_OK || len < 0) continue;
+        auto it = last_inv.find(p);
+        const int32_t inv = it == last_inv.end() ? -1 : it->second;
+        if (h->f[e] == JTB_F_LOOKUP) {
+            if (len % 5 != 0) return fail("lookup at :index %d: payload length %lld is not a multiple of 5",
+                                          h->index[e], len);
+            if (off < 0 || off + len > h->n_payload) return fail("lookup at :index %d: payload out of range",
+                                                                h->index[e]);
+            n_records += len / 5;
+            if (n_records > INT_MAX) { g_err = "more than 2^31-1 lookup records"; return -2; }
+            XLookup l{inv, pos, {}};
+            for (int32_t j = 0; j < len; j += 5) l.ids.insert(rec_id(h->payload + off + j));
+            S.L.push_back(std::move(l));
+            continue;
+        }
+        if (h->f[e] != JTB_F_READ) continue;
+        if (len % 3 != 0 || off < 0 || off + len > h->n_payload)
+            return fail("read at :index %d: malformed payload", h->index[e]);
+        XRead r{inv, pos, h->index[e], {}};
+        for (int32_t j = 0; j < len; j += 3) {
+            const int32_t* t = h->payload + off + j;
+            r.kv.push_back({t[0], (int64_t)(((uint64_t)(uint32_t)t[2] << 32) | (uint32_t)t[1])});
+        }
+        std::sort(r.kv.begin(), r.kv.end());
+        for (size_t j = 1; j < r.kv.size(); ++j)
+            if (r.kv[j].first == r.kv[j - 1].first)
+                return fail("read at :index %d observes key %lld twice", h->index[e], r.kv[j].first);
+        S.R.push_back(std::move(r));
+    }
+    return 0;
+}
+
+// M(t) = min(:ok completion, earliest completion of an :ok lookup returning t); A(t) = latest invocation of an :ok
+// lookup (with an invocation) lacking t
+void classify_inputs(Shard& S) {
+    for (auto& t : S.T) {
+        t.M = t.okcomp;
+        for (auto& l : S.L) {
+            if (l.ids.count(t.id)) t.M = std::min(t.M, l.comp);
+            else if (l.inv >= 0) t.A = std::max(t.A, l.inv);
+        }
+    }
+}
+
+struct Cand {
+    int64_t id;
+    int32_t a, jd, jc;   // jd / jc: column of the debit / credit key, -1 unobserved
+    int32_t t;           // the transfer
+};
+
+// One gap's subset-sum problem: candidates and Delta per column.
+struct Problem {
+    std::vector<Cand> P;
+    std::vector<int64_t> d;
+    std::vector<int32_t> key;
+};
+
+// ---- RG_BRUTE ----------------------------------------------------------------------------------------------------
+// the solutions of P with sum d on every key (only >= 0: on that key alone); first: stop at the first one.  Returns
+// whether one exists; all = the AND of the solutions' masks
+[[maybe_unused]] bool brute(const Problem& pb, int32_t only, bool first, uint64_t& all) {
+    const size_t n = pb.P.size(), K = pb.d.size();
+    if (n > 24) { g_err = "RG_BRUTE: more than 24 candidates"; throw 1; }
+    std::vector<int64_t> s(K);
+    bool any = false;
+    all = ~0ull;
+    for (uint64_t x = 0; x < (1ull << n); ++x) {
+        std::fill(s.begin(), s.end(), 0);
+        for (size_t c = 0; c < n; ++c)
+            if (x >> c & 1) {
+                if (pb.P[c].jd >= 0) s[pb.P[c].jd] += pb.P[c].a;
+                if (pb.P[c].jc >= 0) s[pb.P[c].jc] += pb.P[c].a;
+            }
+        bool ok = true;
+        for (size_t k = 0; k < K && ok; ++k)
+            if (only < 0 || (int32_t)k == only) ok = s[k] == pb.d[k];
+        if (!ok) continue;
+        any = true;
+        all &= x;
+        if (first) return true;
+    }
+    return any;
+}
+
+// ---- RG_SEARCH (K10's search) ------------------------------------------------------------------------------------
+enum { UND = 0, IN = 1, OUT = 2 };
+enum Verdict { EXPLAINED, UNEXPLAINED, UNDECIDED };
+
+struct Search {
+    const Problem& pb;
+    int32_t only;
+    int64_t max_nodes, nodes = 0;
+    std::vector<int64_t> ins, av;
+
+    Search(const Problem& p, int32_t o, int64_t mx) : pb(p), only(o), max_nodes(mx), ins(p.d.size()), av(p.d.size()) {}
+
+    int32_t rel(int32_t j) const { return only < 0 || j == only ? j : -1; }
+
+    bool prune(const std::vector<int32_t>& ids, std::vector<uint8_t>& st, const std::vector<int64_t>& base,
+               int32_t& bad) {
+        const int32_t K = (int32_t)base.size();
+        for (;;) {
+            std::fill(ins.begin(), ins.end(), 0);
+            std::fill(av.begin(), av.end(), 0);
+            for (int32_t c : ids) {
+                if (st[c] == OUT) continue;
+                auto& v = st[c] == IN ? ins : av;
+                const int32_t kd = rel(pb.P[c].jd), kc = rel(pb.P[c].jc);
+                if (kd >= 0) v[kd] += pb.P[c].a;
+                if (kc >= 0) v[kc] += pb.P[c].a;
+            }
+            bad = -1;
+            for (int32_t k = 0; k < K && bad < 0; ++k) {
+                if (rel(k) < 0) continue;
+                const int64_t need = base[k] - ins[k];
+                if (need < 0 || need > av[k]) bad = k;
+            }
+            if (bad >= 0) return false;
+            std::vector<std::pair<int32_t, uint8_t>> upd;
+            for (int32_t c : ids) {
+                if (st[c] != UND) continue;
+                const int32_t ks[2] = {rel(pb.P[c].jd), rel(pb.P[c].jc)};
+                const int64_t a = pb.P[c].a;
+                bool drop = false, force = false;
+                for (int32_t k : ks)
+                    if (k >= 0 && a > base[k] - ins[k]) drop = true;
+                for (int32_t k : ks)
+                    if (!drop && k >= 0 && av[k] - a < base[k] - ins[k]) force = true;
+                if (drop) upd.push_back({c, OUT});
+                else if (force) upd.push_back({c, IN});
+            }
+            if (upd.empty()) return true;
+            for (auto& [c, v] : upd) st[c] = v;
+        }
+    }
+
+    bool dfs(const std::vector<int32_t>& F, std::vector<uint8_t>& st, const std::vector<int64_t>& base) {
+        int32_t b = -1;
+        for (int32_t c : F)
+            if (st[c] == UND) { b = c; break; }
+        for (uint8_t v : {(uint8_t)IN, (uint8_t)OUT}) {
+            if (++nodes > max_nodes) throw 2;
+            std::vector<uint8_t> s2 = st;
+            s2[b] = v;
+            int32_t bad;
+            if (!prune(F, s2, base, bad)) continue;
+            bool any = false;
+            for (int32_t c : F) any |= s2[c] == UND;
+            if (!any || dfs(F, s2, base)) return true;
+        }
+        return false;
+    }
+
+    // root_key: the smallest key the root pruning found unreachable, -1; kept: candidates the root did not drop;
+    // forced: the candidates a feasible root pruning forces in
+    // root_st: the candidates' states after the root pruning, feasible or not
+    Verdict run(int32_t& root_key, int32_t& kept, std::vector<int32_t>* forced = nullptr,
+                std::vector<uint8_t>* root_st = nullptr) {
+        const int32_t n = (int32_t)pb.P.size();
+        std::vector<uint8_t> st(n, UND);
+        std::vector<int32_t> all(n);
+        for (int32_t c = 0; c < n; ++c) {
+            all[c] = c;
+            if (rel(pb.P[c].jd) < 0 && rel(pb.P[c].jc) < 0) st[c] = OUT;
+        }
+        nodes = 1;
+        root_key = -1;
+        kept = 0;
+        int32_t bad;
+        const bool ok = prune(all, st, pb.d, bad);
+        for (int32_t c = 0; c < n; ++c) kept += st[c] != OUT;
+        if (root_st) *root_st = st;
+        if (!ok) { root_key = pb.key[bad]; return UNEXPLAINED; }
+        if (forced)
+            for (int32_t c = 0; c < n; ++c)
+                if (st[c] == IN) forced->push_back(c);
+        std::vector<int32_t> F;
+        for (int32_t c = 0; c < n; ++c)
+            if (st[c] == UND) F.push_back(c);
+        if (F.empty()) return EXPLAINED;
+        if (F.size() > (size_t)JTB_RG_MAX_FREE) return UNDECIDED;
+        std::sort(F.begin(), F.end(), [&](int32_t x, int32_t y) {
+            return pb.P[x].a != pb.P[y].a ? pb.P[x].a > pb.P[y].a : pb.P[x].id < pb.P[y].id;
+        });
+        std::vector<int64_t> base(pb.d.size());
+        for (size_t k = 0; k < base.size(); ++k) base[k] = pb.d[k] - ins[k];   // ins: the forced-in of the root
+        try {
+            return dfs(F, st, base) ? EXPLAINED : UNEXPLAINED;
+        } catch (int) {
+            return UNDECIDED;
+        }
+    }
+};
+
+struct GapOut {
+    int8_t code = G_EXPLAINED;
+    int32_t key = -1, n_eligible = 0;
+    int64_t delta = 0;
+    std::vector<int32_t> forced;   // transfers this gap forces in
+};
+
+int32_t col_of(const std::vector<int32_t>& keys, int64_t key) {
+    auto it = std::lower_bound(keys.begin(), keys.end(), key, [](int32_t a, int64_t b) { return a < b; });
+    return it != keys.end() && *it == key ? (int32_t)(it - keys.begin()) : -1;
+}
+
+// RG_SEARCH's sweep structures: the :ok transfers in invocation order (the order of S.T) with the running max of their
+// completions, and the crashed (:info, never completed) ones with a positive amount in invocation order, by anchor
+// column (the debit key's, else the credit key's; none when the shard observes neither)
+struct Index {
+    std::vector<int32_t> ok, ok_inv, ok_pmax;
+    std::vector<std::vector<int32_t>> crashed, crashed_inv;
+    Index(const Shard& S, const std::vector<int32_t>& keys) : crashed(keys.size()), crashed_inv(keys.size()) {
+        for (size_t i = 0; i < S.T.size(); ++i) {
+            const XTransfer& t = S.T[i];
+            if (t.fate == JTB_T_OK) {
+                ok.push_back((int32_t)i);
+                ok_inv.push_back(t.inv);
+                ok_pmax.push_back(std::max(ok_pmax.empty() ? INT_MIN : ok_pmax.back(), t.okcomp));
+            } else if (t.fate != JTB_T_FAIL && t.amount > 0) {
+                int32_t a = col_of(keys, 2 * (int64_t)t.debit);
+                if (a < 0) a = col_of(keys, 2 * (int64_t)t.credit + 1);
+                if (a < 0) continue;
+                crashed[a].push_back((int32_t)i);
+                crashed_inv[a].push_back(t.inv);
+            }
+        }
+    }
+};
+
+}  // namespace
