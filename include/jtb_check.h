@@ -600,7 +600,9 @@ int jtb_final_configs(jtb_ctx* ctx, const jtb_history* h, const jtb_model* m, in
 /* ---- hot path A4: (checker/set-full {:linearizable? L}) at set_full.clj:157 ------------------ */
 int jtb_check_set_full(jtb_ctx* ctx, const jtb_history* h, int linearizable, jtb_setfull_out* out);
 
-/* ---- hot path A8: bank SI checker, tests/ledger.clj:154-192 (after ledger->bank) -------------- */
+/* ---- hot path A8: bank SI checker, tests/ledger.clj:154-192 (after ledger->bank) -------------- *
+ * accounts->n_accounts must lie in [0, JTB_MAX_ACCOUNTS] (0: every key a read shows is :unexpected-key); <0 otherwise,
+ * with jtb_last_error saying why (the context stays usable). */
 int jtb_check_bank_totals(jtb_ctx* ctx, const jtb_history* h, const jtb_model* accounts,
                           int64_t total_amount, jtb_bank_result* out);
 
@@ -688,7 +690,10 @@ int jtb_get_stats(jtb_ctx* ctx, unsigned long long* out, int n);
  * int64; nemesis / un-keyed events can carry a key of their own).  Out: order[n_events] = original position of the
  * i-th event of the partitioned history (events of one key keep their history order), key_ids[n_keys] ascending,
  * shard_off[n_keys + 1] = the CSR offsets of jtb_history; key_cap = capacity of key_ids (shard_off: key_cap + 1).
- * jtb_ledger_balances is ledger->bank's arithmetic (tests/ledger.clj:100-105): balance = credits-posted - debits-posted. */
+ * Returns <0 with "key_cap too small" when the history has more than key_cap keys (order is written, shard_off and
+ * key_ids are not, *n_keys = 0; the context stays usable).
+ * jtb_ledger_balances is ledger->bank's arithmetic (tests/ledger.clj:100-105): balance = credits-posted - debits-posted,
+ * computed in int64 and truncated to its low 32 bits (two's complement) when the difference leaves int32. */
 int jtb_partition_by_key(jtb_ctx* ctx, int64_t n_events, const int64_t* event_key, int32_t* order, int64_t* shard_off,
                          int64_t* key_ids, int32_t key_cap, int32_t* n_keys);
 int jtb_ledger_balances(jtb_ctx* ctx, int64_t n, const int64_t* credits_posted, const int64_t* debits_posted,

@@ -166,14 +166,18 @@ constexpr int SF_RCHUNK = 512;   // reads per thread-chunk of the column scan
 // eligible read that shows a bit set / clear is that element's last_present / last_absent inside the chunk (chunks
 // merge by atomicMax); pass 2 walks them in completion order: the first eligible present read is known_read (atomicMin).
 // A word stops as soon as all of its 32 elements are settled.
-// grid: (word tiles of 128, read chunks, shards)
+// grid: (word tiles of 128, read chunks chunk0.., shards shard0..); grid.y and grid.z are capped at 65,535, so the host
+// launches one slice of at most that many chunks and shards at a time.
+constexpr int64_t SF_GRID_YZ_MAX = 65535;
 __global__ void __launch_bounds__(128) sf_column_scan(const SfRead* __restrict__ reads, const SfShard* __restrict__ shards,
                                                       const int32_t* __restrict__ order_desc,
-                                                      const uint32_t* __restrict__ bits, SfAcc* __restrict__ acc) {
-    const SfShard sd = shards[blockIdx.z];
+                                                      const uint32_t* __restrict__ bits, SfAcc* __restrict__ acc,
+                                                      int64_t chunk0, int64_t shard0) {
+    const SfShard sd = shards[shard0 + blockIdx.z];
     const int w = blockIdx.x * 128 + threadIdx.x;
-    const int r0 = blockIdx.y * SF_RCHUNK;
-    if (blockIdx.x * 128 >= sd.words_per_row || r0 >= sd.n_reads) return;
+    const int64_t r0_64 = (chunk0 + blockIdx.y) * SF_RCHUNK;
+    if (blockIdx.x * 128 >= sd.words_per_row || r0_64 >= sd.n_reads) return;
+    const int r0 = (int)r0_64;
     const int r1 = min(sd.n_reads, r0 + SF_RCHUNK);
     __shared__ int s_r[SF_RCHUNK], s_inv[SF_RCHUNK], s_elig[SF_RCHUNK];
     const bool live = w < sd.words_per_row;
@@ -455,18 +459,29 @@ inline int run_set_full(cudaStream_t st, cudaEvent_t e0, cudaEvent_t e1, SfBuffe
         JTB_OK(cudaGetLastError());
         ++launches;
     }
-    if (n_reads > 0 && n_elems > 0) {
+    if (n_reads > 0) {
+        // stage A runs even when no shard tracks an element: it is what flags the reads holding untracked ids, whose
+        // repeats count as :duplicated (sf_position finds nothing in an empty shard, so no bit is set)
         const int64_t threads = n_reads * 32;
         sf_build_bits<<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(d_reads, n_reads, d_shards, d_lut, d_sorted, d_payload, d_bits, d_flag);
         JTB_OK(cudaGetLastError());
-        int max_w = 0, max_r = 0;
-        for (auto& sd : shards) { max_w = std::max(max_w, sd.words_per_row); max_r = std::max(max_r, sd.n_reads); }
-        dim3 grid((max_w + 127) / 128, (max_r + SF_RCHUNK - 1) / SF_RCHUNK, n_shards);
-        sf_column_scan<<<grid, 128, 0, st>>>(d_reads, d_shards, d_order, d_bits, d_acc);
-        JTB_OK(cudaGetLastError());
-        sf_final_missing<<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(d_reads, n_reads, d_shards, d_bits, d_missing);
-        JTB_OK(cudaGetLastError());
-        launches += 3;
+        ++launches;
+        if (n_elems > 0) {
+            int max_w = 0, max_r = 0;
+            for (auto& sd : shards) { max_w = std::max(max_w, sd.words_per_row); max_r = std::max(max_r, sd.n_reads); }
+            const int64_t n_chunks = (max_r + SF_RCHUNK - 1) / SF_RCHUNK;
+            for (int64_t s0 = 0; s0 < n_shards; s0 += SF_GRID_YZ_MAX)
+                for (int64_t c0 = 0; c0 < n_chunks; c0 += SF_GRID_YZ_MAX) {
+                    dim3 grid((max_w + 127) / 128, (unsigned)std::min(SF_GRID_YZ_MAX, n_chunks - c0),
+                              (unsigned)std::min(SF_GRID_YZ_MAX, n_shards - s0));
+                    sf_column_scan<<<grid, 128, 0, st>>>(d_reads, d_shards, d_order, d_bits, d_acc, c0, s0);
+                    JTB_OK(cudaGetLastError());
+                    ++launches;
+                }
+            sf_final_missing<<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(d_reads, n_reads, d_shards, d_bits, d_missing);
+            JTB_OK(cudaGetLastError());
+            ++launches;
+        }
         // duplicates (rare): exact multiplicities for flagged reads
         JTB_OK(cudaMemcpyAsync(flag.data(), d_flag, n_reads * 4, cudaMemcpyDeviceToHost, st));
         JTB_OK(cudaStreamSynchronize(st));
@@ -666,6 +681,8 @@ __global__ void bk_scan(const BkRead* __restrict__ reads, int64_t n_reads, const
 inline int run_bank_totals(cudaStream_t st, cudaEvent_t e0, cudaEvent_t e1, const jtb_history* h, const jtb_model* m,
                            int64_t total_amount, jtb_bank_result* out, std::string& err) {
     const double t_start = std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count();
+    // zero accounts is legal (every key of every read is then unexpected); more than the model holds is not
+    if (m->n_accounts < 0 || m->n_accounts > JTB_MAX_ACCOUNTS) { err = "bank model needs 0..8 accounts"; return -2; }
     std::vector<BkRead> reads;
     for (int64_t e = 0; e < h->n_events; ++e) {
         if (h->process[e] < 0 || h->type[e] != JTB_T_OK || h->f[e] != JTB_F_READ) continue;
@@ -685,7 +702,7 @@ inline int run_bank_totals(cudaStream_t st, cudaEvent_t e0, cudaEvent_t e1, cons
     init.lowest_idx = init.highest_idx = init.first_error_idx = 0x7fffffff;
     JTB_OK(cudaMemcpyAsync(d_agg, &init, sizeof init, cudaMemcpyHostToDevice, st));
     int ids[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    for (int i = 0; i < m->n_accounts && i < 8; ++i) ids[i] = m->account_ids[i];
+    for (int i = 0; i < m->n_accounts; ++i) ids[i] = m->account_ids[i];
     const int4 lo = make_int4(ids[0], ids[1], ids[2], ids[3]), hi = make_int4(ids[4], ids[5], ids[6], ids[7]);
     JTB_OK(cudaEventRecord(e0, st));
     if (n > 0) {
