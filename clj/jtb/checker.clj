@@ -538,6 +538,31 @@
                                                                :other-op (by-index (at (+ s 20))))))
           (and (= 2 (at s)) (<= 0 (at (+ s 14)))) (assoc :lower-op (by-index (at (+ s 14)))))))))
 
+(def ^:private sw-cause {4 :partial-read 5 :anomaly 6 :undecided 7 :no-witness 8 :real-time})
+
+(defn serial-witness-checker
+  "A proof that a ledger history is linearizable, on the GPU, or :unknown: the transfer-placement check, then one
+  explanation chosen per read gap (no transfer in two, {:max-rounds n} witness rounds) and the serial order they give
+  checked against real time.  :valid? true means the reads and transfers are linearizable for the per-account
+  counters, and so for the bank model with negative balances allowed (the :linear question); otherwise :unknown with a
+  :cause (:partial-read, :anomaly, :undecided, :no-witness, :real-time), never false.  Add it to the compose map at
+  tests/ledger.clj:363-367 as `:serial-witness (serial-witness-checker {})`.
+  Result: {:valid? :read-count :transfer-count :committed-count :committed-crashed-count :after-count :rounds
+  [:cause :op :transfer-id]}."
+  [opts]
+  (reify checker/Checker
+    (check [_ _test history _opts]
+      (let [{:keys [arrays by-index]} (flatten-history :ledger-lookups history)
+            res (Native/checkSerialWitness @ctx arrays (long (:max-nodes opts 0)) (int (:max-rounds opts 0)))
+            at  (fn [i] (aget res (int i)))
+            s   12]                                        ; shard 0: valid cause reads transfers committed ...
+        (cond-> {:valid? (verdict (at s)) :read-count (at (+ s 2)) :transfer-count (at (+ s 3))
+                 :committed-count (at (+ s 4)) :committed-crashed-count (at (+ s 5)) :after-count (at (+ s 6))
+                 :rounds (at (+ s 8))}
+          (pos? (at (+ s 1)))   (assoc :cause (sw-cause (at (+ s 1))))
+          (<= 0 (at (+ s 9)))   (assoc :op (by-index (at (+ s 9))))
+          (<= 0 (at (+ s 10)))  (assoc :transfer-id (at (+ s 10))))))))
+
 ;; ---- independent ----------------------------------------------------------------------------------------------
 (defn independent-checker
   "Like (independent/checker (checker/compose checkers)) for a map {name checker-kind} built from THIS namespace's

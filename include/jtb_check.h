@@ -24,7 +24,7 @@
 extern "C" {
 #endif
 
-#define JTB_ABI_VERSION 8
+#define JTB_ABI_VERSION 9
 
 /* ---- verdict lattice (jepsen.checker/merge-valid) ------------------------------------------- */
 #define JTB_VALID   0
@@ -152,6 +152,10 @@ typedef struct jtb_lin_shard {
 #define JTB_CAUSE_BUDGET        2 /* max_configs / time budget reached                                */
 #define JTB_CAUSE_TOO_WIDE      3 /* > 64 concurrently open completed ops, or key does not fit        */
 #define JTB_CAUSE_PARTIAL_READ  4 /* monotonic-key check: an :ok read does not observe every key of its shard */
+#define JTB_CAUSE_ANOMALY       5 /* serial-witness check: the transfer-placement check found KEY, JOINT, DOUBLE or LOST */
+#define JTB_CAUSE_UNDECIDED     6 /* serial-witness check: the transfer-placement check left a gap undecided          */
+#define JTB_CAUSE_NO_WITNESS    7 /* serial-witness check: a witness round did not explain a gap, or max_rounds ran out */
+#define JTB_CAUSE_REAL_TIME     8 /* serial-witness check: the serial order of the chosen gaps breaks real time       */
 
 typedef struct jtb_lin_result {
     int32_t  valid;             /* merge-valid over shards                                            */
@@ -553,6 +557,57 @@ typedef struct jtb_tp_result {
     double  seconds_total;      /* host wall time of the call incl. the host pass, H2D, D2H                           */
 } jtb_tp_result;
 
+/* ---- serial-witness check (DESIGN.md "K13 serial-witness check") ---------------------------------------------------
+ * Proves a shard linearizable (VALID) or says nothing (UNKNOWN), never INVALID.  It runs the transfer-placement check
+ * unchanged (same max_nodes, max_rounds); only a shard that check calls VALID gets a witness, otherwise it is UNKNOWN
+ * with cause PARTIAL_READ, ANOMALY (KEY, JOINT, DOUBLE or LOST) or UNDECIDED.  Then:
+ *   - witness rounds (Jacobi): every gap g whose Delta' (Delta minus the transfers g owns) is not zero gathers as a
+ *     transfer-placement round >= 1 does (in-window, unowned, amount <= Delta') and runs the read-explanation search;
+ *     its first solution is g's choice.  After a round, g is fixed when no smaller gap that ran in the round chose one
+ *     of g's transfers; a fixed gap owns its choice, and the others run again without the owned transfers.  A gap the
+ *     search does not explain, or max_rounds rounds with a gap left unfixed, is cause NO_WITNESS.  D_g = the transfers
+ *     g owns;
+ *   - real time, one greedy pass over the reads r_1 ... r_n in the gap order, with event positions and cp = infinity
+ *     for an op that never completed :ok: P_0 = -inf, P_j = max(P_{j-1}, iv(r_j), iv(t) for t in D_{j-1}); every read
+ *     needs P_j < cp(r_j), every t in D_g (g >= 1) P_g < cp(t), and every :ok transfer with a window in no D_g commits
+ *     after the last read and needs P_n < cp(t); otherwise cause REAL_TIME;
+ *   - the counters of every gap are summed again from D_g; a mismatch is an internal error (rc < 0).
+ * A VALID shard's reads and transfers are then linearizable for the per-account counters (place r_j at P_j, t in D_g
+ * at max(P_g, iv(t))), and so for the bank model of ledger->bank with negative balances allowed.  Lookups are not
+ * placed; `:negative-balances? false` is not decided. */
+#define JTB_SW_NEVER  (-1)   /* commit_read: the transfer commits in no read's state and need not commit at all    */
+#define JTB_SW_AFTER  (-2)   /* an :ok transfer that commits after every read of its shard                         */
+#define JTB_SW_FREE   (-3)   /* an :ok transfer no read observes (or of amount 0): it commits inside its interval  */
+
+typedef struct jtb_sw_shard {
+    int32_t valid;              /* JTB_VALID / JTB_UNKNOWN                                                            */
+    int32_t cause;              /* JTB_CAUSE_* when valid == JTB_UNKNOWN                                              */
+    int32_t n_reads;            /* :ok reads of the shard                                                             */
+    int32_t n_transfers;        /* transfer micro-ops of the shard (every fate)                                       */
+    int64_t n_committed;        /* VALID: transfers committed in some gap                                             */
+    int64_t n_committed_crashed;/* VALID: of them, the crashed ones (:info, or never completed)                       */
+    int64_t n_after;            /* VALID: :ok transfers committed after the last read                                 */
+    int64_t nodes;              /* search nodes of the witness rounds                                                 */
+    int32_t rounds;             /* witness rounds that ran a gap of the shard                                         */
+    int32_t fail_index;         /* NO_WITNESS: completion :index of the failing gap's upper read; REAL_TIME: of the read
+                                   or the transfer that failed; -1                                                    */
+    int64_t transfer_id;        /* REAL_TIME on a transfer: its id; -1                                                */
+} jtb_sw_shard;
+
+typedef struct jtb_sw_result {
+    int32_t valid;              /* merge-valid over shards                                                            */
+    int32_t n_failures;         /* shards that are not VALID                                                          */
+    int64_t n_reads;
+    int64_t n_transfers;
+    int64_t n_committed;
+    int64_t n_committed_crashed;
+    int64_t n_after;
+    int64_t nodes;
+    int64_t rounds;             /* the most witness rounds of any shard                                               */
+    double  seconds_kernel;     /* device time (CUDA events)                                                          */
+    double  seconds_total;      /* host wall time of the call incl. the host pass, H2D, D2H                           */
+} jtb_sw_result;
+
 typedef struct jtb_ctx jtb_ctx;
 
 /* ---- lifecycle -------------------------------------------------------------------------------- */
@@ -561,7 +616,7 @@ int         jtb_abi_version(void);
  * 0 jtb_history, 1 jtb_model, 2 jtb_opts, 3 jtb_lin_shard, 4 jtb_lin_result, 5 jtb_setfull_shard,
  * 6 jtb_setfull_out, 7 jtb_bank_result, 8 jtb_final_config, 9 jtb_mono_shard, 10 jtb_mono_result, 11 jtb_cb_shard,
  * 12 jtb_cb_result, 13 jtb_tl_shard, 14 jtb_tl_result, 15 jtb_rx_shard, 16 jtb_rx_result, 17 jtb_rg_shard,
- * 18 jtb_rg_result, 19 jtb_tp_shard, 20 jtb_tp_result; -1 otherwise */
+ * 18 jtb_rg_result, 19 jtb_tp_shard, 20 jtb_tp_result, 21 jtb_sw_shard, 22 jtb_sw_result; -1 otherwise */
 long        jtb_struct_size(int which);
 int         jtb_device_count(void);                 /* number of CUDA devices, <0 on error          */
 jtb_ctx*    jtb_create(const jtb_opts* opts);       /* NULL on failure (no CUDA device etc.)        */
@@ -651,6 +706,16 @@ int jtb_check_read_gaps(jtb_ctx* ctx, const jtb_history* h, int64_t max_nodes, i
  * (jtb_last_error says which; the context stays usable). */
 int jtb_check_transfer_placement(jtb_ctx* ctx, const jtb_history* h, int64_t max_nodes, int32_t max_rounds,
                                  int32_t flags, jtb_tp_shard* shards, jtb_tp_result* out);
+
+/* ---- serial-witness check (see jtb_sw_shard above) ------------------------------------------------------------ *
+ * shards[n_shards] is caller-allocated; max_nodes and max_rounds as for jtb_check_transfer_placement (and passed to
+ * it); flags is reserved and must be 0.  commit_read may be NULL, else it receives one entry per transfer micro-op in
+ * history order: the completion :index of the first read whose state holds the transfer, JTB_SW_NEVER, JTB_SW_AFTER or
+ * JTB_SW_FREE (JTB_SW_NEVER for every transfer of a shard that is not VALID).  Returns 0 on success, <0 on the
+ * transfer-placement check's errors or when the counters of a witness do not add up (jtb_last_error says which; the
+ * context stays usable). */
+int jtb_check_serial_witness(jtb_ctx* ctx, const jtb_history* h, int64_t max_nodes, int32_t max_rounds, int32_t flags,
+                             int32_t* commit_read, jtb_sw_shard* shards, jtb_sw_result* out);
 
 /* ---- multi-GPU fan-out inside the library (SURVEY §8(b) `n_gpus`, §8(e)) ----------------------------------- *
  * What `independent/checker` (set_full.clj:155) does over JVM threads, done over the GPUs of one box for a host

@@ -139,4 +139,15 @@ public final class Native {
      *     witnessIndex, lowerIndex, kind, key, round, delta, transferId, otherIndex, nEligible}
      */
     public static native long[] checkTransferPlacement(long ctx, Object[] history, long maxNodes, int maxRounds);
+
+    /**
+     * {@code jtb_check_serial_witness}: a proof that a ledger history is linearizable (VALID), or UNKNOWN with a
+     * cause; never INVALID.  Input: the ledger-lookups form.  {@code maxNodes} and {@code maxRounds} as for
+     * {@link #checkTransferPlacement}, which it runs first.
+     *
+     * @return {@code [valid, nFailures, nReads, nTransfers, nCommitted, nCommittedCrashed, nAfter, nodes, rounds,
+     *     kernelNs, totalNs, nShards]} followed by 11 longs per shard: {@code valid, cause, nReads, nTransfers,
+     *     nCommitted, nCommittedCrashed, nAfter, nodes, rounds, failIndex, transferId}
+     */
+    public static native long[] checkSerialWitness(long ctx, Object[] history, long maxNodes, int maxRounds);
 }

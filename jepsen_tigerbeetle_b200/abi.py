@@ -5,7 +5,7 @@ import ctypes as C
 
 from .history import MAX_ACCOUNTS
 
-ABI_VERSION = 8
+ABI_VERSION = 9
 OPT_NO_EAGER_READS = 1
 OPT_NO_SCOUTS = 2
 OPT_ENGINE_LEVEL = 4
@@ -13,7 +13,9 @@ OPT_ENGINE_WORKLIST = 8
 OPT_NO_BEAM = 16
 
 CAUSE_NONE, CAUSE_TABLE_FULL, CAUSE_BUDGET, CAUSE_TOO_WIDE, CAUSE_PARTIAL_READ = 0, 1, 2, 3, 4
-CAUSE_NAME = {0: None, 1: "table-full", 2: "budget", 3: "too-wide", 4: "partial-read"}
+CAUSE_ANOMALY, CAUSE_UNDECIDED, CAUSE_NO_WITNESS, CAUSE_REAL_TIME = 5, 6, 7, 8
+CAUSE_NAME = {0: None, 1: "table-full", 2: "budget", 3: "too-wide", 4: "partial-read", 5: "anomaly", 6: "undecided",
+              7: "no-witness", 8: "real-time"}
 MONO_NO_REALTIME = 1
 MONO_EDGE_NONE, MONO_EDGE_MONOTONIC, MONO_EDGE_REALTIME = 0, 1, 2
 CB_BELOW, CB_ABOVE = 1, 2
@@ -32,6 +34,7 @@ TP_KEY, TP_JOINT, TP_DOUBLE, TP_LOST = 1, 2, 3, 4
 TP_KIND_NAME = {1: "key", 2: "joint", 3: "double", 4: "lost"}
 TP_MAX_KEYS, TP_MAX_GATHER, TP_MAX_FREE, TP_DEFAULT_MAX_NODES = RG_MAX_KEYS, RG_MAX_GATHER, RG_MAX_FREE, 4096
 TP_DEFAULT_MAX_ROUNDS = 64
+SW_NEVER, SW_AFTER, SW_FREE = -1, -2, -3
 SF_NEVER_READ, SF_STABLE, SF_LOST = 0, 1, 2
 BANK_OK, BANK_UNEXPECTED_KEY, BANK_NIL_BALANCE, BANK_WRONG_TOTAL, BANK_NEGATIVE_VALUE = range(5)
 BANK_ERR_NAME = {1: "unexpected-key", 2: "nil-balance", 3: "wrong-total", 4: "negative-value"}
@@ -323,3 +326,40 @@ def tp_to_dict(res, shards) -> dict:
         "shards": [{f: (list(s.count_by_kind) if f == "count_by_kind" else getattr(s, f)) for f in TP_SHARD_FIELDS}
                    for s in shards],
     }
+
+
+class CSwShard(C.Structure):
+    """jtb_sw_shard: the serial-witness verdict of one shard."""
+    _fields_ = [("valid", C.c_int32), ("cause", C.c_int32), ("n_reads", C.c_int32), ("n_transfers", C.c_int32),
+                ("n_committed", C.c_int64), ("n_committed_crashed", C.c_int64), ("n_after", C.c_int64),
+                ("nodes", C.c_int64), ("rounds", C.c_int32), ("fail_index", C.c_int32), ("transfer_id", C.c_int64)]
+
+
+class CSwResult(C.Structure):
+    _fields_ = [("valid", C.c_int32), ("n_failures", C.c_int32), ("n_reads", C.c_int64), ("n_transfers", C.c_int64),
+                ("n_committed", C.c_int64), ("n_committed_crashed", C.c_int64), ("n_after", C.c_int64),
+                ("nodes", C.c_int64), ("rounds", C.c_int64), ("seconds_kernel", C.c_double),
+                ("seconds_total", C.c_double)]
+
+
+SW_SHARD_FIELDS = ("valid", "cause", "n_reads", "n_transfers", "n_committed", "n_committed_crashed", "n_after", "nodes",
+                   "rounds", "fail_index", "transfer_id")
+SW_RESULT_FIELDS = ("valid", "n_failures", "n_reads", "n_transfers", "n_committed", "n_committed_crashed", "n_after",
+                    "nodes", "rounds", "seconds_kernel", "seconds_total")
+
+
+def sw_to_dict(res, shards, commit_read=None) -> dict:
+    """One result dict for the library and the oracle; "commit_read" (a numpy int32 array, one entry per transfer
+    micro-op in history order) when it was asked for."""
+    out = {f: getattr(res, f) for f in SW_RESULT_FIELDS}
+    out["shards"] = [{f: getattr(s, f) for f in SW_SHARD_FIELDS} for s in shards]
+    if commit_read is not None:
+        out["commit_read"] = commit_read
+    return out
+
+
+def n_transfer_records(h) -> int:
+    """Transfer micro-ops of a ledger-lookups history: the records of its transfer invokes."""
+    import numpy as np
+    inv = (h.type == 0) & (h.f == 4) & (h.process >= 0) & (h.payload_len > 0)
+    return int(np.sum(h.payload_len[inv] // 5))

@@ -583,6 +583,56 @@ class TransferPlacement(Checker, _Native):
         return out
 
 
+class SerialWitness(Checker, _Native):
+    """A proof that a ledger history is linearizable, on the GPU (K13), or nothing.
+
+    Reads the ledger-lookups form and runs the transfer-placement check (max-nodes, max-rounds).  For a shard it calls
+    valid, one explanation is chosen per read gap, no transfer in two (max-rounds witness rounds), and the serial order
+    they give (each read after the transfers of the gaps up to it) is checked against real time.  A shard that passes
+    is :valid? true: its reads and transfers are linearizable for the per-account counters, and so for the bank model
+    with negative balances allowed (the ledger test's :linear question); lookups are not placed.  Otherwise it is
+    :unknown with a cause ("partial-read", "anomaly", "undecided", "no-witness", "real-time"); never false, since the
+    anomalies are the other ledger checks' business.
+    Result: {valid?, read-count, transfer-count, committed-count, committed-crashed-count, after-count, rounds, [cause,
+    op, transfer-id]}."""
+
+    def __init__(self, checker_opts: Mapping[str, Any] | None = None, ctx: Context | None = None,
+                 **ctx_opts) -> None:
+        _Native.__init__(self, ctx, **ctx_opts)
+        self.max_nodes = int((checker_opts or {}).get("max-nodes", 0))
+        self.max_rounds = int((checker_opts or {}).get("max-rounds", 0))
+
+    def _shard_map(self, s: dict) -> dict:
+        m: dict[str, Any] = {"valid?": VERDICT_NAME[s["valid"]], "read-count": s["n_reads"],
+                             "transfer-count": s["n_transfers"], "committed-count": s["n_committed"],
+                             "committed-crashed-count": s["n_committed_crashed"], "after-count": s["n_after"],
+                             "rounds": s["rounds"]}
+        if s["cause"]:
+            m["cause"] = abi.CAUSE_NAME.get(s["cause"], "unknown")
+        if s["fail_index"] >= 0:
+            m["op"] = {"index": s["fail_index"]}
+        if s["transfer_id"] >= 0:
+            m["transfer-id"] = s["transfer_id"]
+        return m
+
+    def check_flat(self, test, h: FlatHistory) -> tuple[dict, list[dict]]:
+        r = self.ctx.check_serial_witness(h, self.max_nodes, self.max_rounds)
+        top = {"valid?": VERDICT_NAME[r["valid"]], "read-count": r["n_reads"], "transfer-count": r["n_transfers"],
+               "committed-count": r["n_committed"], "committed-crashed-count": r["n_committed_crashed"],
+               "after-count": r["n_after"], "rounds": r["rounds"], "nodes": r["nodes"],
+               "seconds-kernel": r["seconds_kernel"], "seconds-total": r["seconds_total"]}
+        return top, [self._shard_map(s) for s in r["shards"]]
+
+    def check(self, test, history, opts=None) -> dict:
+        h = _flat(history, "ledger-lookups")
+        if h.n_shards != 1:
+            raise ValueError("history has independent keys: wrap with independent_checker(...)")
+        top, per = self.check_flat(test, h)
+        out = dict(per[0])
+        out.update({k: v for k, v in top.items() if k.startswith("seconds-") or k == "nodes"})
+        return out
+
+
 class Compose(Checker):
     """`(checker/compose {name checker ...})`: run each, `:valid?` = merge-valid of the results."""
 
@@ -615,13 +665,13 @@ class Independent(Checker):
             return c.model
         if isinstance(c, (MonotonicKeys, CounterBounds)):
             return "ledger-counters"
-        if isinstance(c, (TransferLookups, ReadExplanations, ReadGaps, TransferPlacement)):
+        if isinstance(c, (TransferLookups, ReadExplanations, ReadGaps, TransferPlacement, SerialWitness)):
             return "ledger-lookups"
         return "set"
 
     def _per_key(self, checker: Checker, test, h: FlatHistory, opts) -> list[dict]:
         if isinstance(checker, (Linearizable, SetFull, ReadAllInvokedAdds, MonotonicKeys, CounterBounds,
-                                TransferLookups, ReadExplanations, ReadGaps, TransferPlacement)):
+                                TransferLookups, ReadExplanations, ReadGaps, TransferPlacement, SerialWitness)):
             try:
                 return checker.check_flat(test, h)[1]
             except Exception:  # noqa: BLE001
@@ -702,6 +752,12 @@ def transfer_placement_checker(opts: Mapping[str, Any] | None = None, **kw) -> T
     """The read-gap check with located transfers carried across gaps to a fixpoint (K12); {"max-nodes": n} sets the
     per-gap search budget and {"max-rounds": n} the number of rounds."""
     return TransferPlacement(opts, **kw)
+
+
+def serial_witness_checker(opts: Mapping[str, Any] | None = None, **kw) -> SerialWitness:
+    """A proof of linearizability for ledger histories, or :unknown (K13); {"max-nodes": n} and {"max-rounds": n} as
+    for the transfer-placement check it runs first."""
+    return SerialWitness(opts, **kw)
 
 
 def compose(checkers: Mapping[str, Checker]) -> Compose:
@@ -872,15 +928,16 @@ def final_reads() -> FinalReads:
 def ledger_checker(checker_opts: Mapping[str, Any] | None = None, ctx: Context | None = None,
                    linear: bool = True, monotonic: bool = False, counter_bounds: bool = False,
                    transfer_lookups: bool = False, read_explanations: bool = False,
-                   read_gaps: bool = False, transfer_placement: bool = False) -> Compose:
+                   read_gaps: bool = False, transfer_placement: bool = False,
+                   serial_witness: bool = False) -> Compose:
     """The ledger test's checker (tests/ledger.clj:363-367) minus the gnuplot plotter, plus the
     linearizability search the north-star adds and, with monotonic=True, the monotonic-key check, with
     counter_bounds=True, the counter-bounds check, with transfer_lookups=True, the transfer-lookup check, with
-    read_explanations=True, the read-explanation check, with read_gaps=True, the read-gap check and, with
-    transfer_placement=True, the transfer-placement check:
+    read_explanations=True, the read-explanation check, with read_gaps=True, the read-gap check, with
+    transfer_placement=True, the transfer-placement check and, with serial_witness=True, the serial-witness check:
         {:SI (checker opts) :lookup-transfers ... :final-reads ... :unexpected-ops ... [:linear ...] [:monotonic ...]
          [:counter-bounds ...] [:transfer-lookups ...] [:read-explanations ...] [:read-gaps ...]
-         [:transfer-placement ...]}"""
+         [:transfer-placement ...] [:serial-witness ...]}"""
     cs: dict[str, Checker] = {"SI": bank_checker(checker_opts, ctx=ctx),
                               "lookup-transfers": lookup_all_invoked_transfers(),
                               "final-reads": final_reads(), "unexpected-ops": unexpected_ops()}
@@ -898,4 +955,6 @@ def ledger_checker(checker_opts: Mapping[str, Any] | None = None, ctx: Context |
         cs["read-gaps"] = read_gap_checker(ctx=ctx)
     if transfer_placement:
         cs["transfer-placement"] = transfer_placement_checker(ctx=ctx)
+    if serial_witness:
+        cs["serial-witness"] = serial_witness_checker(ctx=ctx)
     return compose(cs)

@@ -23,6 +23,7 @@
 #include "jtb_read_explanations.cuh"
 #include "jtb_read_gaps.cuh"
 #include "jtb_transfer_placement.cuh"
+#include "jtb_serial_witness.cuh"
 
 using namespace jtb;
 
@@ -738,6 +739,8 @@ long jtb_struct_size(int which) {
     case 18: return sizeof(jtb_rg_result);
     case 19: return sizeof(jtb_tp_shard);
     case 20: return sizeof(jtb_tp_result);
+    case 21: return sizeof(jtb_sw_shard);
+    case 22: return sizeof(jtb_sw_result);
     }
     return -1;
 }
@@ -1168,6 +1171,17 @@ int jtb_check_transfer_placement(jtb_ctx* ctx, const jtb_history* h, int64_t max
     ctx->fc.valid = false;
     return run_transfer_placement(ctx->stream, ctx->ev0, ctx->ev1, h, max_nodes, max_rounds, flags, shards, out,
                                   ctx->err);
+}
+
+// K13: the serial-witness check (csrc/jtb_serial_witness.cuh)
+int jtb_check_serial_witness(jtb_ctx* ctx, const jtb_history* h, int64_t max_nodes, int32_t max_rounds, int32_t flags,
+                             int32_t* commit_read, jtb_sw_shard* shards, jtb_sw_result* out) {
+    if (!ctx) return -1;
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    if (cudaSetDevice(ctx->device) != cudaSuccess) { ctx->err = "cudaSetDevice failed"; return -1; }
+    ctx->fc.valid = false;
+    return run_serial_witness(ctx->stream, ctx->ev0, ctx->ev1, h, max_nodes, max_rounds, flags, commit_read, shards,
+                              out, ctx->err);
 }
 
 // SURVEY 8(f) N2: the step before the checkers (independent/subhistory, ledger->bank) on the device

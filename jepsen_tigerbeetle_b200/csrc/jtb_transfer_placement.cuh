@@ -14,6 +14,8 @@
 //     like V) and the difference array of the dirtied windows, summed by cub before the next round; the host reads one
 //     changed-flag word per round;
 //   - tp_gap_final, tp_transfer_final and tp_witness_id: the counts, the verdict and the witness.
+// The host side is two stages: tp_stage (the host passes, the first kernels, the windows and the rounds) and tp_finals;
+// the serial-witness check (jtb_serial_witness.cuh) runs both and then its own kernels on the stage's device state.
 // The decision, the caps, the node counts and the rounds equal the TP_SEARCH CPU test oracle's, gap for gap.
 #pragma once
 #include <algorithm>
@@ -321,46 +323,52 @@ __global__ void tp_witness_id(RgDev d, TpDev p) {
 
 // ---- host ---------------------------------------------------------------------------------------------------------
 
-inline int run_transfer_placement(cudaStream_t st, cudaEvent_t ev0, cudaEvent_t ev1, const jtb_history* h,
-                                  int64_t max_nodes, int32_t max_rounds, int32_t flags, jtb_tp_shard* shards,
-                                  jtb_tp_result* out, std::string& err) {
-    const auto t0 = std::chrono::steady_clock::now();
-    if (!h || !shards || !out) { err = "null argument"; return -2; }
+// What K12's stage leaves for the finals of the call that ran it: K7's, K9's and K11's host passes and device reads,
+// and the device state at the end of the rounds.
+struct TpStage {
+    MonoHost H;
+    TlHost T;
+    int32_t S = 0, nT = 0, nL = 0, m = 0;
+    int64_t nR = 0, slots = 0, cells = 0;
+    std::vector<char> dev;                // per shard: it has reads and none is partial (its gaps run on the device)
+    std::vector<int32_t> d_of, shard_v, inv_v, comp_v, rs_off;
+    CallAllocs A;
+    TlDev d;
+    RgDev x;
+    TpDev p;
+    int64_t* own = nullptr;
+    int32_t* tM = nullptr;
+    unsigned long long *cnt = nullptr, *wkey = nullptr, *wtid = nullptr;
+    uint8_t* tmp = nullptr;               // cub's temporary storage
+    size_t tmp_bytes = 0;
+};
+
+// K12 up to its finals: the input checks, the host passes, K7's, K9's and K10's first kernels, the windows and the
+// rounds.  With device reads (g.m > 0), ev0 is recorded before the first kernel.
+inline int tp_stage(cudaStream_t st, cudaEvent_t ev0, const jtb_history* h, int64_t max_nodes, int32_t max_rounds,
+                    int32_t flags, TpStage& g, std::string& err) {
     if (flags != 0) { err = "flags must be 0 (reserved)"; return -2; }
     if (int rc = check_history(h, false, err)) return rc;
     if (max_nodes <= 0) max_nodes = JTB_TP_DEFAULT_MAX_NODES;
     if (max_rounds <= 0) max_rounds = JTB_TP_DEFAULT_MAX_ROUNDS;
-    const int32_t S = h->n_shards;
-    MonoHost H;
+    const int32_t S = g.S = h->n_shards;
+    MonoHost& H = g.H;
     if (int rc = mono_host_pass(h, H, err)) return rc;
-    TlHost T;
+    TlHost& T = g.T;
     if (int rc = tl_host_pass(h, T, err)) return rc;
     if (T.t_id.size() > (size_t)1 << 30) { err = "more than 2^30 transfers"; return -2; }
-    const int32_t nT = (int32_t)T.t_id.size(), nL = (int32_t)T.l_shard.size();
-    const int64_t nR = T.rec_base.back(), slots = (int64_t)H.keys.size();
-    memset(out, 0, sizeof *out);
-    std::vector<char> dev(S, 0);
-    for (int32_t s = 0; s < S; ++s) {
-        jtb_tp_shard& o = shards[s];
-        memset(&o, 0, sizeof o);
-        o.valid = JTB_VALID;
-        o.n_reads = H.n_reads[s];
-        o.n_transfers = T.t_off[s + 1] - T.t_off[s];
-        o.witness_index = o.lower_index = o.key = o.other_index = o.round = -1;
-        if (H.n_reads[s] > 0 && H.min_trip[s] < H.n_keys[s]) {
-            o.valid = JTB_UNKNOWN;
-            o.cause = JTB_CAUSE_PARTIAL_READ;
-        } else if (H.n_reads[s] > 0) dev[s] = 1;
-        out->n_reads += o.n_reads;
-        out->n_transfers += o.n_transfers;
-    }
+    const int32_t nT = g.nT = (int32_t)T.t_id.size(), nL = g.nL = (int32_t)T.l_shard.size();
+    const int64_t nR = g.nR = T.rec_base.back(), slots = g.slots = (int64_t)H.keys.size();
+    g.dev.assign(S, 0);
+    for (int32_t s = 0; s < S; ++s) g.dev[s] = H.n_reads[s] > 0 && H.min_trip[s] >= H.n_keys[s];
     // K11's device reads and sweep structures
-    std::vector<int32_t> d_of, shard_v, inv_v, comp_v, rs_off(S + 1, 0);
+    std::vector<int32_t>&d_of = g.d_of, &shard_v = g.shard_v, &inv_v = g.inv_v, &comp_v = g.comp_v, &rs_off = g.rs_off;
+    rs_off.assign(S + 1, 0);
     std::vector<int64_t> poff_v, row_v;
-    int64_t cells = 0;
+    int64_t& cells = g.cells;
     for (int32_t r = 0; r < (int32_t)H.r_shard.size(); ++r) {
         const int32_t s = H.r_shard[r];
-        if (!dev[s]) continue;
+        if (!g.dev[s]) continue;
         d_of.push_back(r);
         shard_v.push_back(s);
         inv_v.push_back(H.r_inv[r]);
@@ -371,7 +379,8 @@ inline int run_transfer_placement(cudaStream_t st, cudaEvent_t ev0, cudaEvent_t 
         rs_off[s + 1]++;
     }
     for (int32_t s = 0; s < S; ++s) rs_off[s + 1] += rs_off[s];
-    const int32_t m = (int32_t)d_of.size();
+    const int32_t m = g.m = (int32_t)d_of.size();
+    if (m == 0) return 0;
     // the device reads of every shard by invocation (stable over completion order)
     std::vector<int32_t> ivperm(m), ivs(m);
     for (int32_t r = 0; r < m; ++r) ivperm[r] = r;
@@ -410,224 +419,264 @@ inline int run_transfer_placement(cudaStream_t st, cudaEvent_t ev0, cudaEvent_t 
             cr_t[j] = t;
             cr_inv[j] = T.t_inv[t];
         }
-    float ms = 0;
-    if (m > 0) {
-        CallAllocs A;
-        int64_t *V, *own;
-        if (A.alloc(&V, (size_t)cells) != cudaSuccess || A.alloc(&own, (size_t)cells) != cudaSuccess) {
-            err = "cannot allocate the dense value matrices (2 x " + std::to_string((size_t)cells * sizeof(int64_t)) +
-                  " bytes on the device)";
-            return -3;
-        }
-        TlDev d;
-        RgDev x;
-        TpDev p;
-        d.n_t = nT;
-        d.n_l = nL;
-        d.n_rec = nR;
-        x.m = m;
-        x.V = V;
-        x.max_nodes = max_nodes;
-        p.n_t = nT;
-        p.own = own;
-        const int64_t* tid;
-        const int64_t* poff;
-        TlTKey *tk0, *tk;
-        TlRKey *rk0, *rk;
-        MonoKey *key0, *key1;
-        int32_t *tid0, *tperm, *rv0, *rv, *tM, *tA, *id0, *id1, *pos, *cmax, *srev, *rev, *dirty;
-        const int32_t *d_ivperm, *d_ivs;
-        uint64_t* mk;
-        unsigned long long *cnt, *wkey, *wtid;
-        uint8_t* tmp;
-        JTB_OK(A.put(&d.payload, h->payload, (size_t)h->n_payload, st));
-        JTB_OK(A.put(&poff, poff_v, st)); JTB_OK(A.put(&x.row, row_v, st)); JTB_OK(A.put(&x.shard, shard_v, st));
-        JTB_OK(A.put(&x.inv, inv_v, st)); JTB_OK(A.put(&x.comp, comp_v, st));
-        JTB_OK(A.put(&d.n_keys, H.n_keys, st)); JTB_OK(A.put(&d.key_off, H.key_off, st)); JTB_OK(A.put(&d.keys, H.keys, st));
-        x.n_keys = d.n_keys; x.key_off = d.key_off; x.keys = d.keys;
-        JTB_OK(A.put(&d.t_shard, T.t_shard, st)); JTB_OK(A.put(&tid, T.t_id, st)); JTB_OK(A.put(&d.t_rec, T.t_rec, st));
-        JTB_OK(A.put(&d.t_inv, T.t_inv, st)); JTB_OK(A.put(&d.t_okcomp, T.t_okcomp, st));
-        JTB_OK(A.put(&d.t_fate, T.t_fate, st)); JTB_OK(A.put(&d.t_off, T.t_off, st));
-        x.t_rec = d.t_rec; x.t_id = tid;
-        JTB_OK(A.put(&d.l_shard, T.l_shard, st)); JTB_OK(A.put(&d.l_comp, T.l_comp, st));
-        JTB_OK(A.put(&d.l_poff, T.l_poff, st)); JTB_OK(A.put(&d.rec_base, T.rec_base, st));
-        JTB_OK(A.put(&d.ib, T.ib, st)); JTB_OK(A.put(&d.ib_inv, T.ib_inv, st)); JTB_OK(A.put(&d.ib_off, T.ib_off, st));
-        JTB_OK(A.put(&x.ok_t, ok_t, st)); JTB_OK(A.put(&x.ok_inv, ok_inv, st)); JTB_OK(A.put(&x.ok_pmax, ok_pmax, st));
-        JTB_OK(A.put(&x.ok_off, ok_off, st)); JTB_OK(A.put(&x.cr_t, cr_t, st)); JTB_OK(A.put(&x.cr_inv, cr_inv, st));
-        JTB_OK(A.put(&x.cr_off, cr_off, st));
-        JTB_OK(A.put(&p.rs_off, rs_off, st)); JTB_OK(A.put(&d_ivperm, ivperm, st)); JTB_OK(A.put(&d_ivs, ivs, st));
-        JTB_OK(A.alloc(&key0, m)); JTB_OK(A.alloc(&key1, m)); JTB_OK(A.alloc(&id0, m)); JTB_OK(A.alloc(&id1, m));
-        JTB_OK(A.alloc(&tk0, nT)); JTB_OK(A.alloc(&tk, nT)); JTB_OK(A.alloc(&tid0, nT)); JTB_OK(A.alloc(&tperm, nT));
-        JTB_OK(A.alloc(&d.rec_slot, nR)); JTB_OK(A.alloc(&rk0, nR)); JTB_OK(A.alloc(&rk, nR));
-        JTB_OK(A.alloc(&rv0, nR)); JTB_OK(A.alloc(&rv, nR));
-        JTB_OK(A.alloc(&d.mlk, nT)); JTB_OK(A.alloc(&d.mv, nT)); JTB_OK(A.alloc(&d.mfrom, nT)); JTB_OK(A.alloc(&mk, nT));
-        JTB_OK(A.alloc(&d.wid, (size_t)nL * 5)); JTB_OK(A.alloc(&d.count, (size_t)S * JTB_TL_KINDS));
-        JTB_OK(A.alloc(&tM, nT)); JTB_OK(A.alloc(&tA, nT)); JTB_OK(A.alloc(&x.f1, nT)); JTB_OK(A.alloc(&x.f2, nT));
-        JTB_OK(A.alloc(&x.code, m)); JTB_OK(A.alloc(&x.gkey, m)); JTB_OK(A.alloc(&x.gkept, m));
-        JTB_OK(A.alloc(&x.gdelta, m));
-        JTB_OK(A.alloc(&cnt, (size_t)S * TP_COUNTERS)); JTB_OK(A.alloc(&wkey, S)); JTB_OK(A.alloc(&wtid, S));
-        JTB_OK(A.alloc(&pos, m)); JTB_OK(A.alloc(&cmax, m)); JTB_OK(A.alloc(&rev, m)); JTB_OK(A.alloc(&srev, m));
-        JTB_OK(A.alloc(&p.lo, nT)); JTB_OK(A.alloc(&p.hi, nT)); JTB_OK(A.alloc(&p.jd, nT)); JTB_OK(A.alloc(&p.jc, nT));
-        JTB_OK(A.alloc(&p.flag, nT)); JTB_OK(A.alloc(&p.owner, nT)); JTB_OK(A.alloc(&p.pmin, nT));
-        JTB_OK(A.alloc(&p.pmax, nT)); JTB_OK(A.alloc(&p.dround, nT)); JTB_OK(A.alloc(&p.dg1, nT));
-        JTB_OK(A.alloc(&p.dg2, nT)); JTB_OK(A.alloc(&p.lround, nT));
-        JTB_OK(A.alloc(&p.lcode, m)); JTB_OK(A.alloc(&p.lround_g, m)); JTB_OK(A.alloc(&p.inc, m));
-        JTB_OK(A.alloc(&dirty, (size_t)m + 1)); JTB_OK(A.alloc(&p.pn, m)); JTB_OK(A.alloc(&p.dd, (size_t)m + 1));
-        JTB_OK(A.alloc(&p.poss, (size_t)m * JTB_TP_MAX_GATHER)); JTB_OK(A.alloc(&p.changed, 1));
-        JTB_OK(A.alloc(&p.srounds, S));
-        int32_t* incsum;
-        JTB_OK(A.alloc(&incsum, m));
-        d.tkey = tk; d.tperm = tperm; d.rkey = rk; d.rval = rv;
-        x.ord = id1; x.t_M = tM; x.t_A = tA; x.cnt = cnt; x.wkey = wkey; x.wtid = wtid;
-        p.pos = pos; p.t_shard = d.t_shard; p.t_fate = d.t_fate; p.t_inv = d.t_inv; p.dirty = dirty;
-        p.incsum = incsum;
-        size_t tmp_m = 0, tmp_t = 0, tmp_r = 0, tmp_s = 0, tmp_s2 = 0, tmp_s3 = 0;
-        JTB_OK(cub::DeviceRadixSort::SortPairs(nullptr, tmp_m, key0, key1, id0, id1, m, MonoKeyDecomposer{}, st));
-        if (nT > 0)
-            JTB_OK(cub::DeviceRadixSort::SortPairs(nullptr, tmp_t, tk0, tk, tid0, tperm, nT, TlTKeyDecomposer{}, st));
-        if (nR > 0)
-            JTB_OK(cub::DeviceRadixSort::SortPairs(nullptr, tmp_r, rk0, rk, rv0, rv, (int)nR, TlRKeyDecomposer{}, st));
-        JTB_OK(cub::DeviceScan::InclusiveScan(nullptr, tmp_s, pos, cmax, MaxOp{}, m, st));
-        JTB_OK(cub::DeviceScan::InclusiveScan(nullptr, tmp_s2, rev, srev, MinOp{}, m, st));
-        JTB_OK(cub::DeviceScan::InclusiveSum(nullptr, tmp_s3, p.dd, dirty, m + 1, st));
-        const size_t tmp_bytes = std::max({tmp_m, tmp_t, tmp_r, tmp_s, tmp_s2, tmp_s3});
-        JTB_OK(A.alloc(&tmp, tmp_bytes));
-        auto grid = [](int64_t n, int per) { return (unsigned)((n + per - 1) / per); };
+    CallAllocs& A = g.A;
+    int64_t *V, *own;
+    if (A.alloc(&V, (size_t)cells) != cudaSuccess || A.alloc(&own, (size_t)cells) != cudaSuccess) {
+        err = "cannot allocate the dense value matrices (2 x " + std::to_string((size_t)cells * sizeof(int64_t)) +
+              " bytes on the device)";
+        return -3;
+    }
+    TlDev& d = g.d;
+    RgDev& x = g.x;
+    TpDev& p = g.p;
+    d.n_t = nT;
+    d.n_l = nL;
+    d.n_rec = nR;
+    x.m = m;
+    x.V = V;
+    x.max_nodes = max_nodes;
+    p.n_t = nT;
+    p.own = g.own = own;
+    const int64_t* tid;
+    const int64_t* poff;
+    TlTKey *tk0, *tk;
+    TlRKey *rk0, *rk;
+    MonoKey *key0, *key1;
+    int32_t *tid0, *tperm, *rv0, *rv, *tM, *tA, *id0, *id1, *pos, *cmax, *srev, *rev, *dirty;
+    const int32_t *d_ivperm, *d_ivs;
+    uint64_t* mk;
+    unsigned long long *cnt, *wkey, *wtid;
+    uint8_t* tmp;
+    JTB_OK(A.put(&d.payload, h->payload, (size_t)h->n_payload, st));
+    JTB_OK(A.put(&poff, poff_v, st)); JTB_OK(A.put(&x.row, row_v, st)); JTB_OK(A.put(&x.shard, shard_v, st));
+    JTB_OK(A.put(&x.inv, inv_v, st)); JTB_OK(A.put(&x.comp, comp_v, st));
+    JTB_OK(A.put(&d.n_keys, H.n_keys, st)); JTB_OK(A.put(&d.key_off, H.key_off, st)); JTB_OK(A.put(&d.keys, H.keys, st));
+    x.n_keys = d.n_keys; x.key_off = d.key_off; x.keys = d.keys;
+    JTB_OK(A.put(&d.t_shard, T.t_shard, st)); JTB_OK(A.put(&tid, T.t_id, st)); JTB_OK(A.put(&d.t_rec, T.t_rec, st));
+    JTB_OK(A.put(&d.t_inv, T.t_inv, st)); JTB_OK(A.put(&d.t_okcomp, T.t_okcomp, st));
+    JTB_OK(A.put(&d.t_fate, T.t_fate, st)); JTB_OK(A.put(&d.t_off, T.t_off, st));
+    x.t_rec = d.t_rec; x.t_id = tid;
+    JTB_OK(A.put(&d.l_shard, T.l_shard, st)); JTB_OK(A.put(&d.l_comp, T.l_comp, st));
+    JTB_OK(A.put(&d.l_poff, T.l_poff, st)); JTB_OK(A.put(&d.rec_base, T.rec_base, st));
+    JTB_OK(A.put(&d.ib, T.ib, st)); JTB_OK(A.put(&d.ib_inv, T.ib_inv, st)); JTB_OK(A.put(&d.ib_off, T.ib_off, st));
+    JTB_OK(A.put(&x.ok_t, ok_t, st)); JTB_OK(A.put(&x.ok_inv, ok_inv, st)); JTB_OK(A.put(&x.ok_pmax, ok_pmax, st));
+    JTB_OK(A.put(&x.ok_off, ok_off, st)); JTB_OK(A.put(&x.cr_t, cr_t, st)); JTB_OK(A.put(&x.cr_inv, cr_inv, st));
+    JTB_OK(A.put(&x.cr_off, cr_off, st));
+    JTB_OK(A.put(&p.rs_off, rs_off, st)); JTB_OK(A.put(&d_ivperm, ivperm, st)); JTB_OK(A.put(&d_ivs, ivs, st));
+    JTB_OK(A.alloc(&key0, m)); JTB_OK(A.alloc(&key1, m)); JTB_OK(A.alloc(&id0, m)); JTB_OK(A.alloc(&id1, m));
+    JTB_OK(A.alloc(&tk0, nT)); JTB_OK(A.alloc(&tk, nT)); JTB_OK(A.alloc(&tid0, nT)); JTB_OK(A.alloc(&tperm, nT));
+    JTB_OK(A.alloc(&d.rec_slot, nR)); JTB_OK(A.alloc(&rk0, nR)); JTB_OK(A.alloc(&rk, nR));
+    JTB_OK(A.alloc(&rv0, nR)); JTB_OK(A.alloc(&rv, nR));
+    JTB_OK(A.alloc(&d.mlk, nT)); JTB_OK(A.alloc(&d.mv, nT)); JTB_OK(A.alloc(&d.mfrom, nT)); JTB_OK(A.alloc(&mk, nT));
+    JTB_OK(A.alloc(&d.wid, (size_t)nL * 5)); JTB_OK(A.alloc(&d.count, (size_t)S * JTB_TL_KINDS));
+    JTB_OK(A.alloc(&tM, nT)); JTB_OK(A.alloc(&tA, nT)); JTB_OK(A.alloc(&x.f1, nT)); JTB_OK(A.alloc(&x.f2, nT));
+    JTB_OK(A.alloc(&x.code, m)); JTB_OK(A.alloc(&x.gkey, m)); JTB_OK(A.alloc(&x.gkept, m));
+    JTB_OK(A.alloc(&x.gdelta, m));
+    JTB_OK(A.alloc(&cnt, (size_t)S * TP_COUNTERS)); JTB_OK(A.alloc(&wkey, S)); JTB_OK(A.alloc(&wtid, S));
+    JTB_OK(A.alloc(&pos, m)); JTB_OK(A.alloc(&cmax, m)); JTB_OK(A.alloc(&rev, m)); JTB_OK(A.alloc(&srev, m));
+    JTB_OK(A.alloc(&p.lo, nT)); JTB_OK(A.alloc(&p.hi, nT)); JTB_OK(A.alloc(&p.jd, nT)); JTB_OK(A.alloc(&p.jc, nT));
+    JTB_OK(A.alloc(&p.flag, nT)); JTB_OK(A.alloc(&p.owner, nT)); JTB_OK(A.alloc(&p.pmin, nT));
+    JTB_OK(A.alloc(&p.pmax, nT)); JTB_OK(A.alloc(&p.dround, nT)); JTB_OK(A.alloc(&p.dg1, nT));
+    JTB_OK(A.alloc(&p.dg2, nT)); JTB_OK(A.alloc(&p.lround, nT));
+    JTB_OK(A.alloc(&p.lcode, m)); JTB_OK(A.alloc(&p.lround_g, m)); JTB_OK(A.alloc(&p.inc, m));
+    JTB_OK(A.alloc(&dirty, (size_t)m + 1)); JTB_OK(A.alloc(&p.pn, m)); JTB_OK(A.alloc(&p.dd, (size_t)m + 1));
+    JTB_OK(A.alloc(&p.poss, (size_t)m * JTB_TP_MAX_GATHER)); JTB_OK(A.alloc(&p.changed, 1));
+    JTB_OK(A.alloc(&p.srounds, S));
+    int32_t* incsum;
+    JTB_OK(A.alloc(&incsum, m));
+    d.tkey = tk; d.tperm = tperm; d.rkey = rk; d.rval = rv;
+    x.ord = id1; x.t_M = tM; x.t_A = tA; x.cnt = cnt; x.wkey = wkey; x.wtid = wtid;
+    p.pos = pos; p.t_shard = d.t_shard; p.t_fate = d.t_fate; p.t_inv = d.t_inv; p.dirty = dirty;
+    p.incsum = incsum;
+    g.tM = tM; g.cnt = cnt; g.wkey = wkey; g.wtid = wtid;
+    size_t tmp_m = 0, tmp_t = 0, tmp_r = 0, tmp_s = 0, tmp_s2 = 0, tmp_s3 = 0;
+    JTB_OK(cub::DeviceRadixSort::SortPairs(nullptr, tmp_m, key0, key1, id0, id1, m, MonoKeyDecomposer{}, st));
+    if (nT > 0)
+        JTB_OK(cub::DeviceRadixSort::SortPairs(nullptr, tmp_t, tk0, tk, tid0, tperm, nT, TlTKeyDecomposer{}, st));
+    if (nR > 0)
+        JTB_OK(cub::DeviceRadixSort::SortPairs(nullptr, tmp_r, rk0, rk, rv0, rv, (int)nR, TlRKeyDecomposer{}, st));
+    JTB_OK(cub::DeviceScan::InclusiveScan(nullptr, tmp_s, pos, cmax, MaxOp{}, m, st));
+    JTB_OK(cub::DeviceScan::InclusiveScan(nullptr, tmp_s2, rev, srev, MinOp{}, m, st));
+    JTB_OK(cub::DeviceScan::InclusiveSum(nullptr, tmp_s3, p.dd, dirty, m + 1, st));
+    const size_t tmp_bytes = g.tmp_bytes = std::max({tmp_m, tmp_t, tmp_r, tmp_s, tmp_s2, tmp_s3});
+    JTB_OK(A.alloc(&tmp, tmp_bytes));
+    g.tmp = tmp;
+    auto grid = [](int64_t n, int per) { return (unsigned)((n + per - 1) / per); };
 
-        JTB_OK(cudaEventRecord(ev0, st));
-        JTB_OK(cudaMemsetAsync(d.mlk, 0x7f, (size_t)nT * 4, st));
-        JTB_OK(cudaMemsetAsync(d.wid, 0xff, (size_t)nL * 40, st));
-        JTB_OK(cudaMemsetAsync(d.count, 0, (size_t)S * JTB_TL_KINDS * 8, st));
-        JTB_OK(cudaMemsetAsync(cnt, 0, (size_t)S * TP_COUNTERS * 8, st));
-        JTB_OK(cudaMemsetAsync(wkey, 0xff, (size_t)S * 8, st));
-        JTB_OK(cudaMemsetAsync(wtid, 0xff, (size_t)S * 8, st));
-        JTB_OK(cudaMemsetAsync(own, 0, (size_t)cells * 8, st));
-        JTB_OK(cudaMemsetAsync(p.owner, 0x7f, (size_t)nT * 4, st));   // RG_NONE
-        JTB_OK(cudaMemsetAsync(p.dround, 0xff, (size_t)nT * 4, st));
-        JTB_OK(cudaMemsetAsync(p.lround, 0xff, (size_t)nT * 4, st));
-        JTB_OK(cudaMemsetAsync(p.lcode, 0, (size_t)m, st));
-        JTB_OK(cudaMemsetAsync(p.srounds, 0, (size_t)S * 4, st));
-        mono_scatter<<<grid((int64_t)m * 32, 256), 256, 0, st>>>(m, d.payload, poff, x.shard, x.inv, x.row, d.n_keys,
-                                                                 d.key_off, d.keys, V, key0, id0);
-        size_t tb = tmp_bytes;
-        JTB_OK(cub::DeviceRadixSort::SortPairs(tmp, tb, key0, key1, id0, id1, m, MonoKeyDecomposer{}, st));
-        if (nT > 0) {
-            tl_tkeys<<<grid(nT, 256), 256, 0, st>>>(nT, d.t_shard, tid, tk0, tid0);
-            tb = tmp_bytes;
-            JTB_OK(cub::DeviceRadixSort::SortPairs(tmp, tb, tk0, tk, tid0, tperm, nT, TlTKeyDecomposer{}, st));
-        }
-        if (nR > 0) {
-            tl_records<<<grid(nR, 256), 256, 0, st>>>(d, rk0, rv0);
-            tb = tmp_bytes;
-            JTB_OK(cub::DeviceRadixSort::SortPairs(tmp, tb, rk0, rk, rv0, rv, (int)nR, TlRKeyDecomposer{}, st));
-        }
-        if (nT > 0) {
-            tl_mval<<<grid(nT, 256), 256, 0, st>>>(d, mk);
-            rx_mark<<<grid(nT, 256), 256, 0, st>>>(d, tM, tA);
-        }
-        // the windows
-        tp_pos<<<grid(m, 256), 256, 0, st>>>(m, id1, pos);
+    JTB_OK(cudaEventRecord(ev0, st));
+    JTB_OK(cudaMemsetAsync(d.mlk, 0x7f, (size_t)nT * 4, st));
+    JTB_OK(cudaMemsetAsync(d.wid, 0xff, (size_t)nL * 40, st));
+    JTB_OK(cudaMemsetAsync(d.count, 0, (size_t)S * JTB_TL_KINDS * 8, st));
+    JTB_OK(cudaMemsetAsync(cnt, 0, (size_t)S * TP_COUNTERS * 8, st));
+    JTB_OK(cudaMemsetAsync(wkey, 0xff, (size_t)S * 8, st));
+    JTB_OK(cudaMemsetAsync(wtid, 0xff, (size_t)S * 8, st));
+    JTB_OK(cudaMemsetAsync(own, 0, (size_t)cells * 8, st));
+    JTB_OK(cudaMemsetAsync(p.owner, 0x7f, (size_t)nT * 4, st));   // RG_NONE
+    JTB_OK(cudaMemsetAsync(p.dround, 0xff, (size_t)nT * 4, st));
+    JTB_OK(cudaMemsetAsync(p.lround, 0xff, (size_t)nT * 4, st));
+    JTB_OK(cudaMemsetAsync(p.lcode, 0, (size_t)m, st));
+    JTB_OK(cudaMemsetAsync(p.srounds, 0, (size_t)S * 4, st));
+    mono_scatter<<<grid((int64_t)m * 32, 256), 256, 0, st>>>(m, d.payload, poff, x.shard, x.inv, x.row, d.n_keys,
+                                                             d.key_off, d.keys, V, key0, id0);
+    size_t tb = tmp_bytes;
+    JTB_OK(cub::DeviceRadixSort::SortPairs(tmp, tb, key0, key1, id0, id1, m, MonoKeyDecomposer{}, st));
+    if (nT > 0) {
+        tl_tkeys<<<grid(nT, 256), 256, 0, st>>>(nT, d.t_shard, tid, tk0, tid0);
         tb = tmp_bytes;
-        JTB_OK(cub::DeviceScan::InclusiveScan(tmp, tb, pos, cmax, MaxOp{}, m, st));
-        tp_ivpos<<<grid(m, 256), 256, 0, st>>>(m, d_ivperm, pos, rev);
+        JTB_OK(cub::DeviceRadixSort::SortPairs(tmp, tb, tk0, tk, tid0, tperm, nT, TlTKeyDecomposer{}, st));
+    }
+    if (nR > 0) {
+        tl_records<<<grid(nR, 256), 256, 0, st>>>(d, rk0, rv0);
         tb = tmp_bytes;
-        JTB_OK(cub::DeviceScan::InclusiveScan(tmp, tb, rev, srev, MinOp{}, m, st));
-        if (nT > 0) tp_window<<<grid(nT, 256), 256, 0, st>>>(x, p, cmax, d_ivs, srev);
-        // the rounds
-        int32_t rounds = 0;
-        for (int32_t r = 0;; ++r) {
-            if (r >= 2) {
-                tb = tmp_bytes;
-                JTB_OK(cub::DeviceScan::InclusiveSum(tmp, tb, p.dd, dirty, m + 1, st));
-            }
-            JTB_OK(cudaMemsetAsync(p.dd, 0, (size_t)(m + 1) * 4, st));
-            JTB_OK(cudaMemsetAsync(x.f1, 0x7f, (size_t)nT * 4, st));
-            JTB_OK(cudaMemsetAsync(x.f2, 0x7f, (size_t)nT * 4, st));
-            JTB_OK(cudaMemsetAsync(p.pmin, 0x7f, (size_t)nT * 4, st));
-            JTB_OK(cudaMemsetAsync(p.pmax, 0xff, (size_t)nT * 4, st));
-            JTB_OK(cudaMemsetAsync(p.changed, 0, 4, st));
-            p.round = r;
-            tp_gaps<<<grid(m, RG_WARPS), RG_WARPS * 32, 0, st>>>(x, p);
-            tp_possible<<<grid((int64_t)m * 32, 256), 256, 0, st>>>(m, p);
+        JTB_OK(cub::DeviceRadixSort::SortPairs(tmp, tb, rk0, rk, rv0, rv, (int)nR, TlRKeyDecomposer{}, st));
+    }
+    if (nT > 0) {
+        tl_mval<<<grid(nT, 256), 256, 0, st>>>(d, mk);
+        rx_mark<<<grid(nT, 256), 256, 0, st>>>(d, tM, tA);
+    }
+    // the windows
+    tp_pos<<<grid(m, 256), 256, 0, st>>>(m, id1, pos);
+    tb = tmp_bytes;
+    JTB_OK(cub::DeviceScan::InclusiveScan(tmp, tb, pos, cmax, MaxOp{}, m, st));
+    tp_ivpos<<<grid(m, 256), 256, 0, st>>>(m, d_ivperm, pos, rev);
+    tb = tmp_bytes;
+    JTB_OK(cub::DeviceScan::InclusiveScan(tmp, tb, rev, srev, MinOp{}, m, st));
+    if (nT > 0) tp_window<<<grid(nT, 256), 256, 0, st>>>(x, p, cmax, d_ivs, srev);
+    // the rounds
+    for (int32_t r = 0;; ++r) {
+        if (r >= 2) {
             tb = tmp_bytes;
-            JTB_OK(cub::DeviceScan::InclusiveSum(tmp, tb, p.inc, incsum, m, st));
-            if (nT > 0) tp_owner<<<grid(nT, 256), 256, 0, st>>>(x, p);
-            JTB_OK(cudaGetLastError());
-            unsigned int changed = 0;
-            JTB_OK(cudaMemcpyAsync(&changed, p.changed, 4, cudaMemcpyDeviceToHost, st));
-            JTB_OK(cudaStreamSynchronize(st));
-            rounds = r + 1;
-            if (rounds >= max_rounds || (r >= 1 && !changed)) break;
+            JTB_OK(cub::DeviceScan::InclusiveSum(tmp, tb, p.dd, dirty, m + 1, st));
         }
-        tp_gap_final<<<grid(m, 256), 256, 0, st>>>(x, p);
-        if (nT > 0) {
-            tp_transfer_final<<<grid(nT, 256), 256, 0, st>>>(x, p);
-            tp_witness_id<<<grid(nT, 256), 256, 0, st>>>(x, p);
-        }
+        JTB_OK(cudaMemsetAsync(p.dd, 0, (size_t)(m + 1) * 4, st));
+        JTB_OK(cudaMemsetAsync(x.f1, 0x7f, (size_t)nT * 4, st));
+        JTB_OK(cudaMemsetAsync(x.f2, 0x7f, (size_t)nT * 4, st));
+        JTB_OK(cudaMemsetAsync(p.pmin, 0x7f, (size_t)nT * 4, st));
+        JTB_OK(cudaMemsetAsync(p.pmax, 0xff, (size_t)nT * 4, st));
+        JTB_OK(cudaMemsetAsync(p.changed, 0, 4, st));
+        p.round = r;
+        tp_gaps<<<grid(m, RG_WARPS), RG_WARPS * 32, 0, st>>>(x, p);
+        tp_possible<<<grid((int64_t)m * 32, 256), 256, 0, st>>>(m, p);
+        tb = tmp_bytes;
+        JTB_OK(cub::DeviceScan::InclusiveSum(tmp, tb, p.inc, incsum, m, st));
+        if (nT > 0) tp_owner<<<grid(nT, 256), 256, 0, st>>>(x, p);
         JTB_OK(cudaGetLastError());
-        JTB_OK(cudaEventRecord(ev1, st));
-        std::vector<unsigned long long> cnt_h((size_t)S * TP_COUNTERS), wkey_h(S), wtid_h(S);
-        std::vector<int32_t> sr_h(S);
-        JTB_OK(cudaMemcpyAsync(cnt_h.data(), cnt, cnt_h.size() * 8, cudaMemcpyDeviceToHost, st));
-        JTB_OK(cudaMemcpyAsync(wkey_h.data(), wkey, (size_t)S * 8, cudaMemcpyDeviceToHost, st));
-        JTB_OK(cudaMemcpyAsync(wtid_h.data(), wtid, (size_t)S * 8, cudaMemcpyDeviceToHost, st));
-        JTB_OK(cudaMemcpyAsync(sr_h.data(), p.srounds, (size_t)S * 4, cudaMemcpyDeviceToHost, st));
+        unsigned int changed = 0;
+        JTB_OK(cudaMemcpyAsync(&changed, p.changed, 4, cudaMemcpyDeviceToHost, st));
         JTB_OK(cudaStreamSynchronize(st));
-        JTB_OK(cudaEventElapsedTime(&ms, ev0, ev1));
-        auto get = [&](auto* dst, const auto* src) {   // one scalar of a witness
-            return cudaMemcpy(dst, src, sizeof *dst, cudaMemcpyDeviceToHost) == cudaSuccess;
-        };
-        auto index_at = [&](int32_t at) -> int32_t {   // completion :index of the read at a sorted position
-            int32_t r;
-            if (!get(&r, id1 + at)) return INT_MIN;
-            return h->index[H.r_ev[d_of[r]]];
-        };
-        for (int32_t s = 0; s < S; ++s) {
-            jtb_tp_shard& o = shards[s];
-            if (!dev[s]) continue;
-            const unsigned long long* c = &cnt_h[(size_t)s * TP_COUNTERS];
-            o.n_explained = (int64_t)c[0];
-            o.n_undecided = (int64_t)c[1];
-            for (int k = 0; k < 4; ++k) o.count_by_kind[k] = (int64_t)c[2 + k];
-            o.n_placed = (int64_t)c[6];
-            o.nodes = (int64_t)c[7];
-            o.rounds = sr_h[s];
-            if (wkey_h[s] != ~0ull) {
-                const int32_t at = (int32_t)(wkey_h[s] >> 3);
-                bool ok = true;
-                o.kind = (int32_t)(wkey_h[s] & 7);
-                o.witness_index = index_at(at);
-                if (at > rs_off[s]) o.lower_index = index_at(at - 1);
-                ok &= get(&o.n_eligible, x.gkept + at);
-                if (o.kind == JTB_TP_DOUBLE || o.kind == JTB_TP_LOST) {
-                    o.transfer_id = (int64_t)(wtid_h[s] ^ 0x8000000000000000ull);
-                    int32_t t = T.t_off[s];
-                    while (T.t_id[t] != o.transfer_id) ++t;
-                    if (o.kind == JTB_TP_DOUBLE) {
-                        int32_t first;
-                        ok &= get(&o.round, p.dround + t) && get(&first, p.dg1 + t);
-                        o.other_index = index_at(first);
-                    } else {
-                        int32_t M;
-                        ok &= get(&o.round, p.lround + t) && get(&M, tM + t);
-                        o.other_index = h->index[h->shard_off[s] + M];
-                    }
-                } else {
-                    ok &= get(&o.key, x.gkey + at) && get(&o.round, p.lround_g + at);
-                    if (o.kind == JTB_TP_KEY) ok &= get(&o.delta, x.gdelta + at);
-                }
-                if (!ok || o.witness_index == INT_MIN || o.lower_index == INT_MIN || o.other_index == INT_MIN) {
-                    err = "cudaMemcpy of a witness field failed";
-                    return -1;
-                }
-                o.valid = JTB_INVALID;
-            } else if (o.n_undecided > 0) {
-                o.valid = JTB_UNKNOWN;
-            }
+        if (r + 1 >= max_rounds || (r >= 1 && !changed)) break;
+    }
+    return 0;
+}
+
+// K12's finals over the stage's device state: the counts, the verdicts and the witnesses into shards[S] (filled with
+// the verdicts of the shards the device does not run first); ev1 is recorded after the last kernel
+inline int tp_finals(cudaStream_t st, cudaEvent_t ev0, cudaEvent_t ev1, const jtb_history* h, TpStage& g,
+                     jtb_tp_shard* shards, float& ms, std::string& err) {
+    const int32_t S = g.S;
+    const MonoHost& H = g.H;
+    const TlHost& T = g.T;
+    for (int32_t s = 0; s < S; ++s) {
+        jtb_tp_shard& o = shards[s];
+        memset(&o, 0, sizeof o);
+        o.valid = JTB_VALID;
+        o.n_reads = H.n_reads[s];
+        o.n_transfers = T.t_off[s + 1] - T.t_off[s];
+        o.witness_index = o.lower_index = o.key = o.other_index = o.round = -1;
+        if (H.n_reads[s] > 0 && !g.dev[s]) {
+            o.valid = JTB_UNKNOWN;
+            o.cause = JTB_CAUSE_PARTIAL_READ;
         }
     }
+    ms = 0;
+    if (g.m == 0) return 0;
+    const int32_t nT = g.nT;
+    RgDev& x = g.x;
+    TpDev& p = g.p;
+    auto grid = [](int64_t n, int per) { return (unsigned)((n + per - 1) / per); };
+    tp_gap_final<<<grid(g.m, 256), 256, 0, st>>>(x, p);
+    if (nT > 0) {
+        tp_transfer_final<<<grid(nT, 256), 256, 0, st>>>(x, p);
+        tp_witness_id<<<grid(nT, 256), 256, 0, st>>>(x, p);
+    }
+    JTB_OK(cudaGetLastError());
+    JTB_OK(cudaEventRecord(ev1, st));
+    std::vector<unsigned long long> cnt_h((size_t)S * TP_COUNTERS), wkey_h(S), wtid_h(S);
+    std::vector<int32_t> sr_h(S);
+    JTB_OK(cudaMemcpyAsync(cnt_h.data(), g.cnt, cnt_h.size() * 8, cudaMemcpyDeviceToHost, st));
+    JTB_OK(cudaMemcpyAsync(wkey_h.data(), g.wkey, (size_t)S * 8, cudaMemcpyDeviceToHost, st));
+    JTB_OK(cudaMemcpyAsync(wtid_h.data(), g.wtid, (size_t)S * 8, cudaMemcpyDeviceToHost, st));
+    JTB_OK(cudaMemcpyAsync(sr_h.data(), p.srounds, (size_t)S * 4, cudaMemcpyDeviceToHost, st));
+    JTB_OK(cudaStreamSynchronize(st));
+    JTB_OK(cudaEventElapsedTime(&ms, ev0, ev1));
+    auto get = [&](auto* dst, const auto* src) {   // one scalar of a witness
+        return cudaMemcpy(dst, src, sizeof *dst, cudaMemcpyDeviceToHost) == cudaSuccess;
+    };
+    auto index_at = [&](int32_t at) -> int32_t {   // completion :index of the read at a sorted position
+        int32_t r;
+        if (!get(&r, x.ord + at)) return INT_MIN;
+        return h->index[H.r_ev[g.d_of[r]]];
+    };
     for (int32_t s = 0; s < S; ++s) {
+        jtb_tp_shard& o = shards[s];
+        if (!g.dev[s]) continue;
+        const unsigned long long* c = &cnt_h[(size_t)s * TP_COUNTERS];
+        o.n_explained = (int64_t)c[0];
+        o.n_undecided = (int64_t)c[1];
+        for (int k = 0; k < 4; ++k) o.count_by_kind[k] = (int64_t)c[2 + k];
+        o.n_placed = (int64_t)c[6];
+        o.nodes = (int64_t)c[7];
+        o.rounds = sr_h[s];
+        if (wkey_h[s] != ~0ull) {
+            const int32_t at = (int32_t)(wkey_h[s] >> 3);
+            bool ok = true;
+            o.kind = (int32_t)(wkey_h[s] & 7);
+            o.witness_index = index_at(at);
+            if (at > g.rs_off[s]) o.lower_index = index_at(at - 1);
+            ok &= get(&o.n_eligible, x.gkept + at);
+            if (o.kind == JTB_TP_DOUBLE || o.kind == JTB_TP_LOST) {
+                o.transfer_id = (int64_t)(wtid_h[s] ^ 0x8000000000000000ull);
+                int32_t t = T.t_off[s];
+                while (T.t_id[t] != o.transfer_id) ++t;
+                if (o.kind == JTB_TP_DOUBLE) {
+                    int32_t first;
+                    ok &= get(&o.round, p.dround + t) && get(&first, p.dg1 + t);
+                    o.other_index = index_at(first);
+                } else {
+                    int32_t M;
+                    ok &= get(&o.round, p.lround + t) && get(&M, g.tM + t);
+                    o.other_index = h->index[h->shard_off[s] + M];
+                }
+            } else {
+                ok &= get(&o.key, x.gkey + at) && get(&o.round, p.lround_g + at);
+                if (o.kind == JTB_TP_KEY) ok &= get(&o.delta, x.gdelta + at);
+            }
+            if (!ok || o.witness_index == INT_MIN || o.lower_index == INT_MIN || o.other_index == INT_MIN) {
+                err = "cudaMemcpy of a witness field failed";
+                return -1;
+            }
+            o.valid = JTB_INVALID;
+        } else if (o.n_undecided > 0) {
+            o.valid = JTB_UNKNOWN;
+        }
+    }
+    return 0;
+}
+
+inline int run_transfer_placement(cudaStream_t st, cudaEvent_t ev0, cudaEvent_t ev1, const jtb_history* h,
+                                  int64_t max_nodes, int32_t max_rounds, int32_t flags, jtb_tp_shard* shards,
+                                  jtb_tp_result* out, std::string& err) {
+    const auto t0 = std::chrono::steady_clock::now();
+    if (!h || !shards || !out) { err = "null argument"; return -2; }
+    TpStage g;
+    if (int rc = tp_stage(st, ev0, h, max_nodes, max_rounds, flags, g, err)) return rc;
+    float ms = 0;
+    if (int rc = tp_finals(st, ev0, ev1, h, g, shards, ms, err)) return rc;
+    memset(out, 0, sizeof *out);
+    for (int32_t s = 0; s < g.S; ++s) {
         const jtb_tp_shard& o = shards[s];
+        out->n_reads += o.n_reads;
+        out->n_transfers += o.n_transfers;
         out->n_explained += o.n_explained;
         out->n_unexplained += o.count_by_kind[0] + o.count_by_kind[1];
         out->n_double += o.count_by_kind[2];
@@ -637,7 +686,7 @@ inline int run_transfer_placement(cudaStream_t st, cudaEvent_t ev0, cudaEvent_t 
         out->nodes += o.nodes;
         out->rounds = std::max(out->rounds, (int64_t)o.rounds);
     }
-    roll_up(out, shards, S, ms, t0);
+    roll_up(out, shards, g.S, ms, t0);
     return 0;
 }
 

@@ -20,14 +20,14 @@ _SOURCES = ["jtb_abi.cu", "jtb_prep.cpp", "jtb_multi.cpp"]
 _DEPS = _SOURCES + ["jtb_prep.h", "jtb_expand.h", "jtb_wgl.cuh", "jtb_scout.cuh", "jtb_scans.cuh",
                     "jtb_table_bench.cuh", "jtb_level.cuh", "jtb_partition.cuh", "jtb_monotonic.cuh",
                     "jtb_counter_bounds.cuh", "jtb_transfer_lookups.cuh", "jtb_read_explanations.cuh",
-                    "jtb_read_gaps.cuh", "jtb_transfer_placement.cuh", "jtb_call.cuh"]
+                    "jtb_read_gaps.cuh", "jtb_transfer_placement.cuh", "jtb_serial_witness.cuh", "jtb_call.cuh"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared", "-ldl"]
 
 EXPORTS = ["jtb_abi_version", "jtb_device_count", "jtb_create", "jtb_destroy", "jtb_last_error",
            "jtb_check_linearizable", "jtb_check_set_full", "jtb_check_bank_totals", "jtb_check_monotonic_keys",
            "jtb_check_counter_bounds", "jtb_check_transfer_lookups", "jtb_check_read_explanations",
-           "jtb_check_read_gaps", "jtb_check_transfer_placement",
+           "jtb_check_read_gaps", "jtb_check_transfer_placement", "jtb_check_serial_witness",
            "jtb_table_bench", "jtb_get_stats", "jtb_struct_size", "jtb_prepare_seconds", "jtb_prepare_info",
            "jtb_final_configs", "jtb_gather_bench", "jtb_host_alloc", "jtb_host_free", "jtb_partition_by_key", "jtb_ledger_balances", "jtb_multi_create", "jtb_multi_create_error", "jtb_multi_destroy", "jtb_multi_n_gpus",
            "jtb_multi_last_error", "jtb_multi_check_linearizable", "jtb_multi_check_set_full"]
@@ -84,6 +84,8 @@ def lib() -> C.CDLL:
             L.jtb_check_read_gaps.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p]
             L.jtb_check_transfer_placement.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_int32,
                                                        C.c_void_p, C.c_void_p]
+            L.jtb_check_serial_witness.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_int32,
+                                                   C.c_void_p, C.c_void_p, C.c_void_p]
             L.jtb_table_bench.argtypes = [C.c_void_p, C.c_uint64, C.c_int, C.c_int, C.c_void_p,
                                           C.c_void_p, C.c_void_p]
             L.jtb_gather_bench.argtypes = [C.c_void_p, C.c_uint64, C.c_int, C.c_int, C.c_uint32, C.c_int, C.c_int,
@@ -283,6 +285,30 @@ class Context:
         if rc != 0:
             raise NativeError(f"jtb_check_transfer_placement rc={rc}: {self._err()}")
         return abi.tp_to_dict(res, shards[:h.n_shards])
+
+    # ---- K13: serial-witness check --------------------------------------------------------------------------------
+    def check_serial_witness(self, h: FlatHistory, max_nodes: int = 0, max_rounds: int = 0,
+                             witness: bool = False) -> dict:
+        """A proof of linearizability, or nothing: the transfer-placement check, then one explanation chosen per read
+        gap (no transfer in two) and the serial order it gives checked against real time.  A shard is VALID (its reads
+        and transfers are linearizable for the per-account counters, and so for the bank model with negative balances
+        allowed) or UNKNOWN with a cause, never INVALID (input: the ledger-lookups form; max_nodes and max_rounds as for
+        check_transfer_placement).  {"valid", "n_failures", "n_reads", "n_transfers", "n_committed",
+        "n_committed_crashed", "n_after", "nodes", "rounds", "seconds_kernel", "seconds_total", "shards": [{"valid",
+        "cause", "n_reads", "n_transfers", "n_committed", "n_committed_crashed", "n_after", "nodes", "rounds",
+        "fail_index", "transfer_id"}]}; witness=True adds "commit_read": per transfer micro-op in history order, the
+        completion :index of the first read whose state holds it, abi.SW_NEVER, SW_AFTER or SW_FREE."""
+        import numpy as np
+        ch = as_c_history(h)
+        shards = (abi.CSwShard * max(1, h.n_shards))()
+        res = abi.CSwResult()
+        cr = np.zeros(max(1, abi.n_transfer_records(h)), np.int32) if witness else None
+        rc = lib().jtb_check_serial_witness(self._h, C.addressof(ch), max_nodes, max_rounds, 0,
+                                            cr.ctypes.data if witness else None, C.addressof(shards),
+                                            C.addressof(res))
+        if rc != 0:
+            raise NativeError(f"jtb_check_serial_witness rc={rc}: {self._err()}")
+        return abi.sw_to_dict(res, shards[:h.n_shards], cr[:res.n_transfers].copy() if witness else None)
 
     def final_configs(self, h: FlatHistory, model: CModel, shard: int = 0, cap: int = 10) -> dict:
         """knossos' :configs of an INVALID shard (`jtb_final_configs`): call directly after `check_linearizable`

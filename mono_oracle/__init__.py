@@ -9,7 +9,9 @@ minima.  See transfer_lookups.cpp.  RX_BRUTE enumerates every subset of a read's
 library's budgeted pruning and depth-first search over a sweep.  See read_explanations.cpp.  RG_BRUTE enumerates every
 subset of a gap's eligible transfers; RG_SEARCH is the library's amount filter, caps and search per gap.  See
 read_gaps.cpp.  TP_BRUTE enumerates every placement of each transfer in a gap of its window; TP_SEARCH is the
-library's rounds of per-gap searches with owned transfers carried between gaps.  See transfer_placement.cpp."""
+library's rounds of per-gap searches with owned transfers carried between gaps.  See transfer_placement.cpp.
+SW_SEARCH is TP_SEARCH followed by the library's witness rounds, real-time pass and commit_read.  See
+serial_witness.cpp."""
 from __future__ import annotations
 
 import ctypes as C
@@ -26,6 +28,7 @@ TL_LITERAL, TL_SWEEP = 0, 1
 RX_BRUTE, RX_SEARCH = 0, 1
 RG_BRUTE, RG_SEARCH = 0, 1
 TP_BRUTE, TP_SEARCH = 0, 1
+SW_SEARCH = 1
 DECIDE_PARTIAL = 1 << 16   # decide shards with partial reads instead of reporting them UNKNOWN
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB = None
@@ -37,7 +40,7 @@ def build(force: bool = False) -> str:
     so = os.path.join(_HERE, "libjtb_mono_oracle.so")
     srcs = [os.path.join(_HERE, f) for f in ("mono_oracle.cpp", "counter_bounds.cpp", "transfer_lookups.cpp",
                                                 "read_explanations.cpp", "read_gaps.cpp", "transfer_placement.cpp",
-                                                "gaps_common.h", "Makefile")]
+                                                "serial_witness.cpp", "gaps_common.h", "Makefile")]
     srcs.append(os.path.join(_HERE, "..", "include", "jtb_check.h"))
     stale = not os.path.exists(so) or any(os.path.getmtime(s) > os.path.getmtime(so) for s in srcs)
     if force or stale:
@@ -68,6 +71,9 @@ def lib() -> C.CDLL:
         _LIB.jtbm_tp_last_error.restype = C.c_char_p
         _LIB.jtbm_check_transfer_placement.argtypes = [C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_int32,
                                                        C.c_void_p, C.c_void_p]
+        _LIB.jtbm_sw_last_error.restype = C.c_char_p
+        _LIB.jtbm_check_serial_witness.argtypes = [C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_int32,
+                                                   C.c_void_p, C.c_void_p, C.c_void_p]
     return _LIB
 
 
@@ -158,3 +164,18 @@ def check_transfer_placement(h: FlatHistory, algo: int = TP_SEARCH, max_nodes: i
     if rc != 0:
         raise RuntimeError(lib().jtbm_tp_last_error().decode())
     return abi.tp_to_dict(res, shards[:h.n_shards])
+
+
+def check_serial_witness(h: FlatHistory, algo: int = SW_SEARCH, max_nodes: int = 0, max_rounds: int = 0,
+                         flags: int = 0, witness: bool = True) -> dict:
+    """Twin of `jtb_check_serial_witness` (same result dict as `native.Context.check_serial_witness`)."""
+    import numpy as np
+    ch = as_c_history(h)
+    shards = (abi.CSwShard * max(1, h.n_shards))()
+    res = abi.CSwResult()
+    cr = np.zeros(max(1, abi.n_transfer_records(h)), np.int32)
+    rc = lib().jtbm_check_serial_witness(C.addressof(ch), max_nodes, max_rounds, flags, algo,
+                                         cr.ctypes.data if witness else None, C.addressof(shards), C.addressof(res))
+    if rc != 0:
+        raise RuntimeError(lib().jtbm_sw_last_error().decode())
+    return abi.sw_to_dict(res, shards[:h.n_shards], cr[:res.n_transfers].copy() if witness else None)
