@@ -242,8 +242,9 @@ typedef struct jtb_bank_result {
 
 /* ---- monotonic-key check (Elle's monotonic-key graph, src/tigerbeetle/elle/core.clj) ------------------------------
  * Nodes are the :ok reads (process >= 0, f == JTB_F_READ, type == JTB_T_OK, payload_len >= 0).  A read's payload is
- * (key:int32, value_lo:int32, value_hi:int32) triples, value = int64; for ledger histories key = 2*account + field,
- * field 0 = debits-posted, 1 = credits-posted (counters that only grow).  Edges:
+ * (key:int32, value_lo:int32, value_hi:int32) triples, value = int64 of any sign; for ledger histories key = 2*account
+ * + field, field 0 = debits-posted, 1 = credits-posted (counters that only grow), so with accounts in [0, 2^30) every
+ * key lies in [0, INT32_MAX].  Reads are ordered by the sum of their values, taken in 128 bits.  Edges:
  *   monotonic  r -> s  when v_k(r) < v_k(s) for some key k both read
  *   real-time  r -> s  when r's completion precedes s's invocation (the latest invoke of s's process before s
  *                      completes; off with JTB_MONO_NO_REALTIME)
@@ -280,7 +281,8 @@ typedef struct jtb_mono_result {
 /* ---- counter-bounds check (DESIGN.md "K8 counter-bounds check") ------------------------------------------------------
  * The same reads as the monotonic-key check (:ok, f == JTB_F_READ, (key, value_lo, value_hi) triples, key =
  * 2*account + field).  A transfer is an invoke with f == JTB_F_TRANSFER, a = amount, b = debit account, c = credit
- * account; its fate is the next event of its process (:ok, :info, :fail, or none).  It adds `a` to key 2b+0
+ * account (amounts int32 >= 0, accounts in [0, 2^30)); its fate is the next event of its process (:ok, :info, :fail,
+ * or none).  It adds `a` to key 2b+0
  * (debits-posted) and to key 2c+1 (credits-posted); :fail transfers add nothing.  Positions are event positions in the
  * shard.  Counters start at zero and only grow, so under strict serializability every key k an :ok read r observes
  * satisfies L_k(r) <= v_k(r) <= U_k(r):
@@ -322,7 +324,7 @@ typedef struct jtb_cb_result {
  * one 5-int32 record (id_lo, id_hi, debit, credit, amount) per [:t ...] micro-op; each is one transfer with the txn's
  * interval and fate (the next event of its process).  A lookup is an :ok event with f == JTB_F_LOOKUP whose payload is
  * the returned records in the same layout; its invocation is the latest invoke of its process.  Ids are int64
- * (id_hi << 32 | id_lo).  With l an :ok lookup and t a transfer of the same shard, each of these proves an anomaly:
+ * (id_hi << 32 | id_lo) of any sign, ordered as signed integers.  With l an :ok lookup and t a transfer of the same shard, each of these proves an anomaly:
  *   1 PHANTOM            a record whose id no transfer invoke of the shard carries
  *   2 MISMATCH           a record whose (debit, credit, amount) differs from its invocation's
  *   3 FAILED_VISIBLE     a record of a transfer whose fate is :fail
