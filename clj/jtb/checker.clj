@@ -563,6 +563,27 @@
           (<= 0 (at (+ s 9)))   (assoc :op (by-index (at (+ s 9))))
           (<= 0 (at (+ s 10)))  (assoc :transfer-id (at (+ s 10))))))))
 
+(defn repaired-witness-checker
+  "serial-witness-checker with repairs: a shard the serial witness leaves :no-witness or :real-time gets up to
+  {:max-repairs n} repair rounds, each banning the (transfer, gap) pairs the failure blames and choosing the released
+  gaps' explanations again.  :valid? true is the same proof; a history the serial witness proves comes back unchanged.
+  Add it to the compose map at tests/ledger.clj:363-367 as `:repaired-witness (repaired-witness-checker {})`.
+  Result: serial-witness-checker's map plus :repairs and :ban-count."
+  [opts]
+  (reify checker/Checker
+    (check [_ _test history _opts]
+      (let [{:keys [arrays by-index]} (flatten-history :ledger-lookups history)
+            res (Native/checkRepairedWitness @ctx arrays (long (:max-nodes opts 0)) (int (:max-rounds opts 0))
+                                             (int (:max-repairs opts 0)))
+            at  (fn [i] (aget res (int i)))
+            s   14]                                        ; shard 0: valid cause reads transfers committed ...
+        (cond-> {:valid? (verdict (at s)) :read-count (at (+ s 2)) :transfer-count (at (+ s 3))
+                 :committed-count (at (+ s 4)) :committed-crashed-count (at (+ s 5)) :after-count (at (+ s 6))
+                 :rounds (at (+ s 8)) :repairs (at (+ s 11)) :ban-count (at (+ s 12))}
+          (pos? (at (+ s 1)))   (assoc :cause (sw-cause (at (+ s 1))))
+          (<= 0 (at (+ s 9)))   (assoc :op (by-index (at (+ s 9))))
+          (<= 0 (at (+ s 10)))  (assoc :transfer-id (at (+ s 10))))))))
+
 ;; ---- independent ----------------------------------------------------------------------------------------------
 (defn independent-checker
   "Like (independent/checker (checker/compose checkers)) for a map {name checker-kind} built from THIS namespace's

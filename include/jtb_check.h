@@ -24,7 +24,7 @@
 extern "C" {
 #endif
 
-#define JTB_ABI_VERSION 9
+#define JTB_ABI_VERSION 10
 
 /* ---- verdict lattice (jepsen.checker/merge-valid) ------------------------------------------- */
 #define JTB_VALID   0
@@ -610,6 +610,56 @@ typedef struct jtb_sw_result {
     double  seconds_total;      /* host wall time of the call incl. the host pass, H2D, D2H                           */
 } jtb_sw_result;
 
+/* ---- repaired serial witness (DESIGN.md "K14 repaired serial witness") ---------------------------------------------
+ * The serial-witness check, then, on a shard it leaves NO_WITNESS or REAL_TIME, up to max_repairs repair rounds.  A
+ * chosen transfer is one the witness (not the transfer-placement check) put in a gap; a ban is a (gap, transfer) pair,
+ * kept for good.  P^_g is the real-time point of g's lower read from the reads and the owned transfers alone.
+ *   - NO_WITNESS: every gap the failing round did not explain (every unfixed gap when max_rounds ran out) steals: it
+ *     gathers as a witness round does, with the chosen transfers counted as free and the repair filter below, and
+ *     searches; a thief keeps its solution when no smaller thief took one of its transfers, and each chosen transfer
+ *     it takes is banned in the gap that had it;
+ *   - REAL_TIME: a chosen t in D_g is banned in g when cp(t) <= P_g, or when iv(t) is at or after the smallest
+ *     completion of what must follow g (the reads from g's upper read on, D_h for h > g, the failing :ok transfers
+ *     after the last read).
+ * The gaps of the new bans and the failing gaps are released (unfixed, their choices owned by no gap), a kept thief
+ * is fixed with its loot, and the witness rounds run again over the unfixed gaps; their gathers drop banned pairs and
+ * every transfer with cp(t) <= P^_g.  Then the real-time pass and the re-sum run unchanged, so a VALID is the same
+ * proof as the serial-witness check's.  A repair that records no new ban ends the shard's repairs.  A shard the
+ * serial-witness check proves is returned as that check returns it. */
+#define JTB_RW_DEFAULT_MAX_REPAIRS 32
+
+typedef struct jtb_rw_shard {
+    int32_t valid;              /* JTB_VALID / JTB_UNKNOWN                                                            */
+    int32_t cause;              /* JTB_CAUSE_* when valid == JTB_UNKNOWN (of the last witness when it was repaired)   */
+    int32_t n_reads;
+    int32_t n_transfers;
+    int64_t n_committed;        /* VALID: transfers committed in some gap                                             */
+    int64_t n_committed_crashed;/* VALID: of them, the crashed ones                                                   */
+    int64_t n_after;            /* VALID: :ok transfers committed after the last read                                 */
+    int64_t nodes;              /* search nodes of every witness round, repairs included                              */
+    int32_t rounds;             /* witness rounds that ran a gap of the shard, repairs included                       */
+    int32_t fail_index;         /* as jtb_sw_shard's, of the last witness                                             */
+    int64_t transfer_id;        /* as jtb_sw_shard's, of the last witness                                             */
+    int32_t repairs;            /* repair rounds run on the shard                                                     */
+    int32_t n_bans;             /* (transfer, gap) bans recorded                                                      */
+} jtb_rw_shard;
+
+typedef struct jtb_rw_result {
+    int32_t valid;
+    int32_t n_failures;
+    int64_t n_reads;
+    int64_t n_transfers;
+    int64_t n_committed;
+    int64_t n_committed_crashed;
+    int64_t n_after;
+    int64_t nodes;
+    int64_t rounds;             /* the most witness rounds of any shard                                               */
+    int64_t repairs;            /* the most repair rounds of any shard                                                */
+    int64_t n_bans;
+    double  seconds_kernel;
+    double  seconds_total;
+} jtb_rw_result;
+
 typedef struct jtb_ctx jtb_ctx;
 
 /* ---- lifecycle -------------------------------------------------------------------------------- */
@@ -618,7 +668,8 @@ int         jtb_abi_version(void);
  * 0 jtb_history, 1 jtb_model, 2 jtb_opts, 3 jtb_lin_shard, 4 jtb_lin_result, 5 jtb_setfull_shard,
  * 6 jtb_setfull_out, 7 jtb_bank_result, 8 jtb_final_config, 9 jtb_mono_shard, 10 jtb_mono_result, 11 jtb_cb_shard,
  * 12 jtb_cb_result, 13 jtb_tl_shard, 14 jtb_tl_result, 15 jtb_rx_shard, 16 jtb_rx_result, 17 jtb_rg_shard,
- * 18 jtb_rg_result, 19 jtb_tp_shard, 20 jtb_tp_result, 21 jtb_sw_shard, 22 jtb_sw_result; -1 otherwise */
+ * 18 jtb_rg_result, 19 jtb_tp_shard, 20 jtb_tp_result, 21 jtb_sw_shard, 22 jtb_sw_result, 23 jtb_rw_shard,
+ * 24 jtb_rw_result; -1 otherwise */
 long        jtb_struct_size(int which);
 int         jtb_device_count(void);                 /* number of CUDA devices, <0 on error          */
 jtb_ctx*    jtb_create(const jtb_opts* opts);       /* NULL on failure (no CUDA device etc.)        */
@@ -718,6 +769,13 @@ int jtb_check_transfer_placement(jtb_ctx* ctx, const jtb_history* h, int64_t max
  * context stays usable). */
 int jtb_check_serial_witness(jtb_ctx* ctx, const jtb_history* h, int64_t max_nodes, int32_t max_rounds, int32_t flags,
                              int32_t* commit_read, jtb_sw_shard* shards, jtb_sw_result* out);
+
+/* ---- repaired serial witness (see jtb_rw_shard above) ---------------------------------------------------------- *
+ * As jtb_check_serial_witness; max_rounds bounds each run of the witness rounds (the first and one per repair);
+ * max_repairs <= 0 means JTB_RW_DEFAULT_MAX_REPAIRS; flags is reserved and must be 0. */
+int jtb_check_repaired_witness(jtb_ctx* ctx, const jtb_history* h, int64_t max_nodes, int32_t max_rounds,
+                               int32_t max_repairs, int32_t flags, int32_t* commit_read, jtb_rw_shard* shards,
+                               jtb_rw_result* out);
 
 /* ---- multi-GPU fan-out inside the library (SURVEY §8(b) `n_gpus`, §8(e)) ----------------------------------- *
  * What `independent/checker` (set_full.clj:155) does over JVM threads, done over the GPUs of one box for a host

@@ -150,4 +150,15 @@ public final class Native {
      *     nCommitted, nCommittedCrashed, nAfter, nodes, rounds, failIndex, transferId}
      */
     public static native long[] checkSerialWitness(long ctx, Object[] history, long maxNodes, int maxRounds);
+
+    /**
+     * {@code jtb_check_repaired_witness}: {@link #checkSerialWitness} with up to {@code maxRepairs} repair rounds
+     * (<= 0: the library's default) on the shards it leaves no-witness or real-time.
+     *
+     * @return {@code [valid, nFailures, nReads, nTransfers, nCommitted, nCommittedCrashed, nAfter, nodes, rounds,
+     *     repairs, nBans, kernelNs, totalNs, nShards]} followed by 13 longs per shard: {@code valid, cause, nReads,
+     *     nTransfers, nCommitted, nCommittedCrashed, nAfter, nodes, rounds, failIndex, transferId, repairs, nBans}
+     */
+    public static native long[] checkRepairedWitness(long ctx, Object[] history, long maxNodes, int maxRounds,
+                                                     int maxRepairs);
 }

@@ -5,7 +5,7 @@ import ctypes as C
 
 from .history import MAX_ACCOUNTS
 
-ABI_VERSION = 9
+ABI_VERSION = 10
 OPT_NO_EAGER_READS = 1
 OPT_NO_SCOUTS = 2
 OPT_ENGINE_LEVEL = 4
@@ -353,6 +353,31 @@ def sw_to_dict(res, shards, commit_read=None) -> dict:
     micro-op in history order) when it was asked for."""
     out = {f: getattr(res, f) for f in SW_RESULT_FIELDS}
     out["shards"] = [{f: getattr(s, f) for f in SW_SHARD_FIELDS} for s in shards]
+    if commit_read is not None:
+        out["commit_read"] = commit_read
+    return out
+
+
+RW_DEFAULT_MAX_REPAIRS = 32
+
+
+class CRwShard(C.Structure):
+    """jtb_rw_shard: the repaired-serial-witness verdict of one shard."""
+    _fields_ = CSwShard._fields_ + [("repairs", C.c_int32), ("n_bans", C.c_int32)]
+
+
+class CRwResult(C.Structure):
+    _fields_ = CSwResult._fields_[:9] + [("repairs", C.c_int64), ("n_bans", C.c_int64)] + CSwResult._fields_[9:]
+
+
+RW_SHARD_FIELDS = SW_SHARD_FIELDS + ("repairs", "n_bans")
+RW_RESULT_FIELDS = SW_RESULT_FIELDS[:9] + ("repairs", "n_bans") + SW_RESULT_FIELDS[9:]
+
+
+def rw_to_dict(res, shards, commit_read=None) -> dict:
+    """As sw_to_dict, for jtb_rw_result / jtb_rw_shard."""
+    out = {f: getattr(res, f) for f in RW_RESULT_FIELDS}
+    out["shards"] = [{f: getattr(s, f) for f in RW_SHARD_FIELDS} for s in shards]
     if commit_read is not None:
         out["commit_read"] = commit_read
     return out

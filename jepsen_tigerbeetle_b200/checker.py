@@ -633,6 +633,32 @@ class SerialWitness(Checker, _Native):
         return out
 
 
+class RepairedWitness(SerialWitness):
+    """The serial-witness check with repairs, on the GPU (K14): a shard the serial-witness check leaves :unknown
+    ("no-witness" or "real-time") gets up to max-repairs repair rounds, each banning the (transfer, gap) pairs the
+    failure blames and choosing the released gaps' explanations again; a VALID is the same proof, and a shard the
+    serial-witness check proves comes back unchanged.  Result: SerialWitness's map plus repairs and ban-count."""
+
+    def __init__(self, checker_opts: Mapping[str, Any] | None = None, ctx: Context | None = None,
+                 **ctx_opts) -> None:
+        SerialWitness.__init__(self, checker_opts, ctx, **ctx_opts)
+        self.max_repairs = int((checker_opts or {}).get("max-repairs", 0))
+
+    def _shard_map(self, s: dict) -> dict:
+        m = SerialWitness._shard_map(self, s)
+        m.update({"repairs": s["repairs"], "ban-count": s["n_bans"]})
+        return m
+
+    def check_flat(self, test, h: FlatHistory) -> tuple[dict, list[dict]]:
+        r = self.ctx.check_repaired_witness(h, self.max_nodes, self.max_rounds, self.max_repairs)
+        top = {"valid?": VERDICT_NAME[r["valid"]], "read-count": r["n_reads"], "transfer-count": r["n_transfers"],
+               "committed-count": r["n_committed"], "committed-crashed-count": r["n_committed_crashed"],
+               "after-count": r["n_after"], "rounds": r["rounds"], "repairs": r["repairs"],
+               "ban-count": r["n_bans"], "nodes": r["nodes"], "seconds-kernel": r["seconds_kernel"],
+               "seconds-total": r["seconds_total"]}
+        return top, [self._shard_map(s) for s in r["shards"]]
+
+
 class Compose(Checker):
     """`(checker/compose {name checker ...})`: run each, `:valid?` = merge-valid of the results."""
 
@@ -758,6 +784,12 @@ def serial_witness_checker(opts: Mapping[str, Any] | None = None, **kw) -> Seria
     """A proof of linearizability for ledger histories, or :unknown (K13); {"max-nodes": n} and {"max-rounds": n} as
     for the transfer-placement check it runs first."""
     return SerialWitness(opts, **kw)
+
+
+def repaired_witness_checker(opts: Mapping[str, Any] | None = None, **kw) -> RepairedWitness:
+    """The serial-witness check with repair rounds (K14); {"max-nodes": n} and {"max-rounds": n} as for the
+    serial-witness check, {"max-repairs": n} the repair rounds (default abi.RW_DEFAULT_MAX_REPAIRS)."""
+    return RepairedWitness(opts, **kw)
 
 
 def compose(checkers: Mapping[str, Checker]) -> Compose:
@@ -929,15 +961,16 @@ def ledger_checker(checker_opts: Mapping[str, Any] | None = None, ctx: Context |
                    linear: bool = True, monotonic: bool = False, counter_bounds: bool = False,
                    transfer_lookups: bool = False, read_explanations: bool = False,
                    read_gaps: bool = False, transfer_placement: bool = False,
-                   serial_witness: bool = False) -> Compose:
+                   serial_witness: bool = False, repaired_witness: bool = False) -> Compose:
     """The ledger test's checker (tests/ledger.clj:363-367) minus the gnuplot plotter, plus the
     linearizability search the north-star adds and, with monotonic=True, the monotonic-key check, with
     counter_bounds=True, the counter-bounds check, with transfer_lookups=True, the transfer-lookup check, with
     read_explanations=True, the read-explanation check, with read_gaps=True, the read-gap check, with
-    transfer_placement=True, the transfer-placement check and, with serial_witness=True, the serial-witness check:
+    transfer_placement=True, the transfer-placement check, with serial_witness=True, the serial-witness check and,
+    with repaired_witness=True, the repaired serial witness:
         {:SI (checker opts) :lookup-transfers ... :final-reads ... :unexpected-ops ... [:linear ...] [:monotonic ...]
          [:counter-bounds ...] [:transfer-lookups ...] [:read-explanations ...] [:read-gaps ...]
-         [:transfer-placement ...] [:serial-witness ...]}"""
+         [:transfer-placement ...] [:serial-witness ...] [:repaired-witness ...]}"""
     cs: dict[str, Checker] = {"SI": bank_checker(checker_opts, ctx=ctx),
                               "lookup-transfers": lookup_all_invoked_transfers(),
                               "final-reads": final_reads(), "unexpected-ops": unexpected_ops()}
@@ -957,4 +990,6 @@ def ledger_checker(checker_opts: Mapping[str, Any] | None = None, ctx: Context |
         cs["transfer-placement"] = transfer_placement_checker(ctx=ctx)
     if serial_witness:
         cs["serial-witness"] = serial_witness_checker(ctx=ctx)
+    if repaired_witness:
+        cs["repaired-witness"] = repaired_witness_checker(ctx=ctx)
     return compose(cs)

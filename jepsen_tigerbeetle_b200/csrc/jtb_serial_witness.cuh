@@ -84,19 +84,16 @@ __global__ void sw_init(RgDev d, TpDev p, SwDev w) {
     if (!zero) atomicAdd(w.unfixed, 1);
 }
 
-// warp per unfixed gap: the gather of a K12 round >= 1 and one search; its first solution is the gap's choice
-__global__ void __launch_bounds__(RG_WARPS * 32) sw_gaps(RgDev d, TpDev p, SwDev w) {
-    __shared__ RgWarp smem[RG_WARPS];
-    const int lane = threadIdx.x & 31;
-    RgWarp& G = smem[threadIdx.x >> 5];
+// one warp, gap i: gather the candidates `take` admits (with rg_gather's own filters) and run one search; on EXPLAINED
+// its first solution goes into the gap's row of K12's poss (pn = chosen) and every chosen transfer takes the smallest
+// choosing gap (atomicMin into w.cmin)
+template <class Take>
+__device__ __forceinline__ bool sw_solve(const RgDev& d, const TpDev& p, const SwDev& w, RgWarp& G, int lane,
+                                         int32_t i, Take take, int64_t& nodes, int32_t& chosen) {
     RxWarp& W = G.x;
-    const int64_t wi = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
-    if (wi >= d.m || w.fixed[wi]) return;
-    const int32_t i = (int32_t)wi, u = d.ord[i], s = d.shard[u], K = d.n_keys[s], cp = d.comp[u];
+    const int32_t u = d.ord[i], s = d.shard[u], K = d.n_keys[s], cp = d.comp[u];
     const int32_t lower = i > 0 && d.shard[d.ord[i - 1]] == s ? d.ord[i - 1] : -1;
     const int32_t ivl = lower >= 0 ? d.inv[lower] : -1;
-    int64_t nodes = 0;
-    int32_t chosen = 0;
     bool ok = false;
     if (K <= JTB_RG_MAX_KEYS) {
         const int64_t* vu = d.V + d.row[u];
@@ -113,9 +110,7 @@ __global__ void __launch_bounds__(RG_WARPS * 32) sw_gaps(RgDev d, TpDev p, SwDev
         neg = __any_sync(0xffffffffu, neg);
         __syncwarp();
         if (!neg) {
-            const int32_t n = rg_gather(d, G, s, K, cp, ivl, lane, [&](int32_t t) {
-                return (p.flag[t] & TP_WIN) && p.lo[t] <= i && i <= p.hi[t] && p.owner[t] == RG_NONE;
-            });
+            const int32_t n = rg_gather(d, G, s, K, cp, ivl, lane, take);
             __syncwarp();
             if (n <= JTB_RG_MAX_GATHER) {
                 int32_t root_key, kept;
@@ -141,6 +136,22 @@ __global__ void __launch_bounds__(RG_WARPS * 32) sw_gaps(RgDev d, TpDev p, SwDev
             }
         }
     }
+    return ok;
+}
+
+// warp per unfixed gap: the gather of a K12 round >= 1 and one search; its first solution is the gap's choice
+__global__ void __launch_bounds__(RG_WARPS * 32) sw_gaps(RgDev d, TpDev p, SwDev w) {
+    __shared__ RgWarp smem[RG_WARPS];
+    const int lane = threadIdx.x & 31;
+    RgWarp& G = smem[threadIdx.x >> 5];
+    const int64_t wi = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
+    if (wi >= d.m || w.fixed[wi]) return;
+    const int32_t i = (int32_t)wi, s = d.shard[d.ord[i]];
+    int64_t nodes = 0;
+    int32_t chosen = 0;
+    const bool ok = sw_solve(d, p, w, G, lane, i, [&](int32_t t) {
+        return (p.flag[t] & TP_WIN) && p.lo[t] <= i && i <= p.hi[t] && p.owner[t] == RG_NONE;
+    }, nodes, chosen);
     if (lane != 0) return;
     atomicAdd(&w.cnt[(int64_t)s * SW_COUNTERS + 3], (unsigned long long)nodes);
     atomicMax(&p.srounds[s], w.round + 1);

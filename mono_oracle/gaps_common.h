@@ -7,6 +7,7 @@
 #include <climits>
 #include <cstdint>
 #include <cstdio>
+#include <functional>
 #include <string>
 #include <unordered_map>
 #include <unordered_set>
@@ -392,15 +393,18 @@ struct Gap {
 };
 
 // The gather of gap i (upper read u, lower read l) into pb.P, with pb.d = Delta': round 0 every eligible transfer, a
-// later round (or a witness round) only the in-window ones no gap owns.  false: past JTB_TP_MAX_GATHER.
+// later round (or a witness round) only the in-window ones no gap owns; keep (may be null) drops more.  false: past
+// JTB_TP_MAX_GATHER.
 bool gather_gap(const Shard& S, const Index& X, const std::vector<Window>& W, const std::vector<int32_t>& owner,
-                const XRead& u, const XRead* l, int32_t i, int32_t round, Problem& pb) {
+                const XRead& u, const XRead* l, int32_t i, int32_t round, Problem& pb,
+                const std::function<bool(int32_t)>* keep = nullptr) {
     const int32_t K = (int32_t)pb.d.size();
     const int32_t ivl = l ? l->inv : -1;
     auto take = [&](int32_t t) {
         const XTransfer& x = S.T[t];
         if (x.fate == JTB_T_FAIL || !(x.inv < u.comp) || !(x.A < u.comp) || x.M < ivl || x.amount <= 0) return true;
         if (round > 0 && !(W[t].win && W[t].lo <= i && i <= W[t].hi && owner[t] < 0)) return true;
+        if (keep && !(*keep)(t)) return true;
         const int32_t jd = W[t].jd, jc = W[t].jc;
         if (jd < 0 && jc < 0) return true;
         if ((jd >= 0 && x.amount > pb.d[jd]) || (jc >= 0 && x.amount > pb.d[jc])) return true;
