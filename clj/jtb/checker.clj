@@ -584,6 +584,28 @@
           (<= 0 (at (+ s 9)))   (assoc :op (by-index (at (+ s 9))))
           (<= 0 (at (+ s 10)))  (assoc :transfer-id (at (+ s 10))))))))
 
+(defn lifted-witness-checker
+  "repaired-witness-checker with lifted bans: a shard whose repairs stop because a repair recorded no new ban gets up
+  to {:max-lifts n} lift steps, each letting the failing gaps take back transfers their own bans held (once per pair)
+  before the repairs resume.  :valid? true is the same proof; a history the repaired witness proves comes back
+  unchanged.  Add it to the compose map at tests/ledger.clj:363-367 as `:lifted-witness (lifted-witness-checker {})`.
+  Result: repaired-witness-checker's map plus :lifts and :lifted-count."
+  [opts]
+  (reify checker/Checker
+    (check [_ _test history _opts]
+      (let [{:keys [arrays by-index]} (flatten-history :ledger-lookups history)
+            res (Native/checkLiftedWitness @ctx arrays (long (:max-nodes opts 0)) (int (:max-rounds opts 0))
+                                           (int (:max-repairs opts 0)) (int (:max-lifts opts 0)))
+            at  (fn [i] (aget res (int i)))
+            s   16]                                        ; shard 0: valid cause reads transfers committed ...
+        (cond-> {:valid? (verdict (at s)) :read-count (at (+ s 2)) :transfer-count (at (+ s 3))
+                 :committed-count (at (+ s 4)) :committed-crashed-count (at (+ s 5)) :after-count (at (+ s 6))
+                 :rounds (at (+ s 8)) :repairs (at (+ s 11)) :ban-count (at (+ s 12)) :lifts (at (+ s 13))
+                 :lifted-count (at (+ s 14))}
+          (pos? (at (+ s 1)))   (assoc :cause (sw-cause (at (+ s 1))))
+          (<= 0 (at (+ s 9)))   (assoc :op (by-index (at (+ s 9))))
+          (<= 0 (at (+ s 10)))  (assoc :transfer-id (at (+ s 10))))))))
+
 ;; ---- independent ----------------------------------------------------------------------------------------------
 (defn independent-checker
   "Like (independent/checker (checker/compose checkers)) for a map {name checker-kind} built from THIS namespace's

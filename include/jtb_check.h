@@ -660,6 +660,56 @@ typedef struct jtb_rw_result {
     double  seconds_total;
 } jtb_rw_result;
 
+/* ---- lifted serial witness (DESIGN.md "K15 lifted serial witness") -------------------------------------------------
+ * The repaired serial witness, then, on a shard whose repairs stopped because a repair recorded no new ban (not
+ * because max_repairs ran out), lift steps.  P^0_g is the real-time point of g's lower read from the reads alone.
+ *   - every gap the failing round did not explain steals again as in a NO_WITNESS repair, but its gather ignores the
+ *     gap's own bans (except a pair lifted before and banned again) and drops the transfers with cp(t) <= P^0_g in
+ *     place of P^_g; a thief keeps its solution when no smaller thief took one of its transfers;
+ *   - every ban (g, t) of a kept thief g that takes t is lifted, each chosen transfer it takes is banned in the gap
+ *     that had it, and the release and the loot follow as in a repair; the repair rounds then resume unchanged.
+ * A (gap, transfer) pair is lifted at most once; a lift step that lifts nothing, max_lifts lift steps, or
+ * max_repairs + max_lifts repairs (lift steps included) end the shard.  The real-time pass and the re-sum run after
+ * every repair, so a VALID is the serial-witness check's proof.  A shard the repaired serial witness proves, or leaves
+ * after max_repairs repairs, is returned as it returns it. */
+#define JTB_LW_DEFAULT_MAX_LIFTS 32
+
+typedef struct jtb_lw_shard {
+    int32_t valid;              /* JTB_VALID / JTB_UNKNOWN                                                            */
+    int32_t cause;              /* JTB_CAUSE_* when valid == JTB_UNKNOWN (of the last witness)                        */
+    int32_t n_reads;
+    int32_t n_transfers;
+    int64_t n_committed;        /* VALID: transfers committed in some gap                                             */
+    int64_t n_committed_crashed;/* VALID: of them, the crashed ones                                                   */
+    int64_t n_after;            /* VALID: :ok transfers committed after the last read                                 */
+    int64_t nodes;              /* search nodes of every witness round, steal and lift step                           */
+    int32_t rounds;             /* witness rounds that ran a gap of the shard, repairs included                       */
+    int32_t fail_index;         /* as jtb_sw_shard's, of the last witness                                             */
+    int64_t transfer_id;        /* as jtb_sw_shard's, of the last witness                                             */
+    int32_t repairs;            /* repair rounds run on the shard, lift steps included                                */
+    int32_t n_bans;             /* (gap, transfer) bans recorded, a pair banned again after its lift included        */
+    int32_t lifts;              /* lift steps that lifted a ban                                                       */
+    int32_t n_lifted;           /* (gap, transfer) bans lifted                                                        */
+} jtb_lw_shard;
+
+typedef struct jtb_lw_result {
+    int32_t valid;
+    int32_t n_failures;
+    int64_t n_reads;
+    int64_t n_transfers;
+    int64_t n_committed;
+    int64_t n_committed_crashed;
+    int64_t n_after;
+    int64_t nodes;
+    int64_t rounds;             /* the most witness rounds of any shard                                               */
+    int64_t repairs;            /* the most repair rounds of any shard                                                */
+    int64_t n_bans;
+    int64_t lifts;              /* the most lift steps of any shard                                                   */
+    int64_t n_lifted;
+    double  seconds_kernel;
+    double  seconds_total;
+} jtb_lw_result;
+
 typedef struct jtb_ctx jtb_ctx;
 
 /* ---- lifecycle -------------------------------------------------------------------------------- */
@@ -669,7 +719,7 @@ int         jtb_abi_version(void);
  * 6 jtb_setfull_out, 7 jtb_bank_result, 8 jtb_final_config, 9 jtb_mono_shard, 10 jtb_mono_result, 11 jtb_cb_shard,
  * 12 jtb_cb_result, 13 jtb_tl_shard, 14 jtb_tl_result, 15 jtb_rx_shard, 16 jtb_rx_result, 17 jtb_rg_shard,
  * 18 jtb_rg_result, 19 jtb_tp_shard, 20 jtb_tp_result, 21 jtb_sw_shard, 22 jtb_sw_result, 23 jtb_rw_shard,
- * 24 jtb_rw_result; -1 otherwise */
+ * 24 jtb_rw_result, 25 jtb_lw_shard, 26 jtb_lw_result; -1 otherwise */
 long        jtb_struct_size(int which);
 int         jtb_device_count(void);                 /* number of CUDA devices, <0 on error          */
 jtb_ctx*    jtb_create(const jtb_opts* opts);       /* NULL on failure (no CUDA device etc.)        */
@@ -776,6 +826,12 @@ int jtb_check_serial_witness(jtb_ctx* ctx, const jtb_history* h, int64_t max_nod
 int jtb_check_repaired_witness(jtb_ctx* ctx, const jtb_history* h, int64_t max_nodes, int32_t max_rounds,
                                int32_t max_repairs, int32_t flags, int32_t* commit_read, jtb_rw_shard* shards,
                                jtb_rw_result* out);
+
+/* ---- lifted serial witness (see jtb_lw_shard above) ------------------------------------------------------------ *
+ * As jtb_check_repaired_witness; max_lifts <= 0 means JTB_LW_DEFAULT_MAX_LIFTS; flags is reserved and must be 0. */
+int jtb_check_lifted_witness(jtb_ctx* ctx, const jtb_history* h, int64_t max_nodes, int32_t max_rounds,
+                             int32_t max_repairs, int32_t max_lifts, int32_t flags, int32_t* commit_read,
+                             jtb_lw_shard* shards, jtb_lw_result* out);
 
 /* ---- multi-GPU fan-out inside the library (SURVEY §8(b) `n_gpus`, §8(e)) ----------------------------------- *
  * What `independent/checker` (set_full.clj:155) does over JVM threads, done over the GPUs of one box for a host

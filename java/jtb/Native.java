@@ -161,4 +161,16 @@ public final class Native {
      */
     public static native long[] checkRepairedWitness(long ctx, Object[] history, long maxNodes, int maxRounds,
                                                      int maxRepairs);
+
+    /**
+     * {@code jtb_check_lifted_witness}: {@link #checkRepairedWitness} with up to {@code maxLifts} lift steps (<= 0: the
+     * library's default) on the shards whose repairs stop because a repair recorded no new ban.
+     *
+     * @return {@code [valid, nFailures, nReads, nTransfers, nCommitted, nCommittedCrashed, nAfter, nodes, rounds,
+     *     repairs, nBans, lifts, nLifted, kernelNs, totalNs, nShards]} followed by 15 longs per shard: {@code valid,
+     *     cause, nReads, nTransfers, nCommitted, nCommittedCrashed, nAfter, nodes, rounds, failIndex, transferId,
+     *     repairs, nBans, lifts, nLifted}
+     */
+    public static native long[] checkLiftedWitness(long ctx, Object[] history, long maxNodes, int maxRounds,
+                                                   int maxRepairs, int maxLifts);
 }

@@ -383,6 +383,31 @@ def rw_to_dict(res, shards, commit_read=None) -> dict:
     return out
 
 
+LW_DEFAULT_MAX_LIFTS = 32
+
+
+class CLwShard(C.Structure):
+    """jtb_lw_shard: the lifted-serial-witness verdict of one shard."""
+    _fields_ = CRwShard._fields_ + [("lifts", C.c_int32), ("n_lifted", C.c_int32)]
+
+
+class CLwResult(C.Structure):
+    _fields_ = CRwResult._fields_[:11] + [("lifts", C.c_int64), ("n_lifted", C.c_int64)] + CRwResult._fields_[11:]
+
+
+LW_SHARD_FIELDS = RW_SHARD_FIELDS + ("lifts", "n_lifted")
+LW_RESULT_FIELDS = RW_RESULT_FIELDS[:11] + ("lifts", "n_lifted") + RW_RESULT_FIELDS[11:]
+
+
+def lw_to_dict(res, shards, commit_read=None) -> dict:
+    """As sw_to_dict, for jtb_lw_result / jtb_lw_shard."""
+    out = {f: getattr(res, f) for f in LW_RESULT_FIELDS}
+    out["shards"] = [{f: getattr(s, f) for f in LW_SHARD_FIELDS} for s in shards]
+    if commit_read is not None:
+        out["commit_read"] = commit_read
+    return out
+
+
 def n_transfer_records(h) -> int:
     """Transfer micro-ops of a ledger-lookups history: the records of its transfer invokes."""
     import numpy as np

@@ -659,6 +659,32 @@ class RepairedWitness(SerialWitness):
         return top, [self._shard_map(s) for s in r["shards"]]
 
 
+class LiftedWitness(RepairedWitness):
+    """The repaired serial witness with lifted bans, on the GPU (K15): a shard whose repairs stop because a repair
+    recorded no new ban gets up to max-lifts lift steps, each letting the failing gaps take back transfers their own
+    bans held (once per pair) before the repairs resume; a VALID is the same proof, and a shard the repaired witness
+    proves comes back unchanged.  Result: RepairedWitness's map plus lifts and lifted-count."""
+
+    def __init__(self, checker_opts: Mapping[str, Any] | None = None, ctx: Context | None = None,
+                 **ctx_opts) -> None:
+        RepairedWitness.__init__(self, checker_opts, ctx, **ctx_opts)
+        self.max_lifts = int((checker_opts or {}).get("max-lifts", 0))
+
+    def _shard_map(self, s: dict) -> dict:
+        m = RepairedWitness._shard_map(self, s)
+        m.update({"lifts": s["lifts"], "lifted-count": s["n_lifted"]})
+        return m
+
+    def check_flat(self, test, h: FlatHistory) -> tuple[dict, list[dict]]:
+        r = self.ctx.check_lifted_witness(h, self.max_nodes, self.max_rounds, self.max_repairs, self.max_lifts)
+        top = {"valid?": VERDICT_NAME[r["valid"]], "read-count": r["n_reads"], "transfer-count": r["n_transfers"],
+               "committed-count": r["n_committed"], "committed-crashed-count": r["n_committed_crashed"],
+               "after-count": r["n_after"], "rounds": r["rounds"], "repairs": r["repairs"],
+               "ban-count": r["n_bans"], "lifts": r["lifts"], "lifted-count": r["n_lifted"], "nodes": r["nodes"],
+               "seconds-kernel": r["seconds_kernel"], "seconds-total": r["seconds_total"]}
+        return top, [self._shard_map(s) for s in r["shards"]]
+
+
 class Compose(Checker):
     """`(checker/compose {name checker ...})`: run each, `:valid?` = merge-valid of the results."""
 
@@ -790,6 +816,12 @@ def repaired_witness_checker(opts: Mapping[str, Any] | None = None, **kw) -> Rep
     """The serial-witness check with repair rounds (K14); {"max-nodes": n} and {"max-rounds": n} as for the
     serial-witness check, {"max-repairs": n} the repair rounds (default abi.RW_DEFAULT_MAX_REPAIRS)."""
     return RepairedWitness(opts, **kw)
+
+
+def lifted_witness_checker(opts: Mapping[str, Any] | None = None, **kw) -> LiftedWitness:
+    """The repaired serial witness with lift steps (K15); {"max-nodes" "max-rounds" "max-repairs"} as for the
+    repaired serial witness, {"max-lifts": n} the lift steps (default abi.LW_DEFAULT_MAX_LIFTS)."""
+    return LiftedWitness(opts, **kw)
 
 
 def compose(checkers: Mapping[str, Checker]) -> Compose:
@@ -961,16 +993,17 @@ def ledger_checker(checker_opts: Mapping[str, Any] | None = None, ctx: Context |
                    linear: bool = True, monotonic: bool = False, counter_bounds: bool = False,
                    transfer_lookups: bool = False, read_explanations: bool = False,
                    read_gaps: bool = False, transfer_placement: bool = False,
-                   serial_witness: bool = False, repaired_witness: bool = False) -> Compose:
+                   serial_witness: bool = False, repaired_witness: bool = False,
+                   lifted_witness: bool = False) -> Compose:
     """The ledger test's checker (tests/ledger.clj:363-367) minus the gnuplot plotter, plus the
     linearizability search the north-star adds and, with monotonic=True, the monotonic-key check, with
     counter_bounds=True, the counter-bounds check, with transfer_lookups=True, the transfer-lookup check, with
     read_explanations=True, the read-explanation check, with read_gaps=True, the read-gap check, with
-    transfer_placement=True, the transfer-placement check, with serial_witness=True, the serial-witness check and,
-    with repaired_witness=True, the repaired serial witness:
+    transfer_placement=True, the transfer-placement check, with serial_witness=True, the serial-witness check, with
+    repaired_witness=True, the repaired serial witness and, with lifted_witness=True, the lifted serial witness:
         {:SI (checker opts) :lookup-transfers ... :final-reads ... :unexpected-ops ... [:linear ...] [:monotonic ...]
          [:counter-bounds ...] [:transfer-lookups ...] [:read-explanations ...] [:read-gaps ...]
-         [:transfer-placement ...] [:serial-witness ...] [:repaired-witness ...]}"""
+         [:transfer-placement ...] [:serial-witness ...] [:repaired-witness ...] [:lifted-witness ...]}"""
     cs: dict[str, Checker] = {"SI": bank_checker(checker_opts, ctx=ctx),
                               "lookup-transfers": lookup_all_invoked_transfers(),
                               "final-reads": final_reads(), "unexpected-ops": unexpected_ops()}
@@ -992,4 +1025,6 @@ def ledger_checker(checker_opts: Mapping[str, Any] | None = None, ctx: Context |
         cs["serial-witness"] = serial_witness_checker(ctx=ctx)
     if repaired_witness:
         cs["repaired-witness"] = repaired_witness_checker(ctx=ctx)
+    if lifted_witness:
+        cs["lifted-witness"] = lifted_witness_checker(ctx=ctx)
     return compose(cs)

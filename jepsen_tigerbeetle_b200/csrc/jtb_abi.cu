@@ -25,6 +25,7 @@
 #include "jtb_transfer_placement.cuh"
 #include "jtb_serial_witness.cuh"
 #include "jtb_repaired_witness.cuh"
+#include "jtb_lifted_witness.cuh"
 
 using namespace jtb;
 
@@ -744,6 +745,8 @@ long jtb_struct_size(int which) {
     case 22: return sizeof(jtb_sw_result);
     case 23: return sizeof(jtb_rw_shard);
     case 24: return sizeof(jtb_rw_result);
+    case 25: return sizeof(jtb_lw_shard);
+    case 26: return sizeof(jtb_lw_result);
     }
     return -1;
 }
@@ -1197,6 +1200,18 @@ int jtb_check_repaired_witness(jtb_ctx* ctx, const jtb_history* h, int64_t max_n
     ctx->fc.valid = false;
     return run_repaired_witness(ctx->stream, ctx->ev0, ctx->ev1, h, max_nodes, max_rounds, max_repairs, flags,
                                 commit_read, shards, out, ctx->err);
+}
+
+// K15: the lifted serial witness (csrc/jtb_lifted_witness.cuh)
+int jtb_check_lifted_witness(jtb_ctx* ctx, const jtb_history* h, int64_t max_nodes, int32_t max_rounds,
+                             int32_t max_repairs, int32_t max_lifts, int32_t flags, int32_t* commit_read,
+                             jtb_lw_shard* shards, jtb_lw_result* out) {
+    if (!ctx) return -1;
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    if (cudaSetDevice(ctx->device) != cudaSuccess) { ctx->err = "cudaSetDevice failed"; return -1; }
+    ctx->fc.valid = false;
+    return run_lifted_witness(ctx->stream, ctx->ev0, ctx->ev1, h, max_nodes, max_rounds, max_repairs, max_lifts, flags,
+                              commit_read, shards, out, ctx->err);
 }
 
 // SURVEY 8(f) N2: the step before the checkers (independent/subhistory, ledger->bank) on the device

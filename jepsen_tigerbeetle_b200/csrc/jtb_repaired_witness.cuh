@@ -261,301 +261,6 @@ __global__ void rw_count(int32_t m, SwDev w) {
 }
 
 // ---- host ---------------------------------------------------------------------------------------------------------
-
-inline int run_repaired_witness(cudaStream_t st, cudaEvent_t ev0, cudaEvent_t ev1, const jtb_history* h,
-                                int64_t max_nodes, int32_t max_rounds, int32_t max_repairs, int32_t flags,
-                                int32_t* commit_read, jtb_rw_shard* shards, jtb_rw_result* out, std::string& err) {
-    const auto t0 = std::chrono::steady_clock::now();
-    if (!h || !shards || !out) { err = "null argument"; return -2; }
-    if (max_rounds <= 0) max_rounds = JTB_TP_DEFAULT_MAX_ROUNDS;
-    if (max_repairs <= 0) max_repairs = JTB_RW_DEFAULT_MAX_REPAIRS;
-    TpStage g;
-    if (int rc = tp_stage(st, ev0, h, max_nodes, max_rounds, flags, g, err)) return rc;
-    const int32_t S = g.S, nT = g.nT, m = g.m;
-    std::vector<jtb_tp_shard> tp(std::max(S, 1));
-    float ms = 0;
-    if (int rc = tp_finals(st, ev0, ev1, h, g, tp.data(), ms, err)) return rc;
-    const TlHost& T = g.T;
-    std::vector<uint8_t> sok(S, 0);
-    bool any = false;
-    for (int32_t s = 0; s < S; ++s) {
-        jtb_rw_shard& o = shards[s];
-        memset(&o, 0, sizeof o);
-        o.valid = JTB_VALID;
-        o.n_reads = tp[s].n_reads;
-        o.n_transfers = tp[s].n_transfers;
-        o.fail_index = -1;
-        o.transfer_id = -1;
-        if (tp[s].valid != JTB_VALID) {
-            o.valid = JTB_UNKNOWN;
-            o.cause = tp[s].cause ? tp[s].cause : tp[s].valid == JTB_INVALID ? JTB_CAUSE_ANOMALY : JTB_CAUSE_UNDECIDED;
-        }
-        any |= (sok[s] = g.dev[s] && o.valid == JTB_VALID);
-    }
-    std::vector<int32_t> cr_h(nT, JTB_SW_NEVER);
-    if (m > 0 && any) {
-        CallAllocs& A = g.A;
-        RgDev& x = g.x;
-        TpDev& p = g.p;
-        SwDev w;
-        RwDev r;
-        w.t_okcomp = g.d.t_okcomp;
-        std::vector<int32_t> rd_cidx(m);
-        for (int32_t i = 0; i < m; ++i) rd_cidx[i] = h->index[g.H.r_ev[g.d_of[i]]];
-        const int32_t* d_cidx;
-        int32_t *d_cr, *kowner, *Ph, *gmaxh, *fcause, *stot, *reps, *bans, *nbs, *after, *rkey, *ry, *rsm, *words;
-        uint8_t *sact, *svalid, *fprev, *failing, *thief, *rel, *stmp;
-        unsigned long long *fkey, *fid;
-        JTB_OK(A.put(&w.sok, sok, st)); JTB_OK(A.put(&d_cidx, rd_cidx, st));
-        JTB_OK(A.alloc(&sact, S)); JTB_OK(A.alloc(&svalid, S));
-        JTB_OK(cudaMemcpyAsync(sact, w.sok, S, cudaMemcpyDeviceToDevice, st));
-        JTB_OK(A.alloc(&w.fixed, m)); JTB_OK(A.alloc(&w.cmin, nT)); JTB_OK(A.alloc(&w.sfail, S));
-        JTB_OK(A.alloc(&w.sunf, S)); JTB_OK(A.alloc(&w.unfixed, 1)); JTB_OK(A.alloc(&w.cnt, (size_t)S * SW_COUNTERS));
-        JTB_OK(A.alloc(&w.gmax, m)); JTB_OK(A.alloc(&w.gmin, m)); JTB_OK(A.alloc(&w.skey, m));
-        JTB_OK(A.alloc(&w.x, m)); JTB_OK(A.alloc(&w.P, m)); JTB_OK(A.alloc(&w.rtkey, S)); JTB_OK(A.alloc(&w.rtid, S));
-        JTB_OK(A.alloc(&w.bad, 1)); JTB_OK(A.alloc(&d_cr, nT));
-        JTB_OK(A.alloc(&kowner, nT)); JTB_OK(A.alloc(&Ph, m)); JTB_OK(A.alloc(&gmaxh, m));
-        JTB_OK(A.alloc(&fcause, S)); JTB_OK(A.alloc(&fkey, S)); JTB_OK(A.alloc(&fid, S)); JTB_OK(A.alloc(&stot, S));
-        JTB_OK(A.alloc(&reps, S)); JTB_OK(A.alloc(&bans, S)); JTB_OK(A.alloc(&nbs, S)); JTB_OK(A.alloc(&after, S));
-        JTB_OK(A.alloc(&rkey, m)); JTB_OK(A.alloc(&ry, m)); JTB_OK(A.alloc(&rsm, m)); JTB_OK(A.alloc(&words, 2));
-        JTB_OK(A.alloc(&fprev, m)); JTB_OK(A.alloc(&failing, m)); JTB_OK(A.alloc(&thief, m)); JTB_OK(A.alloc(&rel, m));
-        int64_t* kown;
-        JTB_OK(A.alloc(&kown, std::max<int64_t>(g.cells, 1)));
-        // the bans: [0, n_ban) sorted in ban[0]; a repair appends at n_ban, then the whole list is sorted into ban[1]
-        int64_t ban_cap = std::max<int64_t>(2 * (int64_t)nT, 16);
-        unsigned long long* ban[2];
-        JTB_OK(A.alloc(&ban[0], ban_cap)); JTB_OK(A.alloc(&ban[1], ban_cap));
-        size_t stmp_bytes = 0, sort_bytes = 0;
-        JTB_OK(cub::DeviceScan::InclusiveScanByKey(nullptr, stmp_bytes, w.skey, w.x, w.P, MaxOp{}, m,
-                                                   cuda::std::equal_to<>{}, st));
-        JTB_OK(A.alloc(&stmp, stmp_bytes));
-        uint8_t* sort_tmp = nullptr;
-        auto grid = [](int64_t n, int per) { return (unsigned)((n + per - 1) / per); };
-        JTB_OK(cudaMemsetAsync(w.sfail, 0x7f, (size_t)S * 4, st));   // RG_NONE
-        JTB_OK(cudaMemsetAsync(w.sunf, 0x7f, (size_t)S * 4, st));
-        JTB_OK(cudaMemsetAsync(w.cnt, 0, (size_t)S * SW_COUNTERS * 8, st));
-        JTB_OK(cudaMemsetAsync(w.unfixed, 0, 4, st));
-        JTB_OK(cudaMemsetAsync(svalid, 0, S, st));
-        JTB_OK(cudaMemsetAsync(fcause, 0, (size_t)S * 4, st));
-        JTB_OK(cudaMemsetAsync(stot, 0, (size_t)S * 4, st));
-        JTB_OK(cudaMemsetAsync(reps, 0, (size_t)S * 4, st));
-        JTB_OK(cudaMemsetAsync(bans, 0, (size_t)S * 4, st));
-        JTB_OK(cudaMemsetAsync(nbs, 0, (size_t)S * 4, st));
-        JTB_OK(cudaMemsetAsync(thief, 0, m, st));
-        JTB_OK(cudaMemsetAsync(rel, 0, m, st));
-        JTB_OK(cudaMemcpyAsync(kowner, p.owner, (size_t)nT * 4, cudaMemcpyDeviceToDevice, st));
-        JTB_OK(cudaMemcpyAsync(kown, g.own, (size_t)g.cells * 8, cudaMemcpyDeviceToDevice, st));
-        r.kowner = kowner;
-        r.Ph = Ph;
-        r.sact = sact;
-        sw_init<<<grid(m, 256), 256, 0, st>>>(x, p, w);
-        w.sok = sact;   // from here on the kernels see the shards still repairing
-        int32_t n_ban = 0;
-        int32_t* d_nban = words + 1;
-        JTB_OK(cudaMemsetAsync(words, 0, 8, st));
-        for (int32_t rep = 0;; ++rep) {
-            // the witness rounds
-            int32_t unfixed = 0;
-            JTB_OK(cudaMemsetAsync(p.srounds, 0, (size_t)S * 4, st));
-            if (rep > 0) {
-                JTB_OK(cudaMemsetAsync(w.unfixed, 0, 4, st));
-                rw_count<<<grid(m, 256), 256, 0, st>>>(m, w);
-            }
-            JTB_OK(cudaMemcpyAsync(&unfixed, w.unfixed, 4, cudaMemcpyDeviceToHost, st));
-            JTB_OK(cudaStreamSynchronize(st));
-            for (int32_t rd = 0; unfixed > 0 && rd < max_rounds; ++rd) {
-                JTB_OK(cudaMemsetAsync(w.cmin, 0x7f, (size_t)nT * 4, st));
-                JTB_OK(cudaMemsetAsync(w.unfixed, 0, 4, st));
-                rw_snap<<<grid(m, 256), 256, 0, st>>>(m, x, w, fprev);
-                w.round = rd;
-                if (rep == 0) {
-                    sw_gaps<<<grid(m, RG_WARPS), RG_WARPS * 32, 0, st>>>(x, p, w);
-                } else {
-                    // P^ from the reads and the owned transfers
-                    JTB_OK(cudaMemsetAsync(gmaxh, 0x80, (size_t)m * 4, st));
-                    if (nT > 0) rw_gmax<<<grid(nT, 256), 256, 0, st>>>(p, r, gmaxh);
-                    SwDev wh = w;
-                    wh.gmax = gmaxh;
-                    sw_scan_in<<<grid(m, 256), 256, 0, st>>>(x, wh);
-                    size_t tb = stmp_bytes;
-                    JTB_OK(cub::DeviceScan::InclusiveScanByKey(stmp, tb, w.skey, w.x, Ph, MaxOp{}, m,
-                                                               cuda::std::equal_to<>{}, st));
-                    rw_gaps<<<grid(m, RG_WARPS), RG_WARPS * 32, 0, st>>>(x, p, w, r);
-                }
-                sw_fix<<<grid(m, 256), 256, 0, st>>>(m, x, p, w);
-                JTB_OK(cudaGetLastError());
-                JTB_OK(cudaMemcpyAsync(&unfixed, w.unfixed, 4, cudaMemcpyDeviceToHost, st));
-                JTB_OK(cudaStreamSynchronize(st));
-            }
-            if (unfixed > 0) sw_unfixed<<<grid(m, 256), 256, 0, st>>>(m, x, w);
-            // real time and the counters
-            JTB_OK(cudaMemsetAsync(w.gmax, 0x80, (size_t)m * 4, st));   // INT_MIN
-            JTB_OK(cudaMemsetAsync(w.gmin, 0x7f, (size_t)m * 4, st));   // > every position
-            JTB_OK(cudaMemsetAsync(w.rtkey, 0xff, (size_t)S * 8, st));
-            JTB_OK(cudaMemsetAsync(w.rtid, 0xff, (size_t)S * 8, st));
-            JTB_OK(cudaMemsetAsync(w.bad, 0, 4, st));
-            JTB_OK(cudaMemsetAsync(g.own, 0, (size_t)g.cells * 8, st));
-            if (nT > 0) sw_tgap<<<grid(nT, 256), 256, 0, st>>>(x, p, w);
-            sw_scan_in<<<grid(m, 256), 256, 0, st>>>(x, w);
-            size_t tb = stmp_bytes;
-            JTB_OK(cub::DeviceScan::InclusiveScanByKey(stmp, tb, w.skey, w.x, w.P, MaxOp{}, m, cuda::std::equal_to<>{},
-                                                       st));
-            sw_rt<<<grid(m, 256), 256, 0, st>>>(x, p, w);
-            sw_sum<<<grid((int64_t)m * 32, 256), 256, 0, st>>>(x, p, w);
-            if (nT > 0) {
-                sw_after<<<grid(nT, 256), 256, 0, st>>>(x, p, w);
-                sw_rt_id<<<grid(nT, 256), 256, 0, st>>>(x, p, w);
-            }
-            JTB_OK(cudaMemsetAsync(words, 0, 4, st));
-            rw_verdict<<<grid(S, 256), 256, 0, st>>>(S, w, sact, svalid, fcause, fkey, fid, stot, p.srounds, words);
-            JTB_OK(cudaGetLastError());
-            int32_t hw[2] = {0, 0};
-            unsigned int bad = 0;
-            JTB_OK(cudaMemcpyAsync(hw, words, 8, cudaMemcpyDeviceToHost, st));
-            JTB_OK(cudaMemcpyAsync(&bad, w.bad, 4, cudaMemcpyDeviceToHost, st));
-            JTB_OK(cudaStreamSynchronize(st));
-            if (bad) { err = "the counters of a serial witness do not add up"; return -1; }
-            if (hw[0] == 0 || rep >= max_repairs) break;
-            // the blame
-            if (n_ban + (int64_t)nT > ban_cap) {
-                const int64_t cap = std::max<int64_t>(2 * ban_cap, n_ban + (int64_t)nT);
-                unsigned long long *b0, *b1;
-                JTB_OK(A.alloc(&b0, cap)); JTB_OK(A.alloc(&b1, cap));
-                JTB_OK(cudaMemcpyAsync(b0, ban[0], (size_t)n_ban * 8, cudaMemcpyDeviceToDevice, st));
-                ban[0] = b0;
-                ban[1] = b1;
-                ban_cap = cap;
-            }
-            r.ban = ban[0];
-            r.n_ban = n_ban;
-            JTB_OK(cudaMemcpyAsync(g.own, kown, (size_t)g.cells * 8, cudaMemcpyDeviceToDevice, st));
-            // P^ for the steals
-            JTB_OK(cudaMemsetAsync(gmaxh, 0x80, (size_t)m * 4, st));
-            if (nT > 0) rw_gmax<<<grid(nT, 256), 256, 0, st>>>(p, r, gmaxh);
-            {
-                SwDev wh = w;
-                wh.gmax = gmaxh;
-                sw_scan_in<<<grid(m, 256), 256, 0, st>>>(x, wh);
-                size_t tb2 = stmp_bytes;
-                JTB_OK(cub::DeviceScan::InclusiveScanByKey(stmp, tb2, w.skey, w.x, Ph, MaxOp{}, m,
-                                                           cuda::std::equal_to<>{}, st));
-            }
-            // NO_WITNESS: the steals
-            rw_failing<<<grid(m, 256), 256, 0, st>>>(m, x, p, w, sact, fcause, fprev, failing);
-            JTB_OK(cudaMemsetAsync(w.cmin, 0x7f, (size_t)nT * 4, st));
-            rw_steal<<<grid(m, RG_WARPS), RG_WARPS * 32, 0, st>>>(x, p, w, r, failing, thief, rel);
-            rw_take<<<grid(m, 256), 256, 0, st>>>(m, x, p, w, r, thief, ban[0], d_nban, nbs, rel);
-            // REAL_TIME: SM by a min-scan over the reversed positions, then the bans
-            JTB_OK(cudaMemsetAsync(after, 0x7f, (size_t)S * 4, st));
-            if (nT > 0) rw_after_min<<<grid(nT, 256), 256, 0, st>>>(p, w, r, fcause, after);
-            rw_sm_in<<<grid(m, 256), 256, 0, st>>>(x, p, w, after, rkey, ry);
-            tb = stmp_bytes;
-            JTB_OK(cub::DeviceScan::InclusiveScanByKey(stmp, tb, rkey, ry, rsm, MinOp{}, m, cuda::std::equal_to<>{},
-                                                       st));
-            if (nT > 0) rw_rt_blame<<<grid(nT, 256), 256, 0, st>>>(x, p, w, r, fcause, rsm, ban[0], d_nban, nbs, rel);
-            rw_shard<<<grid(S, 256), 256, 0, st>>>(S, sact, nbs, reps, bans);
-            JTB_OK(cudaGetLastError());
-            int32_t total = 0;
-            JTB_OK(cudaMemcpyAsync(&total, d_nban, 4, cudaMemcpyDeviceToHost, st));
-            JTB_OK(cudaStreamSynchronize(st));
-            if (total == n_ban) break;
-            n_ban = total;
-            size_t need = 0;
-            JTB_OK(cub::DeviceRadixSort::SortKeys(nullptr, need, ban[0], ban[1], n_ban, 0, 64, st));
-            if (need > sort_bytes) {
-                JTB_OK(A.alloc(&sort_tmp, need));
-                sort_bytes = need;
-            }
-            JTB_OK(cub::DeviceRadixSort::SortKeys(sort_tmp, need, ban[0], ban[1], n_ban, 0, 64, st));
-            std::swap(ban[0], ban[1]);
-            r.ban = ban[0];
-            r.n_ban = n_ban;
-            // the release, and the thieves take their loot
-            rw_release_g<<<grid(m, 256), 256, 0, st>>>(m, x, w, sact, rel);
-            if (nT > 0) rw_release_t<<<grid(nT, 256), 256, 0, st>>>(p, r, rel);
-            rw_loot<<<grid(m, 256), 256, 0, st>>>(m, x, p, w, sact, thief, rel);
-            rw_reset<<<grid(S, 256), 256, 0, st>>>(S, w, sact);
-            JTB_OK(cudaGetLastError());
-        }
-        // commit_read of the proved shards
-        w.sok = svalid;
-        if (nT > 0) sw_commit<<<grid(nT, 256), 256, 0, st>>>(x, p, w, d_cidx, d_cr);
-        JTB_OK(cudaGetLastError());
-        JTB_OK(cudaEventRecord(ev1, st));
-        std::vector<unsigned long long> cnt_h((size_t)S * SW_COUNTERS), fkey_h(S), fid_h(S);
-        std::vector<int32_t> fcause_h(S), stot_h(S), reps_h(S), bans_h(S);
-        std::vector<uint8_t> svalid_h(S);
-        JTB_OK(cudaMemcpyAsync(cnt_h.data(), w.cnt, cnt_h.size() * 8, cudaMemcpyDeviceToHost, st));
-        JTB_OK(cudaMemcpyAsync(fkey_h.data(), fkey, (size_t)S * 8, cudaMemcpyDeviceToHost, st));
-        JTB_OK(cudaMemcpyAsync(fid_h.data(), fid, (size_t)S * 8, cudaMemcpyDeviceToHost, st));
-        JTB_OK(cudaMemcpyAsync(fcause_h.data(), fcause, (size_t)S * 4, cudaMemcpyDeviceToHost, st));
-        JTB_OK(cudaMemcpyAsync(stot_h.data(), stot, (size_t)S * 4, cudaMemcpyDeviceToHost, st));
-        JTB_OK(cudaMemcpyAsync(reps_h.data(), reps, (size_t)S * 4, cudaMemcpyDeviceToHost, st));
-        JTB_OK(cudaMemcpyAsync(bans_h.data(), bans, (size_t)S * 4, cudaMemcpyDeviceToHost, st));
-        JTB_OK(cudaMemcpyAsync(svalid_h.data(), svalid, S, cudaMemcpyDeviceToHost, st));
-        if (nT > 0) JTB_OK(cudaMemcpyAsync(cr_h.data(), d_cr, (size_t)nT * 4, cudaMemcpyDeviceToHost, st));
-        JTB_OK(cudaStreamSynchronize(st));
-        JTB_OK(cudaEventElapsedTime(&ms, ev0, ev1));
-        auto index_at = [&](int32_t at) -> int32_t {   // completion :index of the read at a sorted position
-            int32_t rr;
-            if (cudaMemcpy(&rr, x.ord + at, 4, cudaMemcpyDeviceToHost) != cudaSuccess) return INT_MIN;
-            return rd_cidx[rr];
-        };
-        for (int32_t s = 0; s < S; ++s) {
-            if (!sok[s]) continue;
-            jtb_rw_shard& o = shards[s];
-            const unsigned long long* c = &cnt_h[(size_t)s * SW_COUNTERS];
-            o.nodes = (int64_t)c[3];
-            o.rounds = stot_h[s];
-            o.repairs = reps_h[s];
-            o.n_bans = bans_h[s];
-            if (svalid_h[s]) {
-                o.n_committed = (int64_t)c[0];
-                o.n_committed_crashed = (int64_t)c[1];
-                o.n_after = (int64_t)c[2];
-                continue;
-            }
-            o.valid = JTB_UNKNOWN;
-            o.cause = fcause_h[s];
-            if (o.cause == JTB_CAUSE_NO_WITNESS) {
-                o.fail_index = index_at((int32_t)fkey_h[s]);
-            } else {
-                const int32_t at = (int32_t)(fkey_h[s] >> 1);
-                if (fkey_h[s] & 1) {
-                    o.fail_index = index_at(at);
-                } else {
-                    o.transfer_id = (int64_t)(fid_h[s] ^ 0x8000000000000000ull);
-                    int32_t t = T.t_off[s];
-                    while (T.t_id[t] != o.transfer_id) ++t;
-                    o.fail_index = T.t_cidx[t];
-                }
-            }
-            if (o.fail_index == INT_MIN) { err = "cudaMemcpy of a failing read failed"; return -1; }
-        }
-    }
-    // commit_read: the shards with no reads commit their :ok transfers freely; a shard that is not VALID commits none
-    for (int32_t s = 0; s < S; ++s) {
-        const bool free_ = shards[s].valid == JTB_VALID && g.H.n_reads[s] == 0;
-        if (shards[s].valid == JTB_VALID && !free_) continue;
-        for (int32_t t = T.t_off[s]; t < T.t_off[s + 1]; ++t)
-            cr_h[t] = free_ && T.t_fate[t] == JTB_T_OK ? JTB_SW_FREE : JTB_SW_NEVER;
-    }
-    if (commit_read && nT > 0) memcpy(commit_read, cr_h.data(), (size_t)nT * 4);
-    memset(out, 0, sizeof *out);
-    for (int32_t s = 0; s < S; ++s) {
-        const jtb_rw_shard& o = shards[s];
-        out->n_reads += o.n_reads;
-        out->n_transfers += o.n_transfers;
-        out->n_committed += o.n_committed;
-        out->n_committed_crashed += o.n_committed_crashed;
-        out->n_after += o.n_after;
-        out->nodes += o.nodes;
-        out->rounds = std::max(out->rounds, (int64_t)o.rounds);
-        out->repairs = std::max(out->repairs, (int64_t)o.repairs);
-        out->n_bans += o.n_bans;
-    }
-    roll_up(out, shards, S, ms, t0);
-    return 0;
-}
+// The repair loop on the host is run_repairs in jtb_lifted_witness.cuh, which K14 runs with no lift steps.
 
 }  // namespace jtb

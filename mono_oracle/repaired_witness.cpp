@@ -6,132 +6,15 @@
 // max_repairs repair rounds: the blame of the failure as (gap, transfer) bans, the release of the blamed gaps and the
 // failing one, the witness rounds again with banned pairs and transfers that complete by P^_g (the point of g's lower
 // read from the reads and the owned transfers, recomputed every round) out of the gather, then the unchanged re-sum
-// and real-time pass.  Node counts, rounds, repairs and bans are the library's.
-#include <chrono>
-#include <cstring>
-#include <set>
-
-#include "witness_common.h"
+// and real-time pass.  Node counts, rounds, repairs and bans are the library's.  The loop is repair_common.h's, with
+// no lift steps.
+#include "repair_common.h"
 
 namespace {
 
 constexpr int RW_SEARCH = 1;
 
-struct RwOut {
-    jtb_rw_shard o;
-    std::vector<int32_t> commit;   // per transfer of the shard
-};
-
-int repaired(const Shard& S, const std::vector<int32_t>& keys, const std::vector<int32_t>& ord, TpState& T,
-             int64_t max_nodes, int32_t max_rounds, int32_t max_repairs, RwOut& w) {
-    jtb_rw_shard& o = w.o;
-    Witness x(S, keys, ord, T);
-    const int32_t n = x.n, nT = x.nT;
-    std::vector<int32_t>& owner = T.owner;
-    std::set<std::pair<int32_t, int32_t>> bans;   // (gap, transfer)
-    std::vector<int32_t> Ph(n);                   // P^ at each position
-    auto hat = [&]() {
-        std::vector<int32_t> gmax(n, INT_MIN);
-        for (int32_t t = 0; t < nT; ++t)
-            if (owner[t] >= 0) gmax[owner[t]] = std::max(gmax[owner[t]], S.T[t].inv);
-        for (int32_t i = 0; i < n; ++i) Ph[i] = std::max({i > 0 ? Ph[i - 1] : INT_MIN, x.upper(i).inv, gmax[i]});
-    };
-    auto keep = [&](int32_t t, int32_t i) { return !bans.count({i, t}) && !(i > 0 && S.T[t].okcomp <= Ph[i - 1]); };
-    for (int32_t rep = 0;; ++rep) {
-        int32_t rounds = 0;
-        const int32_t failed = rep ? x.rounds(max_nodes, max_rounds, hat, keep, rounds, o.nodes)
-                                   : x.rounds(max_nodes, max_rounds, {}, {}, rounds, o.nodes);
-        o.rounds += rounds;
-        o.valid = JTB_VALID;
-        o.cause = 0;
-        o.fail_index = -1;
-        o.transfer_id = -1;
-        if (failed >= 0) {
-            o.valid = JTB_UNKNOWN;
-            o.cause = JTB_CAUSE_NO_WITNESS;
-            o.fail_index = x.upper(failed).comp_index;
-        } else {
-            if (!x.check()) {
-                g_err = "the counters of a serial witness do not add up";
-                return -1;
-            }
-            x.verdict(o, w.commit);
-            if (o.valid == JTB_VALID) return 0;
-        }
-        if (rep >= max_repairs) return 0;
-        // the blame: new bans, and the gaps they release
-        std::vector<std::pair<int32_t, int32_t>> nb;
-        std::vector<char> rel(n, 0);
-        std::vector<std::vector<int32_t>> loot(n);
-        std::vector<char> thief(n, 0);
-        hat();
-        if (failed >= 0) {
-            // the steals (Jacobi): every failing gap g searches the free and the chosen transfers its gather takes
-            // (not banned in g, cp(t) > P^_g); a thief keeps its solution when no smaller thief took one of them
-            std::vector<int32_t> free_(owner), cmin(nT, INT_MAX);
-            for (int32_t t = 0; t < nT; ++t)
-                if (x.chosen_t(t)) free_[t] = -1;
-            for (int32_t g : x.failing) {
-                rel[g] = 1;
-                const std::function<bool(int32_t)> k = [&](int32_t t) { return keep(t, g); };
-                Problem pb;
-                if (!x.gather(g, free_, &k, pb)) continue;
-                Search sr(pb, -1, max_nodes);
-                int32_t root_key, kept;
-                std::vector<uint8_t> sol;
-                const bool ok = sr.run(root_key, kept, nullptr, nullptr, &sol) == EXPLAINED;
-                o.nodes += sr.nodes;
-                if (!ok) continue;
-                thief[g] = 1;
-                for (size_t c = 0; c < pb.P.size(); ++c)
-                    if (sol[c] == IN) {
-                        loot[g].push_back(pb.P[c].t);
-                        cmin[pb.P[c].t] = std::min(cmin[pb.P[c].t], g);
-                    }
-            }
-            for (int32_t g : x.failing) {
-                for (int32_t t : loot[g]) thief[g] &= cmin[t] == g;
-                if (thief[g])
-                    for (int32_t t : loot[g])
-                        if (x.chosen_t(t)) nb.push_back({owner[t], t});
-            }
-        } else {
-            // real time: every chosen transfer of D_g that completes by P_g, and every chosen transfer of a gap h
-            // invoked at or after SM[h], the smallest completion of what must follow it (the reads from r_h on, D_g
-            // for g > h, the failing :ok transfers after the last read)
-            int32_t after = INT_MAX;
-            for (int32_t t = 0; t < nT; ++t)
-                if (x.after_fails(t)) after = std::min(after, S.T[t].okcomp);
-            std::vector<int32_t> SM(n + 1);
-            SM[n] = after;
-            for (int32_t i = n - 1; i >= 0; --i)
-                SM[i] = std::min({SM[i + 1], x.upper(i).comp, i + 1 < n ? x.gmin[i + 1] : INT_MAX});
-            for (int32_t t = 0; t < nT; ++t) {
-                if (!x.chosen_t(t)) continue;
-                const int32_t g = owner[t];
-                if ((g > 0 && S.T[t].okcomp <= x.Q[g - 1]) || S.T[t].inv >= SM[g]) nb.push_back({g, t});
-            }
-        }
-        bool any = false;
-        for (auto& p : nb)
-            if (bans.insert(p).second) {
-                any = true;
-                rel[p.first] = 1;
-            }
-        if (!any) return 0;
-        o.repairs = rep + 1;
-        o.n_bans = (int32_t)bans.size();
-        for (int32_t i = 0; i < n; ++i)
-            if (rel[i]) x.fixed[i] = 0;
-        for (int32_t t = 0; t < nT; ++t)
-            if (x.chosen_t(t) && rel[owner[t]]) owner[t] = -1;
-        for (int32_t g = 0; g < n; ++g)
-            if (thief[g]) {
-                x.fixed[g] = 1;
-                for (int32_t t : loot[g]) owner[t] = g;
-            }
-    }
-}
+void roll_rw(jtb_rw_result*, const jtb_rw_shard&) {}
 
 }  // namespace
 
@@ -142,81 +25,9 @@ const char* jtbm_rw_last_error(void) { return g_err.c_str(); }
 int jtbm_check_repaired_witness(const jtb_history* h, int64_t max_nodes, int32_t max_rounds, int32_t max_repairs,
                                 int32_t flags, int32_t algo, int32_t* commit_read, jtb_rw_shard* shards,
                                 jtb_rw_result* out) {
-    const auto t0 = std::chrono::steady_clock::now();
     if (flags != 0) { g_err = "flags must be 0 (reserved)"; return -2; }
     if (algo != RW_SEARCH) { g_err = "unknown algorithm"; return -2; }
-    if (max_nodes <= 0) max_nodes = JTB_TP_DEFAULT_MAX_NODES;
-    if (max_rounds <= 0) max_rounds = JTB_TP_DEFAULT_MAX_ROUNDS;
-    if (max_repairs <= 0) max_repairs = JTB_RW_DEFAULT_MAX_REPAIRS;
-    memset(out, 0, sizeof *out);
-    int64_t n_records = 0, n_reads = 0;
-    std::vector<RwOut> tmp(h->n_shards);
-    try {
-        for (int32_t s = 0; s < h->n_shards; ++s) {
-            Shard S;
-            if (int rc = parse_shard(h, s, S, n_records)) return rc;
-            n_reads += (int64_t)S.R.size();
-            if (n_reads > INT_MAX) { g_err = "more than 2^31-1 reads"; return -2; }
-            classify_inputs(S);
-            RwOut& w = tmp[s];
-            jtb_rw_shard& o = w.o;
-            memset(&o, 0, sizeof o);
-            o.valid = JTB_VALID;
-            o.n_reads = (int32_t)S.R.size();
-            o.n_transfers = (int32_t)S.T.size();
-            o.fail_index = -1;
-            o.transfer_id = -1;
-            w.commit.assign(S.T.size(), JTB_SW_NEVER);
-            std::vector<int32_t> keys, ord;
-            bool partial;
-            shard_order(S, keys, partial, ord);
-            if (partial) {
-                o.valid = JTB_UNKNOWN;
-                o.cause = JTB_CAUSE_PARTIAL_READ;
-                continue;
-            }
-            if (S.R.empty()) {
-                for (size_t t = 0; t < S.T.size(); ++t)
-                    if (S.T[t].fate == JTB_T_OK) w.commit[t] = JTB_SW_FREE;
-                continue;
-            }
-            jtb_tp_shard p;
-            memset(&p, 0, sizeof p);
-            TpState T;
-            tp_search(h, s, S, keys, ord, max_nodes, max_rounds, p, T);
-            if (p.valid != JTB_VALID) {
-                o.valid = JTB_UNKNOWN;
-                o.cause = p.valid == JTB_INVALID ? JTB_CAUSE_ANOMALY : JTB_CAUSE_UNDECIDED;
-                continue;
-            }
-            if (int rc = repaired(S, keys, ord, T, max_nodes, max_rounds, max_repairs, w)) return rc;
-            if (o.valid != JTB_VALID) {
-                o.n_committed = o.n_committed_crashed = o.n_after = 0;
-                std::fill(w.commit.begin(), w.commit.end(), JTB_SW_NEVER);
-            }
-        }
-    } catch (int) {
-        return -2;
-    }
-    int64_t at = 0;
-    for (int32_t s = 0; s < h->n_shards; ++s) {
-        const jtb_rw_shard& o = shards[s] = tmp[s].o;
-        if (commit_read) std::copy(tmp[s].commit.begin(), tmp[s].commit.end(), commit_read + at);
-        at += (int64_t)tmp[s].commit.size();
-        out->n_reads += o.n_reads;
-        out->n_transfers += o.n_transfers;
-        out->n_committed += o.n_committed;
-        out->n_committed_crashed += o.n_committed_crashed;
-        out->n_after += o.n_after;
-        out->nodes += o.nodes;
-        out->rounds = std::max(out->rounds, (int64_t)o.rounds);
-        out->repairs = std::max(out->repairs, (int64_t)o.repairs);
-        out->n_bans += o.n_bans;
-        out->valid = std::max(out->valid, o.valid);
-        if (o.valid != JTB_VALID) out->n_failures++;
-    }
-    out->seconds_total = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
-    return 0;
+    return repaired_check(h, max_nodes, max_rounds, max_repairs, 0, commit_read, shards, out, roll_rw);
 }
 
 }  // extern "C"
