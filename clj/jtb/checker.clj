@@ -606,6 +606,30 @@
           (<= 0 (at (+ s 9)))   (assoc :op (by-index (at (+ s 9))))
           (<= 0 (at (+ s 10)))  (assoc :transfer-id (at (+ s 10))))))))
 
+(defn class-witness-checker
+  "lifted-witness-checker, then a class pass on every shard it leaves :unknown (undecided, no-witness or real-time):
+  from the transfer-placement check's owners, witness rounds that treat crashed transfers with the same debit, credit,
+  amount and lookup bounds as one class, gather at most as many of a class as a gap can use and hand each gap the
+  earliest members.  :valid? true is the same proof; a history the lifted witness proves comes back unchanged.  Add it
+  to the compose map at tests/ledger.clj:363-367 as `:class-witness (class-witness-checker {})`.  Result:
+  lifted-witness-checker's map plus :class-rounds and :handed-count, and :class-cause when the class pass failed."
+  [opts]
+  (reify checker/Checker
+    (check [_ _test history _opts]
+      (let [{:keys [arrays by-index]} (flatten-history :ledger-lookups history)
+            res (Native/checkClassWitness @ctx arrays (long (:max-nodes opts 0)) (int (:max-rounds opts 0))
+                                          (int (:max-repairs opts 0)) (int (:max-lifts opts 0)))
+            at  (fn [i] (aget res (int i)))
+            s   18]                                        ; shard 0: valid cause reads transfers committed ...
+        (cond-> {:valid? (verdict (at s)) :read-count (at (+ s 2)) :transfer-count (at (+ s 3))
+                 :committed-count (at (+ s 4)) :committed-crashed-count (at (+ s 5)) :after-count (at (+ s 6))
+                 :rounds (at (+ s 8)) :repairs (at (+ s 11)) :ban-count (at (+ s 12)) :lifts (at (+ s 13))
+                 :lifted-count (at (+ s 14)) :class-rounds (at (+ s 16)) :handed-count (at (+ s 17))}
+          (pos? (at (+ s 1)))   (assoc :cause (sw-cause (at (+ s 1))))
+          (pos? (at (+ s 15)))  (assoc :class-cause (sw-cause (at (+ s 15))))
+          (<= 0 (at (+ s 9)))   (assoc :op (by-index (at (+ s 9))))
+          (<= 0 (at (+ s 10)))  (assoc :transfer-id (at (+ s 10))))))))
+
 ;; ---- independent ----------------------------------------------------------------------------------------------
 (defn independent-checker
   "Like (independent/checker (checker/compose checkers)) for a map {name checker-kind} built from THIS namespace's

@@ -710,6 +710,66 @@ typedef struct jtb_lw_result {
     double  seconds_total;
 } jtb_lw_result;
 
+/* ---- class witness (DESIGN.md "K16 class witness") ------------------------------------------------------------------
+ * The lifted serial witness, then a class pass on every shard it leaves UNKNOWN with JTB_CAUSE_UNDECIDED,
+ * JTB_CAUSE_NO_WITNESS or JTB_CAUSE_REAL_TIME.  A class is the set of crashed transfers (:info, or never completed) with
+ * a window that the transfer-placement check placed in no gap and that share (debit, credit, amount, M(t), A(t)); its
+ * members are ordered by (invocation, id).  The class pass starts again from the transfer-placement check's owners:
+ *   - the gaps with Delta' = 0 are fixed; then witness rounds (Jacobi, at most max_rounds).  Each unfixed gap gathers
+ *     as a serial-witness round does, except that of each class it takes at most cap = min over the class's observed
+ *     keys k of floor(Delta'_k / amount) members, the earliest unowned ones; the search keeps its chosen :ok transfers
+ *     and, per class, the number x_{g,c} of members it chose;
+ *   - hand-out: per class, the gaps of the round in gap order receive the unowned members at ranks
+ *     [sum_{h<g} x_{h,c}, sum_{h<=g} x_{h,c}).  A gap fails when a smaller gap of the round chose one of its :ok
+ *     transfers, or a member it receives does not exist or is not eligible for it (window, invocation before the upper
+ *     read completes, A(t) and M(t) as in the gather).  A gap is fixed, and owns what it chose and received, when it
+ *     does not fail and no gap of the round up to it that draws from one of its classes fails;
+ *   - a gap with no explanation, or max_rounds with gaps left, ends the class pass (class_cause JTB_CAUSE_NO_WITNESS);
+ *     otherwise the serial-witness check's real-time pass and re-sum run on the result (JTB_CAUSE_REAL_TIME when real
+ *     time fails; a counter mismatch is an internal error).
+ * A shard the class pass proves is VALID with the class pass's counts and commit_read; any other shard is returned as
+ * the lifted serial witness returns it, with class_cause set when the class pass ran and failed. */
+typedef struct jtb_cw_shard {
+    int32_t valid;              /* JTB_VALID / JTB_UNKNOWN                                                            */
+    int32_t cause;              /* JTB_CAUSE_* when valid == JTB_UNKNOWN (the lifted serial witness's)                */
+    int32_t n_reads;
+    int32_t n_transfers;
+    int64_t n_committed;        /* VALID: transfers committed in some gap                                             */
+    int64_t n_committed_crashed;/* VALID: of them, the crashed ones                                                   */
+    int64_t n_after;            /* VALID: :ok transfers committed after the last read                                 */
+    int64_t nodes;              /* search nodes of the lifted serial witness and of the class pass                    */
+    int32_t rounds;             /* as jtb_lw_shard's                                                                  */
+    int32_t fail_index;         /* as jtb_lw_shard's; -1 when the class pass proves the shard                         */
+    int64_t transfer_id;        /* as jtb_lw_shard's; -1 when the class pass proves the shard                         */
+    int32_t repairs;            /* as jtb_lw_shard's                                                                  */
+    int32_t n_bans;
+    int32_t lifts;
+    int32_t n_lifted;
+    int32_t class_cause;        /* JTB_CAUSE_NO_WITNESS / JTB_CAUSE_REAL_TIME when the class pass ran and failed, else 0 */
+    int32_t class_rounds;       /* class rounds that ran a gap of the shard                                           */
+    int64_t n_handed;           /* crashed transfers the class pass handed to a gap it fixed                          */
+} jtb_cw_shard;
+
+typedef struct jtb_cw_result {
+    int32_t valid;
+    int32_t n_failures;
+    int64_t n_reads;
+    int64_t n_transfers;
+    int64_t n_committed;
+    int64_t n_committed_crashed;
+    int64_t n_after;
+    int64_t nodes;
+    int64_t rounds;
+    int64_t repairs;
+    int64_t n_bans;
+    int64_t lifts;
+    int64_t n_lifted;
+    int64_t class_rounds;       /* the most class rounds of any shard                                                 */
+    int64_t n_handed;
+    double  seconds_kernel;
+    double  seconds_total;
+} jtb_cw_result;
+
 typedef struct jtb_ctx jtb_ctx;
 
 /* ---- lifecycle -------------------------------------------------------------------------------- */
@@ -719,7 +779,7 @@ int         jtb_abi_version(void);
  * 6 jtb_setfull_out, 7 jtb_bank_result, 8 jtb_final_config, 9 jtb_mono_shard, 10 jtb_mono_result, 11 jtb_cb_shard,
  * 12 jtb_cb_result, 13 jtb_tl_shard, 14 jtb_tl_result, 15 jtb_rx_shard, 16 jtb_rx_result, 17 jtb_rg_shard,
  * 18 jtb_rg_result, 19 jtb_tp_shard, 20 jtb_tp_result, 21 jtb_sw_shard, 22 jtb_sw_result, 23 jtb_rw_shard,
- * 24 jtb_rw_result, 25 jtb_lw_shard, 26 jtb_lw_result; -1 otherwise */
+ * 24 jtb_rw_result, 25 jtb_lw_shard, 26 jtb_lw_result, 27 jtb_cw_shard, 28 jtb_cw_result; -1 otherwise */
 long        jtb_struct_size(int which);
 int         jtb_device_count(void);                 /* number of CUDA devices, <0 on error          */
 jtb_ctx*    jtb_create(const jtb_opts* opts);       /* NULL on failure (no CUDA device etc.)        */
@@ -832,6 +892,13 @@ int jtb_check_repaired_witness(jtb_ctx* ctx, const jtb_history* h, int64_t max_n
 int jtb_check_lifted_witness(jtb_ctx* ctx, const jtb_history* h, int64_t max_nodes, int32_t max_rounds,
                              int32_t max_repairs, int32_t max_lifts, int32_t flags, int32_t* commit_read,
                              jtb_lw_shard* shards, jtb_lw_result* out);
+
+/* ---- class witness (see jtb_cw_shard above) -------------------------------------------------------------------- *
+ * As jtb_check_lifted_witness, with the same budgets; max_rounds also bounds the class rounds; flags is reserved and
+ * must be 0. */
+int jtb_check_class_witness(jtb_ctx* ctx, const jtb_history* h, int64_t max_nodes, int32_t max_rounds,
+                            int32_t max_repairs, int32_t max_lifts, int32_t flags, int32_t* commit_read,
+                            jtb_cw_shard* shards, jtb_cw_result* out);
 
 /* ---- multi-GPU fan-out inside the library (SURVEY §8(b) `n_gpus`, §8(e)) ----------------------------------- *
  * What `independent/checker` (set_full.clj:155) does over JVM threads, done over the GPUs of one box for a host

@@ -173,4 +173,16 @@ public final class Native {
      */
     public static native long[] checkLiftedWitness(long ctx, Object[] history, long maxNodes, int maxRounds,
                                                    int maxRepairs, int maxLifts);
+
+    /**
+     * {@code jtb_check_class_witness}: {@link #checkLiftedWitness}, then a class pass on the shards it leaves unknown
+     * (undecided, no-witness or real-time), with the same budgets.
+     *
+     * @return {@code [valid, nFailures, nReads, nTransfers, nCommitted, nCommittedCrashed, nAfter, nodes, rounds,
+     *     repairs, nBans, lifts, nLifted, classRounds, nHanded, kernelNs, totalNs, nShards]} followed by 18 longs per
+     *     shard: {@code valid, cause, nReads, nTransfers, nCommitted, nCommittedCrashed, nAfter, nodes, rounds,
+     *     failIndex, transferId, repairs, nBans, lifts, nLifted, classCause, classRounds, nHanded}
+     */
+    public static native long[] checkClassWitness(long ctx, Object[] history, long maxNodes, int maxRounds,
+                                                  int maxRepairs, int maxLifts);
 }

@@ -408,6 +408,29 @@ def lw_to_dict(res, shards, commit_read=None) -> dict:
     return out
 
 
+class CCwShard(C.Structure):
+    """jtb_cw_shard: the class-witness verdict of one shard."""
+    _fields_ = CLwShard._fields_ + [("class_cause", C.c_int32), ("class_rounds", C.c_int32), ("n_handed", C.c_int64)]
+
+
+class CCwResult(C.Structure):
+    _fields_ = CLwResult._fields_[:13] + [("class_rounds", C.c_int64), ("n_handed", C.c_int64)] + \
+        CLwResult._fields_[13:]
+
+
+CW_SHARD_FIELDS = LW_SHARD_FIELDS + ("class_cause", "class_rounds", "n_handed")
+CW_RESULT_FIELDS = LW_RESULT_FIELDS[:13] + ("class_rounds", "n_handed") + LW_RESULT_FIELDS[13:]
+
+
+def cw_to_dict(res, shards, commit_read=None) -> dict:
+    """As sw_to_dict, for jtb_cw_result / jtb_cw_shard."""
+    out = {f: getattr(res, f) for f in CW_RESULT_FIELDS}
+    out["shards"] = [{f: getattr(s, f) for f in CW_SHARD_FIELDS} for s in shards]
+    if commit_read is not None:
+        out["commit_read"] = commit_read
+    return out
+
+
 def n_transfer_records(h) -> int:
     """Transfer micro-ops of a ledger-lookups history: the records of its transfer invokes."""
     import numpy as np

@@ -685,6 +685,32 @@ class LiftedWitness(RepairedWitness):
         return top, [self._shard_map(s) for s in r["shards"]]
 
 
+class ClassWitness(LiftedWitness):
+    """The lifted serial witness, then a class pass on the GPU (K16) on every shard it leaves unknown (undecided,
+    no-witness or real-time): starting again from the transfer-placement check's owners, the witness rounds treat
+    crashed transfers with the same debit, credit, amount and lookup bounds as one class, gather at most as many of a
+    class as the gap can use, and hand each gap the earliest members of the class; the same real-time pass and re-sum
+    make a :valid? true the same proof.  A shard the lifted witness proves comes back unchanged.  Result:
+    LiftedWitness's map plus class-rounds and handed-count, and class-cause when the class pass ran and failed."""
+
+    def _shard_map(self, s: dict) -> dict:
+        m = LiftedWitness._shard_map(self, s)
+        m.update({"class-rounds": s["class_rounds"], "handed-count": s["n_handed"]})
+        if s["class_cause"]:
+            m["class-cause"] = abi.CAUSE_NAME[s["class_cause"]]
+        return m
+
+    def check_flat(self, test, h: FlatHistory) -> tuple[dict, list[dict]]:
+        r = self.ctx.check_class_witness(h, self.max_nodes, self.max_rounds, self.max_repairs, self.max_lifts)
+        top = {"valid?": VERDICT_NAME[r["valid"]], "read-count": r["n_reads"], "transfer-count": r["n_transfers"],
+               "committed-count": r["n_committed"], "committed-crashed-count": r["n_committed_crashed"],
+               "after-count": r["n_after"], "rounds": r["rounds"], "repairs": r["repairs"],
+               "ban-count": r["n_bans"], "lifts": r["lifts"], "lifted-count": r["n_lifted"],
+               "class-rounds": r["class_rounds"], "handed-count": r["n_handed"], "nodes": r["nodes"],
+               "seconds-kernel": r["seconds_kernel"], "seconds-total": r["seconds_total"]}
+        return top, [self._shard_map(s) for s in r["shards"]]
+
+
 class Compose(Checker):
     """`(checker/compose {name checker ...})`: run each, `:valid?` = merge-valid of the results."""
 
@@ -822,6 +848,12 @@ def lifted_witness_checker(opts: Mapping[str, Any] | None = None, **kw) -> Lifte
     """The repaired serial witness with lift steps (K15); {"max-nodes" "max-rounds" "max-repairs"} as for the
     repaired serial witness, {"max-lifts": n} the lift steps (default abi.LW_DEFAULT_MAX_LIFTS)."""
     return LiftedWitness(opts, **kw)
+
+
+def class_witness_checker(opts: Mapping[str, Any] | None = None, **kw) -> ClassWitness:
+    """The lifted serial witness with a class pass (K16); {"max-nodes" "max-rounds" "max-repairs" "max-lifts"} as for
+    the lifted serial witness ("max-rounds" also bounds the class rounds)."""
+    return ClassWitness(opts, **kw)
 
 
 def compose(checkers: Mapping[str, Checker]) -> Compose:
@@ -994,16 +1026,18 @@ def ledger_checker(checker_opts: Mapping[str, Any] | None = None, ctx: Context |
                    transfer_lookups: bool = False, read_explanations: bool = False,
                    read_gaps: bool = False, transfer_placement: bool = False,
                    serial_witness: bool = False, repaired_witness: bool = False,
-                   lifted_witness: bool = False) -> Compose:
+                   lifted_witness: bool = False, class_witness: bool = False) -> Compose:
     """The ledger test's checker (tests/ledger.clj:363-367) minus the gnuplot plotter, plus the
     linearizability search the north-star adds and, with monotonic=True, the monotonic-key check, with
     counter_bounds=True, the counter-bounds check, with transfer_lookups=True, the transfer-lookup check, with
     read_explanations=True, the read-explanation check, with read_gaps=True, the read-gap check, with
     transfer_placement=True, the transfer-placement check, with serial_witness=True, the serial-witness check, with
-    repaired_witness=True, the repaired serial witness and, with lifted_witness=True, the lifted serial witness:
+    repaired_witness=True, the repaired serial witness, with lifted_witness=True, the lifted serial witness and, with
+    class_witness=True, the class witness:
         {:SI (checker opts) :lookup-transfers ... :final-reads ... :unexpected-ops ... [:linear ...] [:monotonic ...]
          [:counter-bounds ...] [:transfer-lookups ...] [:read-explanations ...] [:read-gaps ...]
-         [:transfer-placement ...] [:serial-witness ...] [:repaired-witness ...] [:lifted-witness ...]}"""
+         [:transfer-placement ...] [:serial-witness ...] [:repaired-witness ...] [:lifted-witness ...]
+         [:class-witness ...]}"""
     cs: dict[str, Checker] = {"SI": bank_checker(checker_opts, ctx=ctx),
                               "lookup-transfers": lookup_all_invoked_transfers(),
                               "final-reads": final_reads(), "unexpected-ops": unexpected_ops()}
@@ -1027,4 +1061,6 @@ def ledger_checker(checker_opts: Mapping[str, Any] | None = None, ctx: Context |
         cs["repaired-witness"] = repaired_witness_checker(ctx=ctx)
     if lifted_witness:
         cs["lifted-witness"] = lifted_witness_checker(ctx=ctx)
+    if class_witness:
+        cs["class-witness"] = class_witness_checker(ctx=ctx)
     return compose(cs)

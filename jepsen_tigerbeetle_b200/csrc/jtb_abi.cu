@@ -26,6 +26,7 @@
 #include "jtb_serial_witness.cuh"
 #include "jtb_repaired_witness.cuh"
 #include "jtb_lifted_witness.cuh"
+#include "jtb_class_witness.cuh"
 
 using namespace jtb;
 
@@ -747,6 +748,8 @@ long jtb_struct_size(int which) {
     case 24: return sizeof(jtb_rw_result);
     case 25: return sizeof(jtb_lw_shard);
     case 26: return sizeof(jtb_lw_result);
+    case 27: return sizeof(jtb_cw_shard);
+    case 28: return sizeof(jtb_cw_result);
     }
     return -1;
 }
@@ -1212,6 +1215,18 @@ int jtb_check_lifted_witness(jtb_ctx* ctx, const jtb_history* h, int64_t max_nod
     ctx->fc.valid = false;
     return run_lifted_witness(ctx->stream, ctx->ev0, ctx->ev1, h, max_nodes, max_rounds, max_repairs, max_lifts, flags,
                               commit_read, shards, out, ctx->err);
+}
+
+// K16: the class witness (csrc/jtb_class_witness.cuh)
+int jtb_check_class_witness(jtb_ctx* ctx, const jtb_history* h, int64_t max_nodes, int32_t max_rounds,
+                            int32_t max_repairs, int32_t max_lifts, int32_t flags, int32_t* commit_read,
+                            jtb_cw_shard* shards, jtb_cw_result* out) {
+    if (!ctx) return -1;
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    if (cudaSetDevice(ctx->device) != cudaSuccess) { ctx->err = "cudaSetDevice failed"; return -1; }
+    ctx->fc.valid = false;
+    return run_class_witness(ctx->stream, ctx->ev0, ctx->ev1, h, max_nodes, max_rounds, max_repairs, max_lifts, flags,
+                             commit_read, shards, out, ctx->err);
 }
 
 // SURVEY 8(f) N2: the step before the checkers (independent/subhistory, ledger->bank) on the device

@@ -154,12 +154,34 @@ inline void lw_roll(jtb_lw_result* out, const jtb_lw_shard& o) {
     out->lifts = std::max(out->lifts, (int64_t)o.lifts);
     out->n_lifted += o.n_lifted;
 }
+inline void lw_set_lifts(jtb_cw_shard& o, int32_t lifts, int32_t n_lifted) {
+    o.lifts = lifts;
+    o.n_lifted = n_lifted;
+}
+inline void lw_roll(jtb_cw_result* out, const jtb_cw_shard& o) {   // K16's class-pass fields too
+    out->lifts = std::max(out->lifts, (int64_t)o.lifts);
+    out->n_lifted += o.n_lifted;
+    out->class_rounds = std::max(out->class_rounds, (int64_t)o.class_rounds);
+    out->n_handed += o.n_handed;
+}
 
-// K14 (O, R = jtb_rw_shard, jtb_rw_result; max_lifts 0: no lift steps) and K15 (jtb_lw_*; max_lifts > 0)
-template <class O, class R>
+// what runs after the repairs: nothing for K14 and K15; K16's class pass (jtb_class_witness.cuh), which snapshots
+// K12's owners before the witness (pre) and runs on the shards the repairs leave unproved (post)
+struct LwNoPass {
+    int pre(cudaStream_t, TpStage&, std::string&) { return 0; }
+    template <class O>
+    int post(cudaStream_t, cudaEvent_t, cudaEvent_t, const jtb_history*, TpStage&, int32_t, O*, std::vector<int32_t>&,
+             float&, std::string&) {
+        return 0;
+    }
+};
+
+// K14 (O, R = jtb_rw_shard, jtb_rw_result; max_lifts 0: no lift steps), K15 (jtb_lw_*; max_lifts > 0) and K16
+// (jtb_cw_*, with its class pass as Pass)
+template <class O, class R, class Pass = LwNoPass>
 inline int run_repairs(cudaStream_t st, cudaEvent_t ev0, cudaEvent_t ev1, const jtb_history* h, int64_t max_nodes,
                        int32_t max_rounds, int32_t max_repairs, int32_t max_lifts, int32_t* commit_read, O* shards,
-                       R* out, int32_t flags, std::string& err) {
+                       R* out, int32_t flags, std::string& err, Pass pass = {}) {
     const auto t0 = std::chrono::steady_clock::now();
     if (!h || !shards || !out) { err = "null argument"; return -2; }
     if (max_rounds <= 0) max_rounds = JTB_TP_DEFAULT_MAX_ROUNDS;
@@ -170,6 +192,8 @@ inline int run_repairs(cudaStream_t st, cudaEvent_t ev0, cudaEvent_t ev1, const 
     std::vector<jtb_tp_shard> tp(std::max(S, 1));
     float ms = 0;
     if (int rc = tp_finals(st, ev0, ev1, h, g, tp.data(), ms, err)) return rc;
+    if (m > 0)
+        if (int rc = pass.pre(st, g, err)) return rc;
     const TlHost& T = g.T;
     std::vector<uint8_t> sok(S, 0);
     bool any = false;
@@ -487,6 +511,8 @@ inline int run_repairs(cudaStream_t st, cudaEvent_t ev0, cudaEvent_t ev1, const 
             if (o.fail_index == INT_MIN) { err = "cudaMemcpy of a failing read failed"; return -1; }
         }
     }
+    if (m > 0)
+        if (int rc = pass.post(st, ev0, ev1, h, g, max_rounds, shards, cr_h, ms, err)) return rc;
     // commit_read: the shards with no reads commit their :ok transfers freely; a shard that is not VALID commits none
     for (int32_t s = 0; s < S; ++s) {
         const bool free_ = shards[s].valid == JTB_VALID && g.H.n_reads[s] == 0;

@@ -94,10 +94,17 @@ struct RgWarp {
 // The gather of the gap closed by a read completed at cp over the previous read invoked at ivl (-1 for gap 0), Delta
 // and the keys in W: the shard's eligible transfers that fit under Delta and pass extra(t), into the candidate arrays
 // of W and G.ct.  Returns how many there are; more than JTB_RG_MAX_GATHER means the gap has too many (the arrays hold
-// the first ones).
-template <class Extra>
+// the first ones).  cap(valid, t, amount, jd, jc, n), called by the whole warp on every batch of crashed transfers,
+// may drop more of them (the class witness's per-class cap); the default keeps them.
+struct RgNoCap {
+    __device__ __forceinline__ bool operator()(bool valid, int32_t, int32_t, int16_t, int16_t, int32_t) const {
+        return valid;
+    }
+};
+
+template <class Extra, class Cap = RgNoCap>
 __device__ __forceinline__ int32_t rg_gather(const RgDev& d, RgWarp& G, int32_t s, int32_t K, int32_t cp, int32_t ivl,
-                                             int lane, Extra extra) {
+                                             int lane, Extra extra, Cap cap = {}) {
     RxWarp& W = G.x;
     int32_t n = 0;
     auto find = [&](int64_t k) {
@@ -108,7 +115,7 @@ __device__ __forceinline__ int32_t rg_gather(const RgDev& d, RgWarp& G, int32_t 
         }
         return (int16_t)(a < K && W.key[a] == k ? a : -1);
     };
-    auto take = [&](bool valid, int32_t t) {
+    auto take = [&](bool valid, int32_t t, auto capped) {
         int16_t jd = -1, jc = -1;
         int32_t a = 0;
         if (valid) {
@@ -121,6 +128,7 @@ __device__ __forceinline__ int32_t rg_gather(const RgDev& d, RgWarp& G, int32_t 
                 valid = (jd >= 0 || jc >= 0) && (jd < 0 || a <= W.d[jd]) && (jc < 0 || a <= W.d[jc]);
             }
         }
+        valid = capped(valid, t, a, jd, jc, n);
         const unsigned bal = __ballot_sync(0xffffffffu, valid);
         const int32_t at = n + __popc(bal & ((1u << lane) - 1));
         if (valid && at < JTB_RG_MAX_GATHER) {
@@ -137,7 +145,7 @@ __device__ __forceinline__ int32_t rg_gather(const RgDev& d, RgWarp& G, int32_t 
         const int32_t j = base - lane;
         const bool valid = j >= olo && d.ok_pmax[j] >= ivl;
         if (!__any_sync(0xffffffffu, valid)) break;
-        take(valid, valid ? d.ok_t[j] : 0);
+        take(valid, valid ? d.ok_t[j] : 0, RgNoCap{});
     }
     for (int32_t c = 0; c < K && n <= JTB_RG_MAX_GATHER; ++c) {
         if (W.d[c] <= 0) continue;   // a crashed transfer anchored at c needs its amount <= Delta_c
@@ -145,7 +153,7 @@ __device__ __forceinline__ int32_t rg_gather(const RgDev& d, RgWarp& G, int32_t 
         const int32_t clo = d.cr_off[slot], bc = rx_lower(d.cr_inv, clo, d.cr_off[slot + 1], cp);
         for (int32_t base = clo; base < bc && n <= JTB_RG_MAX_GATHER; base += 32) {
             const int32_t j = base + lane;
-            take(j < bc, j < bc ? d.cr_t[j] : 0);
+            take(j < bc, j < bc ? d.cr_t[j] : 0, cap);
         }
     }
     return n;

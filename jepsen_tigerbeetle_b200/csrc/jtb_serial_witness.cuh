@@ -86,10 +86,10 @@ __global__ void sw_init(RgDev d, TpDev p, SwDev w) {
 
 // one warp, gap i: gather the candidates `take` admits (with rg_gather's own filters) and run one search; on EXPLAINED
 // its first solution goes into the gap's row of K12's poss (pn = chosen) and every chosen transfer takes the smallest
-// choosing gap (atomicMin into w.cmin)
-template <class Take>
+// choosing gap (atomicMin into w.cmin); cap goes to rg_gather
+template <class Take, class Cap = RgNoCap>
 __device__ __forceinline__ bool sw_solve(const RgDev& d, const TpDev& p, const SwDev& w, RgWarp& G, int lane,
-                                         int32_t i, Take take, int64_t& nodes, int32_t& chosen) {
+                                         int32_t i, Take take, int64_t& nodes, int32_t& chosen, Cap cap = {}) {
     RxWarp& W = G.x;
     const int32_t u = d.ord[i], s = d.shard[u], K = d.n_keys[s], cp = d.comp[u];
     const int32_t lower = i > 0 && d.shard[d.ord[i - 1]] == s ? d.ord[i - 1] : -1;
@@ -110,7 +110,7 @@ __device__ __forceinline__ bool sw_solve(const RgDev& d, const TpDev& p, const S
         neg = __any_sync(0xffffffffu, neg);
         __syncwarp();
         if (!neg) {
-            const int32_t n = rg_gather(d, G, s, K, cp, ivl, lane, take);
+            const int32_t n = rg_gather(d, G, s, K, cp, ivl, lane, take, cap);
             __syncwarp();
             if (n <= JTB_RG_MAX_GATHER) {
                 int32_t root_key, kept;

@@ -393,13 +393,15 @@ struct Gap {
 };
 
 // The gather of gap i (upper read u, lower read l) into pb.P, with pb.d = Delta': round 0 every eligible transfer, a
-// later round (or a witness round) only the in-window ones no gap owns; keep (may be null) drops more.  false: past
-// JTB_TP_MAX_GATHER.
+// later round (or a witness round) only the in-window ones no gap owns; keep (may be null) drops more.  With cls (the
+// class of each crashed transfer, -1 none) the crashed candidates of a class stop at cap = min over its observed keys
+// of floor(Delta'_k / amount), the first ones in gather order.  false: past JTB_TP_MAX_GATHER.
 bool gather_gap(const Shard& S, const Index& X, const std::vector<Window>& W, const std::vector<int32_t>& owner,
                 const XRead& u, const XRead* l, int32_t i, int32_t round, Problem& pb,
-                const std::function<bool(int32_t)>* keep = nullptr) {
+                const std::function<bool(int32_t)>* keep = nullptr, const std::vector<int32_t>* cls = nullptr) {
     const int32_t K = (int32_t)pb.d.size();
     const int32_t ivl = l ? l->inv : -1;
+    std::unordered_map<int32_t, int64_t> had;   // cls: gathered members per class
     auto take = [&](int32_t t) {
         const XTransfer& x = S.T[t];
         if (x.fate == JTB_T_FAIL || !(x.inv < u.comp) || !(x.A < u.comp) || x.M < ivl || x.amount <= 0) return true;
@@ -408,6 +410,12 @@ bool gather_gap(const Shard& S, const Index& X, const std::vector<Window>& W, co
         const int32_t jd = W[t].jd, jc = W[t].jc;
         if (jd < 0 && jc < 0) return true;
         if ((jd >= 0 && x.amount > pb.d[jd]) || (jc >= 0 && x.amount > pb.d[jc])) return true;
+        if (cls && (*cls)[t] >= 0) {
+            int64_t cap = INT64_MAX;
+            if (jd >= 0) cap = pb.d[jd] / x.amount;
+            if (jc >= 0) cap = std::min(cap, pb.d[jc] / x.amount);
+            if (had[(*cls)[t]]++ >= cap) return true;
+        }
         pb.P.push_back({x.id, x.amount, jd, jc, t});
         return pb.P.size() <= (size_t)JTB_TP_MAX_GATHER;
     };

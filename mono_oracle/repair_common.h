@@ -23,6 +23,10 @@ inline void set_lifts(jtb_lw_shard& o, int32_t lifts, int32_t n_lifted) {
     o.lifts = lifts;
     o.n_lifted = n_lifted;
 }
+inline void set_lifts(jtb_cw_shard& o, int32_t lifts, int32_t n_lifted) {
+    o.lifts = lifts;
+    o.n_lifted = n_lifted;
+}
 
 // the steals of the failing gaps (Jacobi): gap g searches the free and the chosen transfers that keep(t, g) admits; a
 // thief keeps its solution when no smaller thief took one of them.  thief, loot and rel (every failing gap) per gap
@@ -174,11 +178,14 @@ int repaired(const Shard& S, const std::vector<int32_t>& keys, const std::vector
 }
 
 // every shard of h: the witness and its repairs where TP_SEARCH calls the shard VALID; O / R the shard and result
-// structs (jtb_rw_* or jtb_lw_*)
+// structs (jtb_rw_*, jtb_lw_* or jtb_cw_*).  post (may be null) runs on every shard that ends UNKNOWN with cause
+// UNDECIDED, NO_WITNESS or REAL_TIME, with TP_SEARCH's state as TP_SEARCH left it
 template <class O, class R>
 int repaired_check(const jtb_history* h, int64_t max_nodes, int32_t max_rounds, int32_t max_repairs,
                    int32_t max_lifts, int32_t* commit_read, O* shards, R* out,
-                   void (*roll)(R*, const O&)) {
+                   void (*roll)(R*, const O&),
+                   int (*post)(const Shard&, const std::vector<int32_t>&, const std::vector<int32_t>&, TpState&,
+                               int64_t, int32_t, RepairOut<O>&) = nullptr) {
     const auto t0 = std::chrono::steady_clock::now();
     if (max_nodes <= 0) max_nodes = JTB_TP_DEFAULT_MAX_NODES;
     if (max_rounds <= 0) max_rounds = JTB_TP_DEFAULT_MAX_ROUNDS;
@@ -222,12 +229,18 @@ int repaired_check(const jtb_history* h, int64_t max_nodes, int32_t max_rounds, 
             if (p.valid != JTB_VALID) {
                 o.valid = JTB_UNKNOWN;
                 o.cause = p.valid == JTB_INVALID ? JTB_CAUSE_ANOMALY : JTB_CAUSE_UNDECIDED;
+                if (post && o.cause == JTB_CAUSE_UNDECIDED)
+                    if (int rc = post(S, keys, ord, T, max_nodes, max_rounds, w)) return rc;
                 continue;
             }
+            TpState T0;
+            if (post) T0 = T;
             if (int rc = repaired(S, keys, ord, T, max_nodes, max_rounds, max_repairs, max_lifts, w)) return rc;
             if (o.valid != JTB_VALID) {
                 o.n_committed = o.n_committed_crashed = o.n_after = 0;
                 std::fill(w.commit.begin(), w.commit.end(), JTB_SW_NEVER);
+                if (post)
+                    if (int rc = post(S, keys, ord, T0, max_nodes, max_rounds, w)) return rc;
             }
         }
     } catch (int) {
