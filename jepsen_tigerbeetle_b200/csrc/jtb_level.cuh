@@ -135,7 +135,11 @@ struct LvScratch {   // per warp, shared memory
     uint32_t start[36];     // exclusive prefix of the child counts; [32] = total
     uint32_t crashed[BEAM ? 32 : 1];   // beam mode: crashed ops consumed by each configuration of the chunk
     uint32_t stage_aux[BEAM ? LV_STAGE : 1];
-    uint64_t stage[LV_STAGE][EW];
+    // staged new children: the key, and (bank) the parent's lane and the transfer; the balances are built from the
+    // parent's S.bal when the entry is flushed, so every chunk flushes what it staged before the next one's phase 1
+    uint32_t stage_mv[BAL ? LV_STAGE : 1];   // owner | d << 5 | c << 8
+    int32_t stage_amt[BAL ? LV_STAGE : 1];
+    uint64_t stage[LV_STAGE][KW];
 };
 
 __device__ __forceinline__ int select64(uint64_t m, int k) {   // position of the k-th (0-based) set bit
@@ -374,8 +378,22 @@ __global__ void __launch_bounds__(LV_THREADS, JTB_LV_CTAS) level_search_kernel(c
             if (base + n <= p.seg_cap) {
                 uint64_t* dst = my_out + base * EW;
                 for (unsigned x = lane; x < n * EW; x += 32) {
-                    const unsigned e = x / EW, k = x - e * EW;
-                    dst[x] = S.stage[(stg_head + e) % LV_STAGE][k];
+                    const unsigned e = x / EW, k = x - e * EW, r = (stg_head + e) % LV_STAGE;
+                    if (k < (unsigned)KW) {
+                        dst[x] = S.stage[r][k];
+                    } else if constexpr (BAL) {   // balances 2i, 2i+1 of the parent, after the transfer
+                        const unsigned mv = S.stage_mv[r], i0 = 2 * (k - KW);
+                        const int owner = (int)(mv & 31), d = (int)((mv >> 5) & 7), c = (int)((mv >> 8) & 7);
+                        const int32_t amt = S.stage_amt[r];
+                        int32_t b0 = S.bal[owner][i0], b1 = S.bal[owner][i0 + 1];
+                        if (amt) {
+                            if ((int)i0 == d) b0 -= amt;
+                            if ((int)i0 + 1 == d) b1 -= amt;
+                            if ((int)i0 == c) b0 += amt;
+                            if ((int)i0 + 1 == c) b1 += amt;
+                        }
+                        dst[x] = u64_of(b0, b1);
+                    }
                 }
                 if (BEAM && (unsigned)lane < n)
                     p.aux[a.in_idx ^ 1][(unsigned long long)my_seg * p.seg_cap + base + lane] = S.stage_aux[(stg_head + lane) % LV_STAGE];
@@ -548,23 +566,14 @@ __global__ void __launch_bounds__(LV_THREADS, JTB_LV_CTAS) level_search_kernel(c
                 const unsigned newm = __ballot_sync(FULL, is_new);
                 if (newm) {
                     if (is_new) {
-                        uint64_t* e = S.stage[(stg_tail + __popc(newm & lt_mask)) % LV_STAGE];
-                        if constexpr (BEAM) S.stage_aux[(stg_tail + __popc(newm & lt_mask)) % LV_STAGE] = child_crashed;
+                        const unsigned r = (stg_tail + __popc(newm & lt_mask)) % LV_STAGE;
+                        uint64_t* e = S.stage[r];
+                        if constexpr (BEAM) S.stage_aux[r] = child_crashed;
 #pragma unroll
                         for (int i = 0; i < KW; ++i) e[i] = ch.w[i];
                         if constexpr (BAL) {
-                            int32_t b[8];
-#pragma unroll
-                            for (int i = 0; i < 8; ++i) b[i] = S.bal[owner][i];
-                            if (ch.amt) {
-#pragma unroll
-                                for (int i = 0; i < 8; ++i) {
-                                    if (i == ch.d) b[i] -= ch.amt;
-                                    if (i == ch.c) b[i] += ch.amt;
-                                }
-                            }
-#pragma unroll
-                            for (int i = 0; i < 4; ++i) e[KW + i] = u64_of(b[2 * i], b[2 * i + 1]);
+                            S.stage_mv[r] = (unsigned)owner | ((unsigned)(ch.d & 7) << 5) | ((unsigned)(ch.c & 7) << 8);
+                            S.stage_amt[r] = ch.amt;
                         }
                     }
                     stg_tail += __popc(newm);
@@ -572,6 +581,8 @@ __global__ void __launch_bounds__(LV_THREADS, JTB_LV_CTAS) level_search_kernel(c
                     if (stg_tail - stg_head >= 32) flush(32);
                 }
             }
+            // the staged balances are built from this chunk's S.bal: flush before the next chunk overwrites it
+            if (BAL && stg_tail != stg_head) flush(stg_tail - stg_head);
             __syncwarp();   // the scratch of this chunk is dead
             LV_PROF(1, tp);   // phase 2
         }
