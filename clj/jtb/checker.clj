@@ -538,7 +538,7 @@
                                                                :other-op (by-index (at (+ s 20))))))
           (and (= 2 (at s)) (<= 0 (at (+ s 14)))) (assoc :lower-op (by-index (at (+ s 14)))))))))
 
-(def ^:private sw-cause {4 :partial-read 5 :anomaly 6 :undecided 7 :no-witness 8 :real-time})
+(def ^:private sw-cause {4 :partial-read 5 :anomaly 6 :undecided 7 :no-witness 8 :real-time 9 :lookup})
 
 (defn serial-witness-checker
   "A proof that a ledger history is linearizable, on the GPU, or :unknown: the transfer-placement check, then one
@@ -627,6 +627,33 @@
                  :lifted-count (at (+ s 14)) :class-rounds (at (+ s 16)) :handed-count (at (+ s 17))}
           (pos? (at (+ s 1)))   (assoc :cause (sw-cause (at (+ s 1))))
           (pos? (at (+ s 15)))  (assoc :class-cause (sw-cause (at (+ s 15))))
+          (<= 0 (at (+ s 9)))   (assoc :op (by-index (at (+ s 9))))
+          (<= 0 (at (+ s 10)))  (assoc :transfer-id (at (+ s 10))))))))
+
+(defn lookup-witness-checker
+  "class-witness-checker, then every :ok lookup of a shard it proves placed in the serial order: each lookup where it
+  returns exactly the transfers committed before it, the lookups of one read gap nested, and one real-time pass over
+  the reads, transfers and lookups together.  :valid? true then covers the whole ledger history, lookups included.  A
+  shard whose lookups have no place is :unknown with :cause :lookup and :lookup-op, the lookup that failed.  Add it to
+  the compose map at tests/ledger.clj:363-367 as `:lookup-witness (lookup-witness-checker {})`.  Result:
+  class-witness-checker's map plus :lookups-placed-count, and :lookup-cause and :lookup-op when the lookups failed."
+  [opts]
+  (reify checker/Checker
+    (check [_ _test history _opts]
+      (let [{:keys [arrays by-index]} (flatten-history :ledger-lookups history)
+            res (Native/checkLookupWitness @ctx arrays (long (:max-nodes opts 0)) (int (:max-rounds opts 0))
+                                           (int (:max-repairs opts 0)) (int (:max-lifts opts 0)))
+            at  (fn [i] (aget res (int i)))
+            s   19]                                        ; shard 0: valid cause reads transfers committed ...
+        (cond-> {:valid? (verdict (at s)) :read-count (at (+ s 2)) :transfer-count (at (+ s 3))
+                 :committed-count (at (+ s 4)) :committed-crashed-count (at (+ s 5)) :after-count (at (+ s 6))
+                 :rounds (at (+ s 8)) :repairs (at (+ s 11)) :ban-count (at (+ s 12)) :lifts (at (+ s 13))
+                 :lifted-count (at (+ s 14)) :class-rounds (at (+ s 16)) :handed-count (at (+ s 17))
+                 :lookups-placed-count (at (+ s 20))}
+          (pos? (at (+ s 1)))   (assoc :cause (sw-cause (at (+ s 1))))
+          (pos? (at (+ s 15)))  (assoc :class-cause (sw-cause (at (+ s 15))))
+          (pos? (at (+ s 18)))  (assoc :lookup-cause (sw-cause (at (+ s 18)))
+                                       :lookup-op (by-index (at (+ s 19))))
           (<= 0 (at (+ s 9)))   (assoc :op (by-index (at (+ s 9))))
           (<= 0 (at (+ s 10)))  (assoc :transfer-id (at (+ s 10))))))))
 

@@ -156,6 +156,7 @@ typedef struct jtb_lin_shard {
 #define JTB_CAUSE_UNDECIDED     6 /* serial-witness check: the transfer-placement check left a gap undecided          */
 #define JTB_CAUSE_NO_WITNESS    7 /* serial-witness check: a witness round did not explain a gap, or max_rounds ran out */
 #define JTB_CAUSE_REAL_TIME     8 /* serial-witness check: the serial order of the chosen gaps breaks real time       */
+#define JTB_CAUSE_LOOKUP        9 /* lookup witness: an :ok lookup has no place in the serial order of a proved shard   */
 
 typedef struct jtb_lin_result {
     int32_t  valid;             /* merge-valid over shards                                            */
@@ -770,6 +771,67 @@ typedef struct jtb_cw_result {
     double  seconds_total;
 } jtb_cw_result;
 
+/* ---- lookup witness (DESIGN.md "K17 lookup witness") ----------------------------------------------------------------
+ * The class witness, then every :ok lookup of a shard it proves is placed in the shard's serial order.  A shard the
+ * class witness does not prove, or with no :ok lookup, is returned as the class witness returns it.  On the others,
+ * with D_g the transfers the witness commits in gap g and n the shard's reads, every transfer gets a commit gap G(t):
+ * g for t in D_g; n (after the last read) for an :ok transfer in no D_g, and for a crashed transfer in no D_g that an
+ * :ok lookup of the shard returns; never otherwise.  Each lookup returns exactly the transfers committed before its
+ * point:
+ *   - a record that names no transfer of the shard, differs from its invocation's (debit, credit, amount), names a :fail
+ *     or a never-committed transfer, or repeats an id, or lo = max G over what it returns above hi = min G over the
+ *     committed transfers it lacks, leaves the lookup unplaceable;
+ *   - each lookup goes to the latest gap of [lo, hi] whose lower read's real-time point is below its completion; the
+ *     lookups of one gap must return nested subsets of D_g, which then come in layers before each lookup;
+ *   - one greedy real-time pass over the merged order of reads, transfers and lookups checks every op.
+ * A failure makes the shard UNKNOWN with cause and lookup_cause JTB_CAUSE_LOOKUP, and fail_index / lookup_fail_index
+ * the completion :index of the lookup that fails (for the real-time pass: the last lookup at or before the first op
+ * that fails). */
+typedef struct jtb_lk_shard {
+    int32_t valid;              /* JTB_VALID / JTB_UNKNOWN                                                            */
+    int32_t cause;              /* JTB_CAUSE_* when valid == JTB_UNKNOWN (the class witness's, or JTB_CAUSE_LOOKUP)    */
+    int32_t n_reads;
+    int32_t n_transfers;
+    int64_t n_committed;        /* VALID: as jtb_cw_shard's                                                           */
+    int64_t n_committed_crashed;
+    int64_t n_after;
+    int64_t nodes;
+    int32_t rounds;
+    int32_t fail_index;         /* as jtb_cw_shard's; the failing lookup's completion :index with JTB_CAUSE_LOOKUP    */
+    int64_t transfer_id;
+    int32_t repairs;
+    int32_t n_bans;
+    int32_t lifts;
+    int32_t n_lifted;
+    int32_t class_cause;
+    int32_t class_rounds;
+    int64_t n_handed;
+    int32_t lookup_cause;       /* JTB_CAUSE_LOOKUP when the lookups of a proved shard could not be placed, else 0     */
+    int32_t lookup_fail_index;  /* the completion :index of that lookup, -1 none                                      */
+    int64_t n_lookups_placed;   /* VALID: :ok lookups placed in the serial order                                      */
+} jtb_lk_shard;
+
+typedef struct jtb_lk_result {
+    int32_t valid;
+    int32_t n_failures;
+    int64_t n_reads;
+    int64_t n_transfers;
+    int64_t n_committed;
+    int64_t n_committed_crashed;
+    int64_t n_after;
+    int64_t nodes;
+    int64_t rounds;
+    int64_t repairs;
+    int64_t n_bans;
+    int64_t lifts;
+    int64_t n_lifted;
+    int64_t class_rounds;
+    int64_t n_handed;
+    int64_t n_lookups_placed;
+    double  seconds_kernel;
+    double  seconds_total;
+} jtb_lk_result;
+
 typedef struct jtb_ctx jtb_ctx;
 
 /* ---- lifecycle -------------------------------------------------------------------------------- */
@@ -779,7 +841,8 @@ int         jtb_abi_version(void);
  * 6 jtb_setfull_out, 7 jtb_bank_result, 8 jtb_final_config, 9 jtb_mono_shard, 10 jtb_mono_result, 11 jtb_cb_shard,
  * 12 jtb_cb_result, 13 jtb_tl_shard, 14 jtb_tl_result, 15 jtb_rx_shard, 16 jtb_rx_result, 17 jtb_rg_shard,
  * 18 jtb_rg_result, 19 jtb_tp_shard, 20 jtb_tp_result, 21 jtb_sw_shard, 22 jtb_sw_result, 23 jtb_rw_shard,
- * 24 jtb_rw_result, 25 jtb_lw_shard, 26 jtb_lw_result, 27 jtb_cw_shard, 28 jtb_cw_result; -1 otherwise */
+ * 24 jtb_rw_result, 25 jtb_lw_shard, 26 jtb_lw_result, 27 jtb_cw_shard, 28 jtb_cw_result, 30 jtb_lk_shard,
+ * 31 jtb_lk_result (29 is unassigned); -1 otherwise */
 long        jtb_struct_size(int which);
 int         jtb_device_count(void);                 /* number of CUDA devices, <0 on error          */
 jtb_ctx*    jtb_create(const jtb_opts* opts);       /* NULL on failure (no CUDA device etc.)        */
@@ -899,6 +962,16 @@ int jtb_check_lifted_witness(jtb_ctx* ctx, const jtb_history* h, int64_t max_nod
 int jtb_check_class_witness(jtb_ctx* ctx, const jtb_history* h, int64_t max_nodes, int32_t max_rounds,
                             int32_t max_repairs, int32_t max_lifts, int32_t flags, int32_t* commit_read,
                             jtb_cw_shard* shards, jtb_cw_result* out);
+
+/* ---- lookup witness (see jtb_lk_shard above) ------------------------------------------------------------------- *
+ * As jtb_check_class_witness, with the same budgets; flags is reserved and must be 0.  commit_read (may be NULL) as
+ * the class witness's, except that a crashed transfer committed after the last read because a lookup returns it is
+ * JTB_SW_AFTER.  lookup_read (may be NULL) gets one entry per :ok lookup in history order: the completion :index of
+ * the read the lookup precedes in the serial order, JTB_SW_AFTER after the last read, and JTB_SW_NEVER for every lookup
+ * of a shard that is not VALID. */
+int jtb_check_lookup_witness(jtb_ctx* ctx, const jtb_history* h, int64_t max_nodes, int32_t max_rounds,
+                             int32_t max_repairs, int32_t max_lifts, int32_t flags, int32_t* commit_read,
+                             int32_t* lookup_read, jtb_lk_shard* shards, jtb_lk_result* out);
 
 /* ---- multi-GPU fan-out inside the library (SURVEY §8(b) `n_gpus`, §8(e)) ----------------------------------- *
  * What `independent/checker` (set_full.clj:155) does over JVM threads, done over the GPUs of one box for a host

@@ -185,4 +185,17 @@ public final class Native {
      */
     public static native long[] checkClassWitness(long ctx, Object[] history, long maxNodes, int maxRounds,
                                                   int maxRepairs, int maxLifts);
+
+    /**
+     * {@code jtb_check_lookup_witness}: {@link #checkClassWitness}, then every :ok lookup of a shard it proves placed
+     * in the serial order, with the same budgets.
+     *
+     * @return {@code [valid, nFailures, nReads, nTransfers, nCommitted, nCommittedCrashed, nAfter, nodes, rounds,
+     *     repairs, nBans, lifts, nLifted, classRounds, nHanded, nLookupsPlaced, kernelNs, totalNs, nShards]} followed
+     *     by 21 longs per shard: {@code valid, cause, nReads, nTransfers, nCommitted, nCommittedCrashed, nAfter, nodes,
+     *     rounds, failIndex, transferId, repairs, nBans, lifts, nLifted, classCause, classRounds, nHanded, lookupCause,
+     *     lookupFailIndex, nLookupsPlaced}
+     */
+    public static native long[] checkLookupWitness(long ctx, Object[] history, long maxNodes, int maxRounds,
+                                                   int maxRepairs, int maxLifts);
 }

@@ -15,7 +15,7 @@ OPT_NO_BEAM = 16
 CAUSE_NONE, CAUSE_TABLE_FULL, CAUSE_BUDGET, CAUSE_TOO_WIDE, CAUSE_PARTIAL_READ = 0, 1, 2, 3, 4
 CAUSE_ANOMALY, CAUSE_UNDECIDED, CAUSE_NO_WITNESS, CAUSE_REAL_TIME = 5, 6, 7, 8
 CAUSE_NAME = {0: None, 1: "table-full", 2: "budget", 3: "too-wide", 4: "partial-read", 5: "anomaly", 6: "undecided",
-              7: "no-witness", 8: "real-time"}
+              7: "no-witness", 8: "real-time", 9: "lookup"}
 MONO_NO_REALTIME = 1
 MONO_EDGE_NONE, MONO_EDGE_MONOTONIC, MONO_EDGE_REALTIME = 0, 1, 2
 CB_BELOW, CB_ABOVE = 1, 2
@@ -429,6 +429,39 @@ def cw_to_dict(res, shards, commit_read=None) -> dict:
     if commit_read is not None:
         out["commit_read"] = commit_read
     return out
+
+
+class CLkShard(C.Structure):
+    """jtb_lk_shard: the lookup-witness verdict of one shard."""
+    _fields_ = CCwShard._fields_ + [("lookup_cause", C.c_int32), ("lookup_fail_index", C.c_int32),
+                                    ("n_lookups_placed", C.c_int64)]
+
+
+class CLkResult(C.Structure):
+    _fields_ = CCwResult._fields_[:15] + [("n_lookups_placed", C.c_int64)] + CCwResult._fields_[15:]
+
+
+CAUSE_LOOKUP = 9
+LK_SHARD_FIELDS = CW_SHARD_FIELDS + ("lookup_cause", "lookup_fail_index", "n_lookups_placed")
+LK_RESULT_FIELDS = CW_RESULT_FIELDS[:15] + ("n_lookups_placed",) + CW_RESULT_FIELDS[15:]
+
+
+def lk_to_dict(res, shards, commit_read=None, lookup_read=None) -> dict:
+    """As sw_to_dict, for jtb_lk_result / jtb_lk_shard; "lookup_read" (one entry per :ok lookup in history order) when
+    it was asked for."""
+    out = {f: getattr(res, f) for f in LK_RESULT_FIELDS}
+    out["shards"] = [{f: getattr(s, f) for f in LK_SHARD_FIELDS} for s in shards]
+    if commit_read is not None:
+        out["commit_read"] = commit_read
+    if lookup_read is not None:
+        out["lookup_read"] = lookup_read
+    return out
+
+
+def n_ok_lookups(h) -> int:
+    """:ok lookups of a ledger-lookups history."""
+    import numpy as np
+    return int(np.sum((h.type == 1) & (h.f == 5) & (h.process >= 0) & (h.payload_len >= 0)))
 
 
 def n_transfer_records(h) -> int:

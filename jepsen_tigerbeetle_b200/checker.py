@@ -711,6 +711,33 @@ class ClassWitness(LiftedWitness):
         return top, [self._shard_map(s) for s in r["shards"]]
 
 
+class LookupWitness(ClassWitness):
+    """The class witness, then every :ok lookup placed in the serial order it proves, on the GPU (K17): each lookup
+    goes where it returns exactly the transfers committed before it, the lookups of one read gap must return nested
+    sets, and one real-time pass checks the reads, transfers and lookups together.  A :valid? true then covers the
+    whole ledger history, lookups included.  A shard whose lookups have no place is :unknown with cause "lookup" and
+    lookup-op, the lookup that failed.  Result: ClassWitness's map plus lookups-placed-count, and lookup-cause."""
+
+    def _shard_map(self, s: dict) -> dict:
+        m = ClassWitness._shard_map(self, s)
+        m["lookups-placed-count"] = s["n_lookups_placed"]
+        if s["lookup_cause"]:
+            m["lookup-cause"] = abi.CAUSE_NAME[s["lookup_cause"]]
+            m["lookup-op"] = {"index": s["lookup_fail_index"]}
+        return m
+
+    def check_flat(self, test, h: FlatHistory) -> tuple[dict, list[dict]]:
+        r = self.ctx.check_lookup_witness(h, self.max_nodes, self.max_rounds, self.max_repairs, self.max_lifts)
+        top = {"valid?": VERDICT_NAME[r["valid"]], "read-count": r["n_reads"], "transfer-count": r["n_transfers"],
+               "committed-count": r["n_committed"], "committed-crashed-count": r["n_committed_crashed"],
+               "after-count": r["n_after"], "rounds": r["rounds"], "repairs": r["repairs"],
+               "ban-count": r["n_bans"], "lifts": r["lifts"], "lifted-count": r["n_lifted"],
+               "class-rounds": r["class_rounds"], "handed-count": r["n_handed"],
+               "lookups-placed-count": r["n_lookups_placed"], "nodes": r["nodes"],
+               "seconds-kernel": r["seconds_kernel"], "seconds-total": r["seconds_total"]}
+        return top, [self._shard_map(s) for s in r["shards"]]
+
+
 class Compose(Checker):
     """`(checker/compose {name checker ...})`: run each, `:valid?` = merge-valid of the results."""
 
@@ -854,6 +881,12 @@ def class_witness_checker(opts: Mapping[str, Any] | None = None, **kw) -> ClassW
     """The lifted serial witness with a class pass (K16); {"max-nodes" "max-rounds" "max-repairs" "max-lifts"} as for
     the lifted serial witness ("max-rounds" also bounds the class rounds)."""
     return ClassWitness(opts, **kw)
+
+
+def lookup_witness_checker(opts: Mapping[str, Any] | None = None, **kw) -> LookupWitness:
+    """The class witness with its lookups placed (K17); {"max-nodes" "max-rounds" "max-repairs" "max-lifts"} as for
+    the class witness."""
+    return LookupWitness(opts, **kw)
 
 
 def compose(checkers: Mapping[str, Checker]) -> Compose:
@@ -1026,18 +1059,19 @@ def ledger_checker(checker_opts: Mapping[str, Any] | None = None, ctx: Context |
                    transfer_lookups: bool = False, read_explanations: bool = False,
                    read_gaps: bool = False, transfer_placement: bool = False,
                    serial_witness: bool = False, repaired_witness: bool = False,
-                   lifted_witness: bool = False, class_witness: bool = False) -> Compose:
+                   lifted_witness: bool = False, class_witness: bool = False,
+                   lookup_witness: bool = False) -> Compose:
     """The ledger test's checker (tests/ledger.clj:363-367) minus the gnuplot plotter, plus the
     linearizability search the north-star adds and, with monotonic=True, the monotonic-key check, with
     counter_bounds=True, the counter-bounds check, with transfer_lookups=True, the transfer-lookup check, with
     read_explanations=True, the read-explanation check, with read_gaps=True, the read-gap check, with
     transfer_placement=True, the transfer-placement check, with serial_witness=True, the serial-witness check, with
-    repaired_witness=True, the repaired serial witness, with lifted_witness=True, the lifted serial witness and, with
-    class_witness=True, the class witness:
+    repaired_witness=True, the repaired serial witness, with lifted_witness=True, the lifted serial witness, with
+    class_witness=True, the class witness and, with lookup_witness=True, the lookup witness:
         {:SI (checker opts) :lookup-transfers ... :final-reads ... :unexpected-ops ... [:linear ...] [:monotonic ...]
          [:counter-bounds ...] [:transfer-lookups ...] [:read-explanations ...] [:read-gaps ...]
          [:transfer-placement ...] [:serial-witness ...] [:repaired-witness ...] [:lifted-witness ...]
-         [:class-witness ...]}"""
+         [:class-witness ...] [:lookup-witness ...]}"""
     cs: dict[str, Checker] = {"SI": bank_checker(checker_opts, ctx=ctx),
                               "lookup-transfers": lookup_all_invoked_transfers(),
                               "final-reads": final_reads(), "unexpected-ops": unexpected_ops()}
@@ -1063,4 +1097,6 @@ def ledger_checker(checker_opts: Mapping[str, Any] | None = None, ctx: Context |
         cs["lifted-witness"] = lifted_witness_checker(ctx=ctx)
     if class_witness:
         cs["class-witness"] = class_witness_checker(ctx=ctx)
+    if lookup_witness:
+        cs["lookup-witness"] = lookup_witness_checker(ctx=ctx)
     return compose(cs)

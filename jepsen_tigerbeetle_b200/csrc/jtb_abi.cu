@@ -27,6 +27,7 @@
 #include "jtb_repaired_witness.cuh"
 #include "jtb_lifted_witness.cuh"
 #include "jtb_class_witness.cuh"
+#include "jtb_lookup_witness.cuh"
 
 using namespace jtb;
 
@@ -750,6 +751,8 @@ long jtb_struct_size(int which) {
     case 26: return sizeof(jtb_lw_result);
     case 27: return sizeof(jtb_cw_shard);
     case 28: return sizeof(jtb_cw_result);
+    case 30: return sizeof(jtb_lk_shard);
+    case 31: return sizeof(jtb_lk_result);
     }
     return -1;
 }
@@ -1227,6 +1230,18 @@ int jtb_check_class_witness(jtb_ctx* ctx, const jtb_history* h, int64_t max_node
     ctx->fc.valid = false;
     return run_class_witness(ctx->stream, ctx->ev0, ctx->ev1, h, max_nodes, max_rounds, max_repairs, max_lifts, flags,
                              commit_read, shards, out, ctx->err);
+}
+
+// K17: the lookup witness (csrc/jtb_lookup_witness.cuh)
+int jtb_check_lookup_witness(jtb_ctx* ctx, const jtb_history* h, int64_t max_nodes, int32_t max_rounds,
+                             int32_t max_repairs, int32_t max_lifts, int32_t flags, int32_t* commit_read,
+                             int32_t* lookup_read, jtb_lk_shard* shards, jtb_lk_result* out) {
+    if (!ctx) return -1;
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    if (cudaSetDevice(ctx->device) != cudaSuccess) { ctx->err = "cudaSetDevice failed"; return -1; }
+    ctx->fc.valid = false;
+    return run_lookup_witness(ctx->stream, ctx->ev0, ctx->ev1, h, max_nodes, max_rounds, max_repairs, max_lifts, flags,
+                              commit_read, lookup_read, shards, out, ctx->err);
 }
 
 // SURVEY 8(f) N2: the step before the checkers (independent/subhistory, ledger->bank) on the device

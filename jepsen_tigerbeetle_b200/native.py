@@ -21,7 +21,7 @@ _DEPS = _SOURCES + ["jtb_prep.h", "jtb_expand.h", "jtb_wgl.cuh", "jtb_scout.cuh"
                     "jtb_table_bench.cuh", "jtb_level.cuh", "jtb_partition.cuh", "jtb_monotonic.cuh",
                     "jtb_counter_bounds.cuh", "jtb_transfer_lookups.cuh", "jtb_read_explanations.cuh",
                     "jtb_read_gaps.cuh", "jtb_transfer_placement.cuh", "jtb_serial_witness.cuh", "jtb_repaired_witness.cuh",
-                    "jtb_lifted_witness.cuh", "jtb_class_witness.cuh", "jtb_call.cuh"]
+                    "jtb_lifted_witness.cuh", "jtb_class_witness.cuh", "jtb_lookup_witness.cuh", "jtb_call.cuh"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared", "-ldl"]
 
@@ -30,6 +30,7 @@ EXPORTS = ["jtb_abi_version", "jtb_device_count", "jtb_create", "jtb_destroy", "
            "jtb_check_counter_bounds", "jtb_check_transfer_lookups", "jtb_check_read_explanations",
            "jtb_check_read_gaps", "jtb_check_transfer_placement", "jtb_check_serial_witness",
            "jtb_check_repaired_witness", "jtb_check_lifted_witness", "jtb_check_class_witness",
+           "jtb_check_lookup_witness",
            "jtb_table_bench", "jtb_get_stats", "jtb_struct_size", "jtb_prepare_seconds", "jtb_prepare_info",
            "jtb_final_configs", "jtb_gather_bench", "jtb_host_alloc", "jtb_host_free", "jtb_partition_by_key", "jtb_ledger_balances", "jtb_multi_create", "jtb_multi_create_error", "jtb_multi_destroy", "jtb_multi_n_gpus",
            "jtb_multi_last_error", "jtb_multi_check_linearizable", "jtb_multi_check_set_full"]
@@ -94,6 +95,9 @@ def lib() -> C.CDLL:
                                                    C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
             L.jtb_check_class_witness.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_int32,
                                                   C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
+            L.jtb_check_lookup_witness.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_int32,
+                                                   C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                   C.c_void_p]
             L.jtb_table_bench.argtypes = [C.c_void_p, C.c_uint64, C.c_int, C.c_int, C.c_void_p,
                                           C.c_void_p, C.c_void_p]
             L.jtb_gather_bench.argtypes = [C.c_void_p, C.c_uint64, C.c_int, C.c_int, C.c_uint32, C.c_int, C.c_int,
@@ -379,6 +383,31 @@ class Context:
         if rc != 0:
             raise NativeError(f"jtb_check_class_witness rc={rc}: {self._err()}")
         return abi.cw_to_dict(res, shards[:h.n_shards], cr[:res.n_transfers].copy() if witness else None)
+
+    # ---- K17: lookup witness -------------------------------------------------------------------------------------
+    def check_lookup_witness(self, h: FlatHistory, max_nodes: int = 0, max_rounds: int = 0, max_repairs: int = 0,
+                             max_lifts: int = 0, witness: bool = False, flags: int = 0) -> dict:
+        """check_class_witness, then every :ok lookup of a shard it proves is placed in the shard's serial order: each
+        lookup at a point where it returns exactly the transfers committed before it, the lookups of one read gap
+        nested, and one real-time pass over the reads, transfers and lookups together.  A shard whose lookups cannot
+        be placed is UNKNOWN with cause "lookup".  The dict of check_class_witness with "n_lookups_placed" added, and
+        per shard "lookup_cause", "lookup_fail_index" and "n_lookups_placed"; with witness=True also "lookup_read" (one
+        entry per :ok lookup in history order).  flags must be 0."""
+        import numpy as np
+        ch = as_c_history(h)
+        shards = (abi.CLkShard * max(1, h.n_shards))()
+        res = abi.CLkResult()
+        cr = np.zeros(max(1, abi.n_transfer_records(h)), np.int32) if witness else None
+        nl = abi.n_ok_lookups(h)
+        lr = np.zeros(max(1, nl), np.int32) if witness else None
+        rc = lib().jtb_check_lookup_witness(self._h, C.addressof(ch), max_nodes, max_rounds, max_repairs, max_lifts,
+                                            flags, cr.ctypes.data if witness else None,
+                                            lr.ctypes.data if witness else None, C.addressof(shards),
+                                            C.addressof(res))
+        if rc != 0:
+            raise NativeError(f"jtb_check_lookup_witness rc={rc}: {self._err()}")
+        return abi.lk_to_dict(res, shards[:h.n_shards], cr[:res.n_transfers].copy() if witness else None,
+                              lr[:nl].copy() if witness else None)
 
     def final_configs(self, h: FlatHistory, model: CModel, shard: int = 0, cap: int = 10) -> dict:
         """knossos' :configs of an INVALID shard (`jtb_final_configs`): call directly after `check_linearizable`

@@ -744,3 +744,46 @@ JNIEXPORT jlongArray JNICALL Java_jtb_Native_checkClassWitness(JNIEnv* env, jcla
     free(shards);
     return out;
 }
+
+/* ---- K17: lookup witness ----------------------------------------------------------------------------------------- */
+JNIEXPORT jlongArray JNICALL Java_jtb_Native_checkLookupWitness(JNIEnv* env, jclass cls, jlong handle,
+                                                                jobjectArray history, jlong max_nodes, jint max_rounds,
+                                                                jint max_repairs, jint max_lifts) {
+    (void)cls;
+    jtb_history hist;
+    hist_pins pins;
+    if (pin_history(env, history, &hist, &pins)) return NULL;
+    const int ns = hist.n_shards;
+    jtb_lk_shard* shards = (jtb_lk_shard*)calloc(ns > 0 ? (size_t)ns : 1, sizeof *shards);
+    jtb_lk_result r;
+    memset(&r, 0, sizeof r);
+    const int rc = jtb_check_lookup_witness((jtb_ctx*)(intptr_t)handle, &hist, (int64_t)max_nodes,
+                                            (int32_t)max_rounds, (int32_t)max_repairs, (int32_t)max_lifts, 0, NULL,
+                                            NULL, shards, &r);
+    unpin_history(env, &pins);
+    if (rc != 0) {
+        free(shards);
+        throw_rt(env, jtb_last_error((jtb_ctx*)(intptr_t)handle));
+        return NULL;
+    }
+    const int64_t total = 19 + 21ll * ns;
+    jlong* v = (jlong*)calloc((size_t)total, sizeof *v);
+    int64_t k = 0;
+    v[k++] = r.valid; v[k++] = r.n_failures; v[k++] = r.n_reads; v[k++] = r.n_transfers; v[k++] = r.n_committed;
+    v[k++] = r.n_committed_crashed; v[k++] = r.n_after; v[k++] = r.nodes; v[k++] = r.rounds; v[k++] = r.repairs;
+    v[k++] = r.n_bans; v[k++] = r.lifts; v[k++] = r.n_lifted; v[k++] = r.class_rounds; v[k++] = r.n_handed;
+    v[k++] = r.n_lookups_placed; v[k++] = ns_of(r.seconds_kernel); v[k++] = ns_of(r.seconds_total); v[k++] = ns;
+    for (int s = 0; s < ns; ++s) {
+        const jtb_lk_shard* q = &shards[s];
+        v[k++] = q->valid; v[k++] = q->cause; v[k++] = q->n_reads; v[k++] = q->n_transfers; v[k++] = q->n_committed;
+        v[k++] = q->n_committed_crashed; v[k++] = q->n_after; v[k++] = q->nodes; v[k++] = q->rounds;
+        v[k++] = q->fail_index; v[k++] = q->transfer_id; v[k++] = q->repairs; v[k++] = q->n_bans; v[k++] = q->lifts;
+        v[k++] = q->n_lifted; v[k++] = q->class_cause; v[k++] = q->class_rounds; v[k++] = q->n_handed;
+        v[k++] = q->lookup_cause; v[k++] = q->lookup_fail_index; v[k++] = q->n_lookups_placed;
+    }
+    jlongArray out = (*env)->NewLongArray(env, (jsize)k);
+    if (out) (*env)->SetLongArrayRegion(env, out, 0, (jsize)k, v);
+    free(v);
+    free(shards);
+    return out;
+}

@@ -13,7 +13,9 @@ library's rounds of per-gap searches with owned transfers carried between gaps. 
 SW_SEARCH is TP_SEARCH followed by the library's witness rounds, real-time pass and commit_read.  See
 serial_witness.cpp.  RW_SEARCH is SW_SEARCH followed by the library's repair rounds.  See repaired_witness.cpp.
 LW_SEARCH is RW_SEARCH with lift steps where its repairs would stop.  See lifted_witness.cpp and repair_common.h.
-CW_SEARCH is LW_SEARCH followed by the library's class pass on the shards it leaves unproved.  See class_witness.cpp."""
+CW_SEARCH is LW_SEARCH followed by the library's class pass on the shards it leaves unproved.  See class_witness.cpp.
+LK_SEARCH is CW_SEARCH followed by the library's placement of the lookups; LK_BRUTE is its definition on tiny
+histories.  See lookup_witness.cpp."""
 from __future__ import annotations
 
 import ctypes as C
@@ -34,6 +36,7 @@ SW_SEARCH = 1
 RW_SEARCH = 1
 LW_SEARCH = 1
 CW_SEARCH = 1
+LK_BRUTE, LK_SEARCH = 0, 1
 DECIDE_PARTIAL = 1 << 16   # decide shards with partial reads instead of reporting them UNKNOWN
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB = None
@@ -46,7 +49,7 @@ def build(force: bool = False) -> str:
     srcs = [os.path.join(_HERE, f) for f in ("mono_oracle.cpp", "counter_bounds.cpp", "transfer_lookups.cpp",
                                                 "read_explanations.cpp", "read_gaps.cpp", "transfer_placement.cpp",
                                                 "serial_witness.cpp", "repaired_witness.cpp", "lifted_witness.cpp",
-                                                "class_witness.cpp", "gaps_common.h", "witness_common.h",
+                                                "class_witness.cpp", "lookup_witness.cpp", "gaps_common.h", "witness_common.h",
                                                 "repair_common.h", "Makefile")]
     srcs.append(os.path.join(_HERE, "..", "include", "jtb_check.h"))
     stale = not os.path.exists(so) or any(os.path.getmtime(s) > os.path.getmtime(so) for s in srcs)
@@ -90,6 +93,10 @@ def lib() -> C.CDLL:
         _LIB.jtbm_cw_last_error.restype = C.c_char_p
         _LIB.jtbm_check_class_witness.argtypes = [C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_int32,
                                                   C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
+        _LIB.jtbm_lk_last_error.restype = C.c_char_p
+        _LIB.jtbm_check_lookup_witness.argtypes = [C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_int32,
+                                                   C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                   C.c_void_p]
     return _LIB
 
 
@@ -241,3 +248,23 @@ def check_class_witness(h: FlatHistory, algo: int = CW_SEARCH, max_nodes: int = 
     if rc != 0:
         raise RuntimeError(lib().jtbm_cw_last_error().decode())
     return abi.cw_to_dict(res, shards[:h.n_shards], cr[:res.n_transfers].copy() if witness else None)
+
+
+def check_lookup_witness(h: FlatHistory, algo: int = LK_SEARCH, max_nodes: int = 0, max_rounds: int = 0,
+                         max_repairs: int = 0, max_lifts: int = 0, flags: int = 0, witness: bool = True) -> dict:
+    """Twin of `jtb_check_lookup_witness` (same result dict as `native.Context.check_lookup_witness`).  LK_BRUTE fills
+    only each shard's valid (JTB_VALID when a serial order exists, else JTB_INVALID), n_reads and n_transfers."""
+    import numpy as np
+    ch = as_c_history(h)
+    shards = (abi.CLkShard * max(1, h.n_shards))()
+    res = abi.CLkResult()
+    cr = np.zeros(max(1, abi.n_transfer_records(h)), np.int32)
+    nl = abi.n_ok_lookups(h)
+    lr = np.zeros(max(1, nl), np.int32)
+    rc = lib().jtbm_check_lookup_witness(C.addressof(ch), max_nodes, max_rounds, max_repairs, max_lifts, flags, algo,
+                                         cr.ctypes.data if witness else None, lr.ctypes.data if witness else None,
+                                         C.addressof(shards), C.addressof(res))
+    if rc != 0:
+        raise RuntimeError(lib().jtbm_lk_last_error().decode())
+    return abi.lk_to_dict(res, shards[:h.n_shards], cr[:res.n_transfers].copy() if witness else None,
+                          lr[:nl].copy() if witness else None)
