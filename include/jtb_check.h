@@ -842,7 +842,8 @@ int         jtb_abi_version(void);
  * 12 jtb_cb_result, 13 jtb_tl_shard, 14 jtb_tl_result, 15 jtb_rx_shard, 16 jtb_rx_result, 17 jtb_rg_shard,
  * 18 jtb_rg_result, 19 jtb_tp_shard, 20 jtb_tp_result, 21 jtb_sw_shard, 22 jtb_sw_result, 23 jtb_rw_shard,
  * 24 jtb_rw_result, 25 jtb_lw_shard, 26 jtb_lw_result, 27 jtb_cw_shard, 28 jtb_cw_result, 30 jtb_lk_shard,
- * 31 jtb_lk_result (29 is unassigned); -1 otherwise */
+ * 31 jtb_lk_result, 33 jtb_edn_history (29 and 32 are unassigned: bindings built against earlier libraries test
+ * them as unknown ids); -1 otherwise */
 long        jtb_struct_size(int which);
 int         jtb_device_count(void);                 /* number of CUDA devices, <0 on error          */
 jtb_ctx*    jtb_create(const jtb_opts* opts);       /* NULL on failure (no CUDA device etc.)        */
@@ -972,6 +973,32 @@ int jtb_check_class_witness(jtb_ctx* ctx, const jtb_history* h, int64_t max_node
 int jtb_check_lookup_witness(jtb_ctx* ctx, const jtb_history* h, int64_t max_nodes, int32_t max_rounds,
                              int32_t max_repairs, int32_t max_lifts, int32_t flags, int32_t* commit_read,
                              int32_t* lookup_read, jtb_lk_shard* shards, jtb_lk_result* out);
+
+/* ---- K18: a stored ledger history.edn read on the device ------------------------------------------------------ *
+ * The bytes of a Jepsen history.edn (one op map per top-level form, optionally tagged #jepsen.history.Op{...}, or one
+ * top-level vector of op maps) flattened into one of the ledger forms: exactly the arrays of the Python path
+ * edn.read_history + history.flatten_ops(ops, form), and meta["multi_transfer_txns"] (0 for JTB_FORM_BANK).  The
+ * history is one shard (key id -1).  Its arrays are page-locked host memory the library owns (jtb_host_alloc); release
+ * them with jtb_edn_history_free.  The EDN read is the subset Jepsen's store writes: keys in any order, unknown keys
+ * with arbitrary values, integers with an optional N suffix, nil, true, false, keywords, strings with escapes and ','
+ * as whitespace; ';' comments, #_ discard, character literals and a float where an integer is read are refused.
+ * Returns 0, or <0 where the Python path raises or the EDN is unsupported, with jtb_last_error giving the byte and the
+ * reason (out is left empty; the context stays usable).  flags is reserved and must be 0. */
+#define JTB_FORM_BANK            0   /* flatten_ops(..., "bank")            */
+#define JTB_FORM_LEDGER_COUNTERS 1   /* flatten_ops(..., "ledger-counters") */
+#define JTB_FORM_LEDGER_LOOKUPS  2   /* flatten_ops(..., "ledger-lookups")  */
+typedef struct jtb_edn_history {
+    jtb_history history;
+    int64_t multi_transfer_txns;   /* transfer invokes with more than one micro-op (ledger forms)          */
+    int64_t n_ops;                 /* top-level op maps read, client and nemesis alike                      */
+    double  seconds_h2d;           /* copy of the text to the device                                        */
+    double  seconds_kernel;        /* device passes (CUDA events)                                           */
+    double  seconds_d2h;           /* copy of the arrays back into page-locked host memory                  */
+    double  seconds_total;
+} jtb_edn_history;
+int  jtb_read_ledger_edn(jtb_ctx* ctx, const char* text, int64_t n_bytes, int32_t form, int32_t flags,
+                         jtb_edn_history* out);
+void jtb_edn_history_free(jtb_edn_history* out);
 
 /* ---- multi-GPU fan-out inside the library (SURVEY §8(b) `n_gpus`, §8(e)) ----------------------------------- *
  * What `independent/checker` (set_full.clj:155) does over JVM threads, done over the GPUs of one box for a host

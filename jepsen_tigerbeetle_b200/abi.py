@@ -3,7 +3,7 @@ from __future__ import annotations
 
 import ctypes as C
 
-from .history import MAX_ACCOUNTS
+from .history import MAX_ACCOUNTS, CHistory
 
 ABI_VERSION = 10
 OPT_NO_EAGER_READS = 1
@@ -469,3 +469,17 @@ def n_transfer_records(h) -> int:
     import numpy as np
     inv = (h.type == 0) & (h.f == 4) & (h.process >= 0) & (h.payload_len > 0)
     return int(np.sum(h.payload_len[inv] // 5))
+
+
+# ---- K18: the stored-history reader --------------------------------------------------------------------------------
+FORM_BANK, FORM_LEDGER_COUNTERS, FORM_LEDGER_LOOKUPS = 0, 1, 2
+FORMS = {"bank": FORM_BANK, "ledger-counters": FORM_LEDGER_COUNTERS, "ledger-lookups": FORM_LEDGER_LOOKUPS}
+
+
+class CEdnHistory(C.Structure):
+    """ctypes image of `struct jtb_edn_history`."""
+
+    _fields_ = [("history", CHistory), ("multi_transfer_txns", C.c_int64), ("n_ops", C.c_int64),
+                ("seconds_h2d", C.c_double), ("seconds_kernel", C.c_double), ("seconds_d2h", C.c_double),
+                ("seconds_total", C.c_double)]
+

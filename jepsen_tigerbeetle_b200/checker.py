@@ -57,9 +57,56 @@ def check_safe(checker: Checker, test, history, opts=None) -> dict:
         return {"valid?": "unknown", "error": traceback.format_exc()}
 
 
+class StoredLedgerHistory:
+    """A stored ledger history.edn (a path or its bytes) that the ledger checks read on the GPU (K18).
+
+    `_flat` asks it for the "bank", "ledger-counters" or "ledger-lookups" form and gets the device reader's FlatHistory,
+    read once per form and cached, instead of flattening op maps in Python.  Iterating it yields the op maps of
+    `edn.read_history` (parsed once, on first use, and cached), so the host-only checkers of a `ledger_checker()`
+    compose (unexpected-ops, final-reads, lookup-transfers, stats) still work, but they still pay the Python parse.
+    ctx: the native.Context to read on; None opens one on device 0 when the first form is asked for."""
+
+    def __init__(self, path_or_bytes, ctx=None) -> None:
+        if isinstance(path_or_bytes, (bytes, bytearray, memoryview)):
+            self._data = bytes(path_or_bytes)
+        else:
+            with open(path_or_bytes, "rb") as fh:
+                self._data = fh.read()
+        self._ctx = ctx
+        self._forms: dict[str, FlatHistory] = {}
+        self._ops: list | None = None
+
+    def flat(self, form: str) -> FlatHistory:
+        if form not in self._forms:
+            if self._ctx is None:
+                from .native import Context
+                self._ctx = Context(device=0)
+            self._forms[form] = self._ctx.read_ledger_edn(self._data, form)
+        return self._forms[form]
+
+    def ops(self) -> list:
+        if self._ops is None:
+            from .edn import read_history
+            self._ops = read_history(self._data.decode())
+        return self._ops
+
+    def __iter__(self):
+        return iter(self.ops())
+
+    def __len__(self) -> int:
+        return len(self.ops())
+
+    def __getitem__(self, i):
+        return self.ops()[i]
+
+
 def _flat(history, model: str) -> FlatHistory:
     if isinstance(history, FlatHistory):
         return history
+    if isinstance(history, StoredLedgerHistory):
+        if model in ("bank", "ledger-counters", "ledger-lookups"):
+            return history.flat(model)
+        return flatten_ops(history.ops(), model)
     return flatten_ops(history, model)
 
 

@@ -28,6 +28,7 @@
 #include "jtb_lifted_witness.cuh"
 #include "jtb_class_witness.cuh"
 #include "jtb_lookup_witness.cuh"
+#include "jtb_edn.cuh"
 
 using namespace jtb;
 
@@ -753,6 +754,7 @@ long jtb_struct_size(int which) {
     case 28: return sizeof(jtb_cw_result);
     case 30: return sizeof(jtb_lk_shard);
     case 31: return sizeof(jtb_lk_result);
+    case 33: return sizeof(jtb_edn_history);
     }
     return -1;
 }
@@ -1242,6 +1244,20 @@ int jtb_check_lookup_witness(jtb_ctx* ctx, const jtb_history* h, int64_t max_nod
     ctx->fc.valid = false;
     return run_lookup_witness(ctx->stream, ctx->ev0, ctx->ev1, h, max_nodes, max_rounds, max_repairs, max_lifts, flags,
                               commit_read, lookup_read, shards, out, ctx->err);
+}
+
+// K18: a stored ledger history.edn read on the device (csrc/jtb_edn.cuh)
+int jtb_read_ledger_edn(jtb_ctx* ctx, const char* text, int64_t n_bytes, int32_t form, int32_t flags,
+                        jtb_edn_history* out) {
+    if (!ctx) return -1;
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    if (cudaSetDevice(ctx->device) != cudaSuccess) { ctx->err = "cudaSetDevice failed"; return -1; }
+    ctx->fc.valid = false;
+    return run_read_ledger_edn(ctx->stream, ctx->ev0, ctx->ev1, text, n_bytes, form, flags, out, ctx->err);
+}
+
+void jtb_edn_history_free(jtb_edn_history* out) {
+    if (out) jtb_edn_history_release(out);
 }
 
 // SURVEY 8(f) N2: the step before the checkers (independent/subhistory, ledger->bank) on the device

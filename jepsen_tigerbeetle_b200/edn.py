@@ -186,3 +186,15 @@ def read_history(text_or_lines: str | Iterable[str], independent: bool = False) 
             raise EDNError("history entries must be maps")
         ops.append(_tuplify(f, independent))
     return ops
+
+
+def read_ledger_flat(path, form: str, ctx=None):
+    """history.edn (a path or its bytes) -> the FlatHistory flatten_ops(read_history(text), form) makes, for the ledger
+    forms "bank", "ledger-counters" and "ledger-lookups", read on the GPU (K18, `Context.read_ledger_edn`).  ctx: a
+    native.Context to use; None opens one on device 0 for this call."""
+    from . import native
+    if ctx is not None:
+        return ctx.read_ledger_edn(path, form)
+    with native.Context(device=0) as c:
+        return c.read_ledger_edn(path, form)
+

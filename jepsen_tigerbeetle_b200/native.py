@@ -21,7 +21,7 @@ _DEPS = _SOURCES + ["jtb_prep.h", "jtb_expand.h", "jtb_wgl.cuh", "jtb_scout.cuh"
                     "jtb_table_bench.cuh", "jtb_level.cuh", "jtb_partition.cuh", "jtb_monotonic.cuh",
                     "jtb_counter_bounds.cuh", "jtb_transfer_lookups.cuh", "jtb_read_explanations.cuh",
                     "jtb_read_gaps.cuh", "jtb_transfer_placement.cuh", "jtb_serial_witness.cuh", "jtb_repaired_witness.cuh",
-                    "jtb_lifted_witness.cuh", "jtb_class_witness.cuh", "jtb_lookup_witness.cuh", "jtb_call.cuh"]
+                    "jtb_lifted_witness.cuh", "jtb_class_witness.cuh", "jtb_lookup_witness.cuh", "jtb_edn.cuh", "jtb_call.cuh"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared", "-ldl"]
 
@@ -30,7 +30,7 @@ EXPORTS = ["jtb_abi_version", "jtb_device_count", "jtb_create", "jtb_destroy", "
            "jtb_check_counter_bounds", "jtb_check_transfer_lookups", "jtb_check_read_explanations",
            "jtb_check_read_gaps", "jtb_check_transfer_placement", "jtb_check_serial_witness",
            "jtb_check_repaired_witness", "jtb_check_lifted_witness", "jtb_check_class_witness",
-           "jtb_check_lookup_witness",
+           "jtb_check_lookup_witness", "jtb_read_ledger_edn", "jtb_edn_history_free",
            "jtb_table_bench", "jtb_get_stats", "jtb_struct_size", "jtb_prepare_seconds", "jtb_prepare_info",
            "jtb_final_configs", "jtb_gather_bench", "jtb_host_alloc", "jtb_host_free", "jtb_partition_by_key", "jtb_ledger_balances", "jtb_multi_create", "jtb_multi_create_error", "jtb_multi_destroy", "jtb_multi_n_gpus",
            "jtb_multi_last_error", "jtb_multi_check_linearizable", "jtb_multi_check_set_full"]
@@ -98,6 +98,8 @@ def lib() -> C.CDLL:
             L.jtb_check_lookup_witness.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_int32,
                                                    C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                                    C.c_void_p]
+            L.jtb_read_ledger_edn.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_void_p]
+            L.jtb_edn_history_free.argtypes = [C.c_void_p]
             L.jtb_table_bench.argtypes = [C.c_void_p, C.c_uint64, C.c_int, C.c_int, C.c_void_p,
                                           C.c_void_p, C.c_void_p]
             L.jtb_gather_bench.argtypes = [C.c_void_p, C.c_uint64, C.c_int, C.c_int, C.c_uint32, C.c_int, C.c_int,
@@ -409,6 +411,31 @@ class Context:
         return abi.lk_to_dict(res, shards[:h.n_shards], cr[:res.n_transfers].copy() if witness else None,
                               lr[:nl].copy() if witness else None)
 
+    # ---- K18: a stored ledger history.edn read on the device ------------------------------------------------------
+    def read_ledger_edn(self, data, form: str, timings: dict | None = None) -> FlatHistory:
+        """The bytes of a Jepsen history.edn (bytes, bytearray, memoryview, or a path) flattened on the device into
+        `form` ("bank", "ledger-counters" or "ledger-lookups"): the arrays flatten_ops(edn.read_history(text), form)
+        makes, in page-locked memory the returned FlatHistory owns.  Raises NativeError where the Python path raises or
+        the EDN is outside the subset Jepsen's store writes.  `timings`, when given, receives the call's seconds_h2d,
+        seconds_kernel, seconds_d2h, seconds_total and n_ops."""
+        if form not in abi.FORMS:
+            raise ValueError(f"unknown ledger form {form!r}")
+        if isinstance(data, (str, os.PathLike)):
+            with open(data, "rb") as fh:
+                data = fh.read()
+        if not isinstance(data, bytes):
+            data = bytes(data)
+        n = len(data)
+        keep = C.c_char_p(data)   # the bytes object's own buffer, no copy
+        out = abi.CEdnHistory()
+        rc = lib().jtb_read_ledger_edn(self._h, C.cast(keep, C.c_void_p), n, abi.FORMS[form], 0, C.addressof(out))
+        if rc != 0:
+            raise NativeError(f"jtb_read_ledger_edn rc={rc}: {self._err()}")
+        if timings is not None:
+            timings.update(seconds_h2d=out.seconds_h2d, seconds_kernel=out.seconds_kernel,
+                           seconds_d2h=out.seconds_d2h, seconds_total=out.seconds_total, n_ops=out.n_ops)
+        return _owned_flat(out, form)
+
     def final_configs(self, h: FlatHistory, model: CModel, shard: int = 0, cap: int = 10) -> dict:
         """knossos' :configs of an INVALID shard (`jtb_final_configs`): call directly after `check_linearizable`
         on the same history.  Returns {"total": all such configurations, "configs": the first `cap` of them}."""
@@ -556,6 +583,44 @@ def prepare_info(h: FlatHistory, model: CModel) -> dict:
     info = (C.c_longlong * 4)()
     sec = lib().jtb_prepare_info(C.addressof(ch), C.addressof(model), C.addressof(info))
     return {"seconds": sec, "key_bytes": info[0], "slot_lanes": info[1], "max_classes": info[2], "ranks": info[3]}
+
+
+class _EdnArrays:
+    """The page-locked arrays of one jtb_edn_history, released when the last numpy view of them is gone."""
+
+    def __init__(self, out) -> None:
+        self.out, self.live = out, 0
+
+    def view(self, ptr, dtype, n):
+        import weakref
+
+        import numpy as np
+        dt = np.dtype(dtype)
+        raw = (C.c_char * max(n * dt.itemsize, 1)).from_address(ptr)
+        base = np.frombuffer(raw, dtype=dt, count=n)
+        self.live += 1
+        weakref.finalize(base, self._drop)
+        return base
+
+    def _drop(self) -> None:
+        self.live -= 1
+        if self.live == 0 and _lib is not None:
+            _lib.jtb_edn_history_free(C.addressof(self.out))
+
+
+def _owned_flat(out, form: str) -> FlatHistory:
+    import numpy as np
+    h, n, owner = out.history, out.history.n_events, _EdnArrays(out)
+    arr = {name: owner.view(getattr(h, name), dt, n) for name, dt in (
+        ("type", np.uint8), ("f", np.uint8), ("flags", np.uint8), ("process", np.int32), ("index", np.int32),
+        ("time_ns", np.int64), ("a", np.int32), ("b", np.int32), ("c", np.int32), ("payload_off", np.int64),
+        ("payload_len", np.int32))}
+    meta = {"model": form}
+    if form != "bank":
+        meta["multi_transfer_txns"] = int(out.multi_transfer_txns)
+    return FlatHistory(payload=owner.view(h.payload, np.int32, h.n_payload),
+                       shard_off=owner.view(h.shard_off, np.int64, 2), key_ids=owner.view(h.key_ids, np.int64, 1),
+                       meta=meta, **arr)
 
 
 def device_count() -> int:
