@@ -842,7 +842,7 @@ int         jtb_abi_version(void);
  * 12 jtb_cb_result, 13 jtb_tl_shard, 14 jtb_tl_result, 15 jtb_rx_shard, 16 jtb_rx_result, 17 jtb_rg_shard,
  * 18 jtb_rg_result, 19 jtb_tp_shard, 20 jtb_tp_result, 21 jtb_sw_shard, 22 jtb_sw_result, 23 jtb_rw_shard,
  * 24 jtb_rw_result, 25 jtb_lw_shard, 26 jtb_lw_result, 27 jtb_cw_shard, 28 jtb_cw_result, 30 jtb_lk_shard,
- * 31 jtb_lk_result, 33 jtb_edn_history (29 and 32 are unassigned: bindings built against earlier libraries test
+ * 31 jtb_lk_result, 33 jtb_edn_history, 34 jtb_edn_checks (29 and 32 are unassigned: bindings built against earlier libraries test
  * them as unknown ids); -1 otherwise */
 long        jtb_struct_size(int which);
 int         jtb_device_count(void);                 /* number of CUDA devices, <0 on error          */
@@ -999,6 +999,57 @@ typedef struct jtb_edn_history {
 int  jtb_read_ledger_edn(jtb_ctx* ctx, const char* text, int64_t n_bytes, int32_t form, int32_t flags,
                          jtb_edn_history* out);
 void jtb_edn_history_free(jtb_edn_history* out);
+
+/* ---- K19: the host checks of a ledger compose on a stored history.edn ------------------------------------------ *
+ * The bytes jtb_read_ledger_edn reads, summarised for the checkers unexpected-ops, lookup-all-invoked-transfers,
+ * final-reads and stats (tests/ledger.clj:194-282, jepsen.checker/stats) as they run on the op maps of
+ * edn.read_history: a missing :index or :time counts as 0, and a txn's tag is its first micro-op's (an empty value has
+ * none).  Client ops are those with an integer :process.  Reported per flagged op: its ordinal among the top-level op
+ * maps, the bytes of its map, its :index and :time with their presence, and where they apply its class of equal
+ * :value and its suspect bit.  The flagged ops' arrays are page-locked host memory the library owns; release them with
+ * jtb_edn_checks_free.  Where the summary could differ from those checkers the call refuses the input instead:
+ * refused = 1, refused_at = the byte (-1 none) and refused_reason; the arrays are then empty.  It refuses whatever
+ * jtb_read_ledger_edn refuses in JTB_FORM_LEDGER_LOOKUPS; a micro-op of a :final? :ok read or lookup that is not
+ * [keyword id map-or-nil] with an int64 id; a key of its map other than :debit-acct :credit-acct :amount
+ * :debits-posted :credits-posted, or a value there that is not an int64 or nil; a transfer invoke's id that is not an
+ * int64; and a collision of the 128-bit digests that group equal final values.  Returns 0 (refused or not), <0 on
+ * malformed arguments, CUDA and allocation errors.  flags is reserved and must be 0. */
+typedef struct jtb_edn_flag {
+    int64_t op;          /* ordinal among the top-level op maps                                                  */
+    int64_t begin, end;  /* the op map's bytes [begin, end), from its '{' (a tag before it is not included)       */
+    int64_t time;        /* :time, 0 when absent                                                                  */
+    int64_t first;       /* open invokes: the ordinal of the first invoke of the process's last run of invokes
+                            (where unexpected-ops puts the process in its map); -1 otherwise                      */
+    int32_t index;       /* :index, 0 when absent                                                                 */
+    int32_t cls;         /* final reads and final lookups: the class of equal :value, from 0 per kind; -1 otherwise */
+    uint8_t has_time, has_index;
+    uint8_t suspect;     /* final lookups: the lookup lacks an id some transfer invoke has                         */
+    uint8_t pad[5];
+} jtb_edn_flag;
+typedef struct jtb_edn_checks {
+    int64_t n_ops;             /* top-level op maps read, client and nemesis alike                                  */
+    int64_t n_client;          /* ops with an integer :process                                                      */
+    int64_t n_ok, n_fail, n_info;   /* client completions by :type (every client op is :f :txn)                    */
+    int64_t n_open;            /* invokes that are the last client op of their process                             */
+    int64_t n_final_reads, n_final_lookups;   /* :final? :ok ops whose first micro-op is :r, :l-t              */
+    int64_t n_read_classes, n_lookup_classes; /* distinct :value among them                                       */
+    int64_t n_invoked;         /* distinct ids of the micro-ops of :t invokes                                       */
+    int64_t n_suspect;         /* final lookups that lack one of them                                               */
+    jtb_edn_flag last;         /* the last client op (op = -1: none)                                                */
+    jtb_edn_flag* open;        /* n_open, by :process                                                              */
+    jtb_edn_flag* fails;       /* n_fail, in history order                                                          */
+    jtb_edn_flag* final_reads; /* n_final_reads, in history order                                                   */
+    jtb_edn_flag* final_lookups;   /* n_final_lookups, in history order                                             */
+    int32_t refused, reserved;
+    int64_t refused_at;
+    char    refused_reason[128];
+    double  seconds_h2d;       /* copy of the text to the device                                                    */
+    double  seconds_kernel;    /* device passes (CUDA events)                                                       */
+    double  seconds_d2h;       /* copy of the flagged ops back                                                      */
+    double  seconds_total;
+} jtb_edn_checks;
+int  jtb_ledger_edn_checks(jtb_ctx* ctx, const char* text, int64_t n_bytes, int32_t flags, jtb_edn_checks* out);
+void jtb_edn_checks_free(jtb_edn_checks* out);
 
 /* ---- multi-GPU fan-out inside the library (SURVEY §8(b) `n_gpus`, §8(e)) ----------------------------------- *
  * What `independent/checker` (set_full.clj:155) does over JVM threads, done over the GPUs of one box for a host

@@ -483,3 +483,29 @@ class CEdnHistory(C.Structure):
                 ("seconds_h2d", C.c_double), ("seconds_kernel", C.c_double), ("seconds_d2h", C.c_double),
                 ("seconds_total", C.c_double)]
 
+
+
+# ---- K19: the host checks of a ledger compose on a stored history.edn ----------------------------------------------
+class CEdnFlag(C.Structure):
+    """ctypes image of `struct jtb_edn_flag`: one flagged op of a stored history."""
+
+    _fields_ = [("op", C.c_int64), ("begin", C.c_int64), ("end", C.c_int64), ("time", C.c_int64),
+                ("first", C.c_int64), ("index", C.c_int32), ("cls", C.c_int32), ("has_time", C.c_uint8),
+                ("has_index", C.c_uint8), ("suspect", C.c_uint8), ("pad", C.c_uint8 * 5)]
+
+
+EDN_FLAG_DTYPE = [("op", "<i8"), ("begin", "<i8"), ("end", "<i8"), ("time", "<i8"), ("first", "<i8"),
+                  ("index", "<i4"), ("cls", "<i4"), ("has_time", "u1"), ("has_index", "u1"), ("suspect", "u1"),
+                  ("pad", "u1", (5,))]
+EDN_CHECKS_COUNTS = ("n_ops", "n_client", "n_ok", "n_fail", "n_info", "n_open", "n_final_reads", "n_final_lookups",
+                     "n_read_classes", "n_lookup_classes", "n_invoked", "n_suspect")
+
+
+class CEdnChecks(C.Structure):
+    """ctypes image of `struct jtb_edn_checks`."""
+
+    _fields_ = ([(name, C.c_int64) for name in EDN_CHECKS_COUNTS]
+                + [("last", CEdnFlag), ("open", C.c_void_p), ("fails", C.c_void_p), ("final_reads", C.c_void_p),
+                   ("final_lookups", C.c_void_p), ("refused", C.c_int32), ("reserved", C.c_int32),
+                   ("refused_at", C.c_int64), ("refused_reason", C.c_char * 128), ("seconds_h2d", C.c_double),
+                   ("seconds_kernel", C.c_double), ("seconds_d2h", C.c_double), ("seconds_total", C.c_double)])

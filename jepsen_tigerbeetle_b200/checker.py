@@ -18,7 +18,8 @@ Histories may be given as Jepsen op maps (list of dicts) or as an already flatte
 from __future__ import annotations
 
 import traceback
-from typing import Any, Mapping
+from collections.abc import Mapping
+from typing import Any
 
 import numpy as np
 
@@ -57,37 +58,82 @@ def check_safe(checker: Checker, test, history, opts=None) -> dict:
         return {"valid?": "unknown", "error": traceback.format_exc()}
 
 
+class StoredOp(Mapping):
+    """One op map of a stored history.edn, given by its bytes [begin, end) and parsed (`edn.loads`) only when it is
+    first read.  It equals the dict `edn.read_history` gives for that op, so a result holding the 40 MB final lookups of
+    a large history costs nothing until someone reads them."""
+
+    __slots__ = ("_data", "_begin", "_end", "_op")
+
+    def __init__(self, data: bytes, begin: int, end: int) -> None:
+        self._data, self._begin, self._end, self._op = data, int(begin), int(end), None
+
+    @property
+    def parsed(self) -> bool:
+        return self._op is not None
+
+    def _map(self) -> dict:
+        if self._op is None:
+            from .edn import loads
+            self._op = loads(self._data[self._begin:self._end].decode())
+        return self._op
+
+    def __getitem__(self, key):
+        return self._map()[key]
+
+    def __iter__(self):
+        return iter(self._map())
+
+    def __len__(self) -> int:
+        return len(self._map())
+
+    def __repr__(self) -> str:
+        return repr(self._op) if self._op is not None else f"StoredOp(bytes {self._begin}..{self._end})"
+
+
 class StoredLedgerHistory:
-    """A stored ledger history.edn (a path or its bytes) that the ledger checks read on the GPU (K18).
+    """A stored ledger history.edn (a path or its bytes) that the ledger checks read on the GPU (K18, K19).
 
     `_flat` asks it for the "bank", "ledger-counters" or "ledger-lookups" form and gets the device reader's FlatHistory,
-    read once per form and cached, instead of flattening op maps in Python.  Iterating it yields the op maps of
-    `edn.read_history` (parsed once, on first use, and cached), so the host-only checkers of a `ledger_checker()`
-    compose (unexpected-ops, final-reads, lookup-transfers, stats) still work, but they still pay the Python parse.
-    ctx: the native.Context to read on; None opens one on device 0 when the first form is asked for."""
+    read once per form and cached, instead of flattening op maps in Python.  The host checkers of a `ledger_checker()`
+    compose (unexpected-ops, final-reads, lookup-transfers) and stats build their results from one device summary
+    (`checks()`, K19), whose flagged ops are `StoredOp`s parsed only when read.  When the device refuses the file they
+    iterate it instead: iterating yields the op maps of `edn.read_history` (parsed once, on first use, and cached).
+    ctx: the native.Context to read on; None opens one on device 0 when the device is first needed."""
 
     def __init__(self, path_or_bytes, ctx=None) -> None:
         if isinstance(path_or_bytes, (bytes, bytearray, memoryview)):
-            self._data = bytes(path_or_bytes)
+            self.data = bytes(path_or_bytes)
         else:
             with open(path_or_bytes, "rb") as fh:
-                self._data = fh.read()
+                self.data = fh.read()
         self._ctx = ctx
         self._forms: dict[str, FlatHistory] = {}
         self._ops: list | None = None
+        self._checks: dict | None = None
+
+    def _context(self):
+        if self._ctx is None:
+            from .native import Context
+            self._ctx = Context(device=0)
+        return self._ctx
 
     def flat(self, form: str) -> FlatHistory:
         if form not in self._forms:
-            if self._ctx is None:
-                from .native import Context
-                self._ctx = Context(device=0)
-            self._forms[form] = self._ctx.read_ledger_edn(self._data, form)
+            self._forms[form] = self._context().read_ledger_edn(self.data, form)
         return self._forms[form]
+
+    def checks(self) -> dict | None:
+        """The device summary the host checkers use (`Context.ledger_edn_checks`), computed once; None when the device
+        refused the file."""
+        if self._checks is None:
+            self._checks = self._context().ledger_edn_checks(self.data)
+        return None if self._checks["refused"] else self._checks
 
     def ops(self) -> list:
         if self._ops is None:
             from .edn import read_history
-            self._ops = read_history(self._data.decode())
+            self._ops = read_history(self.data.decode())
         return self._ops
 
     def __iter__(self):
@@ -98,6 +144,14 @@ class StoredLedgerHistory:
 
     def __getitem__(self, i):
         return self.ops()[i]
+
+
+def _summary(history) -> dict | None:
+    return history.checks() if isinstance(history, StoredLedgerHistory) else None
+
+
+def _stored(data: bytes, rec) -> StoredOp:
+    return StoredOp(data, rec["begin"], rec["end"])
 
 
 def _flat(history, model: str) -> FlatHistory:
@@ -987,6 +1041,9 @@ class UnexpectedOps(Checker):
     result :unknown ({:valid? :unknown :open-ops [...] :fail-ops [...]})."""
 
     def check(self, test, history, opts=None) -> dict:
+        s = _summary(history)
+        if s is not None:
+            return self.from_summary(s, history.data)
         hist = [op for op in history if _is_client(op)]
         end_time = _g(hist[-1], "time", 0) if hist else 0
         open_by_process: dict = {}
@@ -1007,12 +1064,31 @@ class UnexpectedOps(Checker):
             out.update({"valid?": "unknown", "fail-ops": fails})
         return out
 
+    @staticmethod
+    def from_summary(s: Mapping[str, Any], data: bytes) -> dict:
+        """The result from a stored history's device summary (`Context.ledger_edn_checks`) and its bytes; an absent
+        :time or :index is 0 in the records, as `_g` reads it."""
+        end_time = int(s["last"]["time"]) if s["last"] is not None else 0
+        open_recs = sorted(s["open"], key=lambda r: int(r["first"]))   # the order processes enter open_by_process
+        open_recs = sorted(open_recs, key=lambda r: int(r["index"]))
+        opens = [[(end_time - int(r["time"])) / 1e6, _stored(data, r)] for r in open_recs][::-1]
+        fails = [_stored(data, r) for r in s["fails"]]
+        out: dict = {"valid?": True}
+        if opens:
+            out.update({"valid?": "unknown", "open-ops": opens})
+        if fails:
+            out.update({"valid?": "unknown", "fail-ops": fails})
+        return out
+
 
 class LookupAllInvokedTransfers(Checker):
     """`(lookup-all-invoked-transfers)` — tests/ledger.clj:222-252: every :final? :ok :l-t lookup must
     contain the id of every invoked transfer."""
 
     def check(self, test, history, opts=None) -> dict:
+        s = _summary(history)
+        if s is not None:
+            return self.from_summary(s, history.data)
         hist = [op for op in history if _is_client(op)]
         invoked = set()
         for op in hist:
@@ -1030,12 +1106,23 @@ class LookupAllInvokedTransfers(Checker):
             out.update({"valid?": False, "suspect-final-lookups": suspects})
         return out
 
+    @staticmethod
+    def from_summary(s: Mapping[str, Any], data: bytes) -> dict:
+        suspects = [_stored(data, r) for r in s["final_lookups"] if r["suspect"]]
+        out: dict = {"valid?": True}
+        if suspects:
+            out.update({"valid?": False, "suspect-final-lookups": suspects})
+        return out
+
 
 class FinalReads(Checker):
     """`(final-reads)` — tests/ledger.clj:254-282: final reads (and final :l-t lookups) must exist and be
     all equal: exactly one distinct :value among the :final? :ok :r ops, and among the :l-t ones."""
 
     def check(self, test, history, opts=None) -> dict:
+        s = _summary(history)
+        if s is not None:
+            return self.from_summary(s, history.data)
         hist = [op for op in history if _is_client(op)]
 
         def finals(tag):
@@ -1050,6 +1137,25 @@ class FinalReads(Checker):
             out.update({"valid?": False, "unequal-final-lookups": lookups})
         return out
 
+    @staticmethod
+    def from_summary(s: Mapping[str, Any], data: bytes) -> dict:
+        """Only when a kind does not have exactly one class are its values needed: one op per class is parsed."""
+        def finals(recs, n_classes):
+            first: dict = {}
+            for r in recs:
+                first.setdefault(int(r["cls"]), r)
+            values = {_freeze(_g(_stored(data, r), "value")) for r in first.values()}
+            assert len(values) == n_classes, (len(values), n_classes)
+            return values
+
+        out: dict = {"valid?": True}
+        if s["n_read_classes"] != 1:
+            out.update({"valid?": False, "unequal-final-reads": finals(s["final_reads"], s["n_read_classes"])})
+        if s["n_lookup_classes"] != 1:
+            out.update({"valid?": False,
+                        "unequal-final-lookups": finals(s["final_lookups"], s["n_lookup_classes"])})
+        return out
+
 
 class Stats(Checker):
     """`(checker/stats)` as composed at core.clj:144 [UPSTREAM-RECALL, jepsen.checker/stats]: success / failure counts of
@@ -1058,19 +1164,34 @@ class Stats(Checker):
     Host code, as in the reference (a linear pass over the history; nothing to put on a GPU)."""
 
     @staticmethod
+    def _counts(ok: int, fail: int, info: int) -> dict:
+        return {"valid?": ok > 0, "count": ok + fail + info, "ok-count": ok, "fail-count": fail, "info-count": info}
+
+    @staticmethod
     def _tally(ops) -> dict:
         ok = sum(1 for o in ops if _kw(_g(o, "type")) == "ok")
         fail = sum(1 for o in ops if _kw(_g(o, "type")) == "fail")
         info = sum(1 for o in ops if _kw(_g(o, "type")) == "info")
-        return {"valid?": ok > 0, "count": ok + fail + info, "ok-count": ok, "fail-count": fail, "info-count": info}
+        return Stats._counts(ok, fail, info)
 
     def check(self, test, history, opts=None) -> dict:
+        s = _summary(history)
+        if s is not None:
+            return self.from_summary(s)
         done = [op for op in history if _is_client(op) and _kw(_g(op, "type")) != "invoke"]
         by_f: dict = {}
         for op in done:
             by_f.setdefault(_kw(_g(op, "f")), []).append(op)
         out = self._tally(done)
         out["by-f"] = {f: self._tally(ops) for f, ops in sorted(by_f.items(), key=lambda kv: str(kv[0]))}
+        out["valid?"] = merge_valid_bool([r["valid?"] for r in out["by-f"].values()])
+        return out
+
+    @staticmethod
+    def from_summary(s: Mapping[str, Any]) -> dict:
+        """Every client op of a stored ledger history is :f :txn (the device refuses others)."""
+        out = Stats._counts(s["n_ok"], s["n_fail"], s["n_info"])
+        out["by-f"] = {"txn": Stats._counts(s["n_ok"], s["n_fail"], s["n_info"])} if out["count"] else {}
         out["valid?"] = merge_valid_bool([r["valid?"] for r in out["by-f"].values()])
         return out
 

@@ -29,6 +29,7 @@
 #include "jtb_class_witness.cuh"
 #include "jtb_lookup_witness.cuh"
 #include "jtb_edn.cuh"
+#include "jtb_edn_checks.cuh"
 
 using namespace jtb;
 
@@ -755,6 +756,7 @@ long jtb_struct_size(int which) {
     case 30: return sizeof(jtb_lk_shard);
     case 31: return sizeof(jtb_lk_result);
     case 33: return sizeof(jtb_edn_history);
+    case 34: return sizeof(jtb_edn_checks);
     }
     return -1;
 }
@@ -1258,6 +1260,19 @@ int jtb_read_ledger_edn(jtb_ctx* ctx, const char* text, int64_t n_bytes, int32_t
 
 void jtb_edn_history_free(jtb_edn_history* out) {
     if (out) jtb_edn_history_release(out);
+}
+
+// K19: the host checks of a ledger compose on a stored history.edn (csrc/jtb_edn_checks.cuh)
+int jtb_ledger_edn_checks(jtb_ctx* ctx, const char* text, int64_t n_bytes, int32_t flags, jtb_edn_checks* out) {
+    if (!ctx) return -1;
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    if (cudaSetDevice(ctx->device) != cudaSuccess) { ctx->err = "cudaSetDevice failed"; return -1; }
+    ctx->fc.valid = false;
+    return run_ledger_edn_checks(ctx->stream, ctx->ev0, ctx->ev1, text, n_bytes, flags, out, ctx->err);
+}
+
+void jtb_edn_checks_free(jtb_edn_checks* out) {
+    if (out) jtb_edn_checks_release(out);
 }
 
 // SURVEY 8(f) N2: the step before the checkers (independent/subhistory, ledger->bank) on the device

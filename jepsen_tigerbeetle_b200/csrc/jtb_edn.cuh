@@ -727,69 +727,118 @@ inline unsigned edn_blocks(int64_t n, int threads = 256) {
     return (unsigned)std::max<int64_t>(1, std::min<int64_t>((n + threads - 1) / threads, INT_MAX));
 }
 
-// the host side of jtb_read_ledger_edn
-inline int run_read_ledger_edn(cudaStream_t st, cudaEvent_t ev0, cudaEvent_t ev1, const char* text, int64_t n,
-                               int32_t form, int32_t flags, jtb_edn_history* out, std::string& err) {
-    using Clock = std::chrono::steady_clock;
-    const auto t0 = Clock::now();
-    if (!out || n < 0 || (n > 0 && !text)) return input_error(err, "malformed arguments");
-    if (flags != 0) return input_error(err, "flags must be 0");
-    if (form != JTB_FORM_BANK && form != JTB_FORM_LEDGER_COUNTERS && form != JTB_FORM_LEDGER_LOOKUPS)
-        return input_error(err, "unknown form %d", (int)form);
-    std::memset(out, 0, sizeof *out);
+// The device state passes 1–5 leave behind, on one call's allocations, and the scratch they share with the passes
+// after them (the cub temporary storage grows as a later call needs more).  K18 (`run_read_ledger_edn`) and K19
+// (`run_ledger_edn_checks`, jtb_edn_checks.cuh) both start with `edn_parse`.
+struct EdnParse {
+    cudaStream_t st;
+    CallAllocs& A;
+    void* tmp = nullptr;
+    size_t tmp_cap = 0, bytes = 0;
+    int64_t* d_cnt = nullptr;           // 4 counters for reductions and selections
+    char* text = nullptr;               // the text, padded with 64 spaces
+    int64_t N = 0;                      // max(n, 1)
+    unsigned long long* err = nullptr;  // [0] the first error (byte << 8 | EdnErr), [1] multi-transfer txns
+    int base = 0;                       // the depth of the op maps (1: one vector of ops)
+    uint32_t* lv2 = nullptr;            // the brackets sorted by (level, position): levels ...
+    int64_t *br2 = nullptr, nb = 0;     // ... and positions; pairs (2k, 2k + 1) match
+    int64_t *ops = nullptr, n_ops = 0, *ch = nullptr, n_ch = 0, *it_pos = nullptr, n_it = 0;
+    int32_t* field = nullptr;           // per op and EK_*: the child index of the key's value + 1, 0 absent
+    EdnOp* op = nullptr;
+    EdnItem* items = nullptr;
+    int64_t* contrib = nullptr;
+    int32_t *cl = nullptr, *cl2 = nullptr, *key2 = nullptr;   // ledger-lookups: client ops in history order, sorted
+    int64_t n_cl = 0;                                         // by (process, position), and their processes
+    std::chrono::steady_clock::time_point t_h2d;              // when the text was on the device
+
+    EdnParse(cudaStream_t s, CallAllocs& a) : st(s), A(a) {}
+
+    cudaError_t need_tmp(size_t b) {   // grow the cub temporary storage
+        if (b <= tmp_cap) return cudaSuccess;
+        char* p;
+        const cudaError_t e = A.alloc(&p, b);
+        if (e == cudaSuccess) { tmp = p; tmp_cap = b; }
+        return e;
+    }
+    cudaError_t fetch(int64_t* dst, const int64_t* src) {
+        cudaError_t e = cudaMemcpyAsync(dst, src, 8, cudaMemcpyDeviceToHost, st);
+        return e == cudaSuccess ? cudaStreamSynchronize(st) : e;
+    }
+    cudaError_t error_word(unsigned long long* w) {
+        cudaError_t e = cudaMemcpyAsync(w, err, 8, cudaMemcpyDeviceToHost, st);
+        return e == cudaSuccess ? cudaStreamSynchronize(st) : e;
+    }
+    // how many of in[0, n_in) satisfy pred
+    template <class In, class Pred>
+    cudaError_t count(In in, int64_t n_in, Pred pred, int64_t* n_out) {
+        auto flags_it = thrust::make_transform_iterator(in, EdnCount<Pred>{pred});
+        cudaError_t e = cub::DeviceReduce::Sum(nullptr, bytes, flags_it, d_cnt, n_in, st);
+        if (e == cudaSuccess) e = need_tmp(bytes);
+        if (e == cudaSuccess) e = cub::DeviceReduce::Sum(tmp, bytes, flags_it, d_cnt, n_in, st);
+        return e == cudaSuccess ? fetch(n_out, d_cnt) : e;
+    }
+    // the elements of in[0, n_in) that satisfy pred, in order, into out (sized by count)
+    template <class In, class Out, class Pred>
+    cudaError_t select_into(In in, int64_t n_in, Pred pred, Out* out) {
+        cudaError_t e = cub::DeviceSelect::If(nullptr, bytes, in, out, d_cnt, n_in, pred, st);
+        if (e == cudaSuccess) e = need_tmp(bytes);
+        return e == cudaSuccess ? cub::DeviceSelect::If(tmp, bytes, in, out, d_cnt, n_in, pred, st) : e;
+    }
+    // count, then select into a buffer of that size
+    template <class In, class Pred>
+    cudaError_t select(In in, int64_t n_in, Pred pred, int64_t** outp, int64_t* n_out) {
+        cudaError_t e = count(in, n_in, pred, n_out);
+        if (e == cudaSuccess) e = A.alloc(outp, (size_t)std::max<int64_t>(*n_out, 1));
+        return e == cudaSuccess ? select_into(in, n_in, pred, *outp) : e;
+    }
+};
+
+// Why the input was refused: a byte position (-1: none) and a reason; reason == nullptr when it was not.
+struct EdnRefusal {
+    int64_t at = -1;
+    const char* reason = nullptr;
+    void set(unsigned long long w) { at = (int64_t)(w >> 8); reason = edn_err_text((uint32_t)(w & 0xff)); }
+};
+
+// Passes 1–5 on text[0, n) read as `form`: the text copied to the device (P.t_h2d, then ev0 recorded), string state,
+// depth, bracket pairing, form starts, op keys and fields, micro-ops, tags, the per-process sort (ledger-lookups), and
+// the events' and payload's checks.  Returns 0 (r.reason set when the input is refused: the first error in the file) or
+// -1 with err on a CUDA or allocation error.
+inline int edn_parse(EdnParse& P, cudaEvent_t ev0, const char* text, int64_t n, int32_t form, EdnRefusal& r,
+                     std::string& err) {
+    cudaStream_t st = P.st;
+    CallAllocs& A = P.A;
     const int T = 256;
-    const int64_t N = std::max<int64_t>(n, 1);
-    CallAllocs A;
-    char* d_text;
-    unsigned long long* d_err;
-    JTB_OK(A.alloc(&d_text, (size_t)N + 64));
-    JTB_OK(A.alloc(&d_err, 2));
+    const int64_t N = P.N = std::max<int64_t>(n, 1);
+    JTB_OK(A.alloc(&P.text, (size_t)N + 64));
+    JTB_OK(A.alloc(&P.err, 2));
+    char* d_text = P.text;
+    unsigned long long* d_err = P.err;
     JTB_OK(cudaMemsetAsync(d_text, ' ', (size_t)N + 64, st));
     JTB_OK(cudaMemsetAsync(d_err, 0xff, 16, st));
     if (n) JTB_OK(cudaMemcpyAsync(d_text, text, (size_t)n, cudaMemcpyHostToDevice, st));
     JTB_OK(cudaStreamSynchronize(st));
-    const auto t1 = Clock::now();
+    P.t_h2d = std::chrono::steady_clock::now();
     JTB_OK(cudaEventRecord(ev0, st));
-
-    void* tmp = nullptr;
-    size_t tmp_cap = 0;
-    auto need_tmp = [&](size_t bytes) -> cudaError_t {   // grow the cub temporary storage
-        if (bytes <= tmp_cap) return cudaSuccess;
-        char* p;
-        const cudaError_t e = A.alloc(&p, bytes);
-        if (e == cudaSuccess) { tmp = p; tmp_cap = bytes; }
-        return e;
-    };
-    auto fetch = [&](int64_t* dst, const int64_t* src) -> cudaError_t {
-        cudaError_t e = cudaMemcpyAsync(dst, src, 8, cudaMemcpyDeviceToHost, st);
-        return e == cudaSuccess ? cudaStreamSynchronize(st) : e;
-    };
-    auto error_word = [&](unsigned long long* w) -> cudaError_t {
-        cudaError_t e = cudaMemcpyAsync(w, d_err, 8, cudaMemcpyDeviceToHost, st);
-        return e == cudaSuccess ? cudaStreamSynchronize(st) : e;
-    };
-    auto report = [&](unsigned long long w) -> int {
-        return input_error(err, "history.edn at byte %lld: %s", (long long)(w >> 8), edn_err_text((uint32_t)(w & 0xff)));
-    };
-    size_t bytes = 0;
+    size_t& bytes = P.bytes;
     unsigned long long w = ~0ull;
 
     // ---- 1, 2: string state, depth, byte checks, bracket pairing ----------------------------------------------------
     uint8_t* par;
     int* depth;
-    int64_t* d_cnt;
     JTB_OK(A.alloc(&par, (size_t)N));
     JTB_OK(A.alloc(&depth, (size_t)N));
-    JTB_OK(A.alloc(&d_cnt, 4));
+    JTB_OK(A.alloc(&P.d_cnt, 4));
+    int64_t* d_cnt = P.d_cnt;
     auto cnt = thrust::counting_iterator<int64_t>(0);
     auto quotes = thrust::make_transform_iterator(cnt, EdnQuote{d_text});
     auto deltas = thrust::make_transform_iterator(cnt, EdnDelta{d_text, par});
     JTB_OK(cub::DeviceScan::InclusiveScan(nullptr, bytes, quotes, par, EdnXor{}, N, st));
-    JTB_OK(need_tmp(bytes));
-    JTB_OK(cub::DeviceScan::InclusiveScan(tmp, bytes, quotes, par, EdnXor{}, N, st));
+    JTB_OK(P.need_tmp(bytes));
+    JTB_OK(cub::DeviceScan::InclusiveScan(P.tmp, bytes, quotes, par, EdnXor{}, N, st));
     JTB_OK(cub::DeviceScan::InclusiveSum(nullptr, bytes, deltas, depth, N, st));
-    JTB_OK(need_tmp(bytes));
-    JTB_OK(cub::DeviceScan::InclusiveSum(tmp, bytes, deltas, depth, N, st));
+    JTB_OK(P.need_tmp(bytes));
+    JTB_OK(cub::DeviceScan::InclusiveSum(P.tmp, bytes, deltas, depth, N, st));
     edn_byte_check_kernel<<<edn_blocks(N / 4), T, 0, st>>>(d_text, par, depth, N, d_err);
     JTB_OK(cudaGetLastError());
     {
@@ -797,55 +846,42 @@ inline int run_read_ledger_edn(cudaStream_t st, cudaEvent_t ev0, cudaEvent_t ev1
         int last_depth = 0;
         JTB_OK(cudaMemcpyAsync(&last_par, par + N - 1, 1, cudaMemcpyDeviceToHost, st));
         JTB_OK(cudaMemcpyAsync(&last_depth, depth + N - 1, 4, cudaMemcpyDeviceToHost, st));
-        JTB_OK(error_word(&w));
-        if (w != ~0ull) return report(w);
-        if (last_par) return input_error(err, "history.edn: unterminated string");
-        if (last_depth != 0) return input_error(err, "history.edn: unbalanced brackets");
+        JTB_OK(P.error_word(&w));
+        if (w != ~0ull) { r.set(w); return 0; }
+        if (last_par) { r.reason = "unterminated string"; return 0; }
+        if (last_depth != 0) { r.reason = "unbalanced brackets"; return 0; }
     }
-    // ---- selections: count, then select into a buffer of that size ---------------------------------------------------
-    auto select = [&](auto in, int64_t n_in, auto pred, int64_t** outp, int64_t* n_out) -> cudaError_t {
-        auto flags_it = thrust::make_transform_iterator(in, EdnCount<decltype(pred)>{pred});
-        cudaError_t e = cub::DeviceReduce::Sum(nullptr, bytes, flags_it, d_cnt, n_in, st);
-        if (e == cudaSuccess) e = need_tmp(bytes);
-        if (e == cudaSuccess) e = cub::DeviceReduce::Sum(tmp, bytes, flags_it, d_cnt, n_in, st);
-        if (e == cudaSuccess) e = fetch(n_out, d_cnt);
-        if (e == cudaSuccess) e = A.alloc(outp, (size_t)std::max<int64_t>(*n_out, 1));
-        if (e == cudaSuccess) e = cub::DeviceSelect::If(nullptr, bytes, in, *outp, d_cnt, n_in, pred, st);
-        if (e == cudaSuccess) e = need_tmp(bytes);
-        if (e == cudaSuccess) e = cub::DeviceSelect::If(tmp, bytes, in, *outp, d_cnt, n_in, pred, st);
-        return e;
-    };
-    int64_t *br, nb = 0;
-    JTB_OK(select(cnt, N, EdnIsBracket{d_text, par}, &br, &nb));
+    int64_t* br;
+    JTB_OK(P.select(cnt, N, EdnIsBracket{d_text, par}, &br, &P.nb));
+    const int64_t nb = P.nb;
     if (nb) {
-        uint32_t *lv, *lv2;
-        int64_t* br2;
+        uint32_t* lv;
         JTB_OK(A.alloc(&lv, (size_t)nb));
-        JTB_OK(A.alloc(&lv2, (size_t)nb));
-        JTB_OK(A.alloc(&br2, (size_t)nb));
+        JTB_OK(A.alloc(&P.lv2, (size_t)nb));
+        JTB_OK(A.alloc(&P.br2, (size_t)nb));
         edn_bracket_level_kernel<<<edn_blocks(nb), T, 0, st>>>(d_text, depth, br, nb, lv);
         JTB_OK(cudaGetLastError());
         uint32_t* d_max = (uint32_t*)d_cnt;
         JTB_OK(cub::DeviceReduce::Max(nullptr, bytes, lv, d_max, nb, st));
-        JTB_OK(need_tmp(bytes));
-        JTB_OK(cub::DeviceReduce::Max(tmp, bytes, lv, d_max, nb, st));
+        JTB_OK(P.need_tmp(bytes));
+        JTB_OK(cub::DeviceReduce::Max(P.tmp, bytes, lv, d_max, nb, st));
         uint32_t max_level = 0;
         JTB_OK(cudaMemcpyAsync(&max_level, d_max, 4, cudaMemcpyDeviceToHost, st));
         JTB_OK(cudaStreamSynchronize(st));
         int end_bit = 1;
         while (end_bit < 32 && (max_level >> end_bit)) ++end_bit;
-        JTB_OK(cub::DeviceRadixSort::SortPairs(nullptr, bytes, lv, lv2, br, br2, nb, 0, end_bit, st));
-        JTB_OK(need_tmp(bytes));
-        JTB_OK(cub::DeviceRadixSort::SortPairs(tmp, bytes, lv, lv2, br, br2, nb, 0, end_bit, st));
-        edn_bracket_pair_kernel<<<edn_blocks((nb + 1) / 2), T, 0, st>>>(d_text, lv2, br2, nb, d_err);
+        JTB_OK(cub::DeviceRadixSort::SortPairs(nullptr, bytes, lv, P.lv2, br, P.br2, nb, 0, end_bit, st));
+        JTB_OK(P.need_tmp(bytes));
+        JTB_OK(cub::DeviceRadixSort::SortPairs(P.tmp, bytes, lv, P.lv2, br, P.br2, nb, 0, end_bit, st));
+        edn_bracket_pair_kernel<<<edn_blocks((nb + 1) / 2), T, 0, st>>>(d_text, P.lv2, P.br2, nb, d_err);
         JTB_OK(cudaGetLastError());
-        JTB_OK(error_word(&w));
-        if (w != ~0ull) return report(w);
+        JTB_OK(P.error_word(&w));
+        if (w != ~0ull) { r.set(w); return 0; }
     }
 
     // ---- 3: form starts, the base depth, ops, their children and micro-ops ------------------------------------------
     int64_t *forms, nf = 0;
-    JTB_OK(select(cnt, N, EdnFormStart{d_text, par, depth}, &forms, &nf));
+    JTB_OK(P.select(cnt, N, EdnFormStart{d_text, par, depth}, &forms, &nf));
     int base = 0;
     if (nf) {
         int* d_top = (int*)d_cnt;
@@ -863,25 +899,30 @@ inline int run_read_ledger_edn(cudaStream_t st, cudaEvent_t ev0, cudaEvent_t ev1
         JTB_OK(cudaStreamSynchronize(st));
         if (n_top == 1 && (first_c == '[' || first_c == '(') && before != '#') base = 1;   // one vector of ops
     }
-    int64_t *ops, n_ops = 0, *ch, n_ch = 0, *it_pos, n_it = 0;
-    JTB_OK(select(forms, nf, EdnAtDepth{d_text, depth, base}, &ops, &n_ops));
-    JTB_OK(select(forms, nf, EdnAtDepth{d_text, depth, base + 1}, &ch, &n_ch));
-    JTB_OK(select(forms, nf, EdnAtDepth{d_text, depth, base + 2}, &it_pos, &n_it));
-    if (n_ops >= INT_MAX || n_ch >= INT_MAX - 2 || n_it >= INT_MAX)
-        return input_error(err, "history.edn: more than 2^31 - 3 ops, map entries or micro-ops");
+    P.base = base;
+    JTB_OK(P.select(forms, nf, EdnAtDepth{d_text, depth, base}, &P.ops, &P.n_ops));
+    JTB_OK(P.select(forms, nf, EdnAtDepth{d_text, depth, base + 1}, &P.ch, &P.n_ch));
+    JTB_OK(P.select(forms, nf, EdnAtDepth{d_text, depth, base + 2}, &P.it_pos, &P.n_it));
+    const int64_t *ops = P.ops, *ch = P.ch, *it_pos = P.it_pos;
+    const int64_t n_ops = P.n_ops, n_ch = P.n_ch, n_it = P.n_it;
+    if (n_ops >= INT_MAX || n_ch >= INT_MAX - 2 || n_it >= INT_MAX) {
+        r.reason = "more than 2^31 - 3 ops, map entries or micro-ops";
+        return 0;
+    }
 
     // ---- 4: op keys and fields ----------------------------------------------------------------------------------------
-    int32_t *ch_op, *first_child, *n_child, *field;
-    EdnOp* op;
+    int32_t *ch_op, *first_child, *n_child;
     JTB_OK(A.alloc(&ch_op, (size_t)n_ch));
     JTB_OK(A.alloc(&first_child, (size_t)n_ops));
     JTB_OK(A.alloc(&n_child, (size_t)n_ops));
-    JTB_OK(A.alloc(&field, (size_t)n_ops * EK_N));
-    JTB_OK(A.alloc(&op, (size_t)n_ops));
+    JTB_OK(A.alloc(&P.field, (size_t)n_ops * EK_N));
+    JTB_OK(A.alloc(&P.op, (size_t)n_ops));
+    int32_t* field = P.field;
+    EdnOp* op = P.op;
     JTB_OK(cudaMemsetAsync(first_child, 0x7f, (size_t)n_ops * 4, st));
     JTB_OK(cudaMemsetAsync(n_child, 0, (size_t)n_ops * 4, st));
     JTB_OK(cudaMemsetAsync(field, 0, (size_t)n_ops * EK_N * 4, st));
-    unsigned long long* d_multi = (unsigned long long*)d_err + 1;
+    unsigned long long* d_multi = d_err + 1;
     JTB_OK(cudaMemsetAsync(d_multi, 0, 8, st));
     if (n_ops) {
         if (n_ch) {
@@ -893,10 +934,9 @@ inline int run_read_ledger_edn(cudaStream_t st, cudaEvent_t ev0, cudaEvent_t ev1
     }
 
     // ---- 5: micro-ops, tags, pending tags, payload --------------------------------------------------------------------
-    EdnItem* items;
-    int64_t* contrib;
-    JTB_OK(A.alloc(&items, (size_t)n_it));
-    JTB_OK(A.alloc(&contrib, (size_t)n_it));
+    JTB_OK(A.alloc(&P.items, (size_t)n_it));
+    JTB_OK(A.alloc(&P.contrib, (size_t)n_it));
+    EdnItem* items = P.items;
     if (n_ops) {
         if (n_it)
             edn_item_kernel<<<edn_blocks(n_it), T, 0, st>>>(d_text, N, ops, n_ops, ch, n_ch, it_pos, n_it, op, items,
@@ -906,34 +946,63 @@ inline int run_read_ledger_edn(cudaStream_t st, cudaEvent_t ev0, cudaEvent_t ev1
     }
     if (form == JTB_FORM_LEDGER_LOOKUPS && n_ops) {
         int64_t* d_ncl = d_cnt + 1;
-        int32_t *cl, *cl2, *key, *key2;
-        JTB_OK(A.alloc(&cl, (size_t)n_ops));
-        JTB_OK(A.alloc(&cl2, (size_t)n_ops));
+        int32_t *key;
+        JTB_OK(A.alloc(&P.cl, (size_t)n_ops));
+        JTB_OK(A.alloc(&P.cl2, (size_t)n_ops));
         JTB_OK(A.alloc(&key, (size_t)n_ops));
-        JTB_OK(A.alloc(&key2, (size_t)n_ops));
+        JTB_OK(A.alloc(&P.key2, (size_t)n_ops));
         auto ci = thrust::counting_iterator<int32_t>(0);
-        JTB_OK(cub::DeviceSelect::If(nullptr, bytes, ci, cl, d_ncl, n_ops, EdnIsClient{op}, st));
-        JTB_OK(need_tmp(bytes));
-        JTB_OK(cub::DeviceSelect::If(tmp, bytes, ci, cl, d_ncl, n_ops, EdnIsClient{op}, st));
-        int64_t n_cl = 0;
-        JTB_OK(fetch(&n_cl, d_ncl));
+        JTB_OK(cub::DeviceSelect::If(nullptr, bytes, ci, P.cl, d_ncl, n_ops, EdnIsClient{op}, st));
+        JTB_OK(P.need_tmp(bytes));
+        JTB_OK(cub::DeviceSelect::If(P.tmp, bytes, ci, P.cl, d_ncl, n_ops, EdnIsClient{op}, st));
+        JTB_OK(P.fetch(&P.n_cl, d_ncl));
+        const int64_t n_cl = P.n_cl;
         if (n_cl) {
-            edn_proc_key_kernel<<<edn_blocks(n_cl), T, 0, st>>>(op, cl, n_cl, key);
+            edn_proc_key_kernel<<<edn_blocks(n_cl), T, 0, st>>>(op, P.cl, n_cl, key);
             JTB_OK(cudaGetLastError());
-            JTB_OK(cub::DeviceRadixSort::SortPairs(nullptr, bytes, key, key2, cl, cl2, n_cl, 0, 32, st));
-            JTB_OK(need_tmp(bytes));
-            JTB_OK(cub::DeviceRadixSort::SortPairs(tmp, bytes, key, key2, cl, cl2, n_cl, 0, 32, st));
-            edn_pending_kernel<<<edn_blocks(n_cl), T, 0, st>>>(ops, op, key2, cl2, n_cl, d_err);
+            JTB_OK(cub::DeviceRadixSort::SortPairs(nullptr, bytes, key, P.key2, P.cl, P.cl2, n_cl, 0, 32, st));
+            JTB_OK(P.need_tmp(bytes));
+            JTB_OK(cub::DeviceRadixSort::SortPairs(P.tmp, bytes, key, P.key2, P.cl, P.cl2, n_cl, 0, 32, st));
+            edn_pending_kernel<<<edn_blocks(n_cl), T, 0, st>>>(ops, op, P.key2, P.cl2, n_cl, d_err);
             JTB_OK(cudaGetLastError());
         }
     }
     if (n_ops) {
         edn_event_kernel<<<edn_blocks(n_ops), T, 0, st>>>(ops, n_ops, op, items, it_pos, form, d_err, d_multi);
-        if (n_it) edn_contrib_kernel<<<edn_blocks(n_it), T, 0, st>>>(it_pos, items, n_it, op, contrib, d_err);
+        if (n_it) edn_contrib_kernel<<<edn_blocks(n_it), T, 0, st>>>(it_pos, items, n_it, op, P.contrib, d_err);
         JTB_OK(cudaGetLastError());
     }
-    JTB_OK(error_word(&w));
-    if (w != ~0ull) return report(w);
+    JTB_OK(P.error_word(&w));
+    if (w != ~0ull) r.set(w);
+    return 0;
+}
+
+// the host side of jtb_read_ledger_edn
+inline int run_read_ledger_edn(cudaStream_t st, cudaEvent_t ev0, cudaEvent_t ev1, const char* text, int64_t n,
+                               int32_t form, int32_t flags, jtb_edn_history* out, std::string& err) {
+    using Clock = std::chrono::steady_clock;
+    const auto t0 = Clock::now();
+    if (!out || n < 0 || (n > 0 && !text)) return input_error(err, "malformed arguments");
+    if (flags != 0) return input_error(err, "flags must be 0");
+    if (form != JTB_FORM_BANK && form != JTB_FORM_LEDGER_COUNTERS && form != JTB_FORM_LEDGER_LOOKUPS)
+        return input_error(err, "unknown form %d", (int)form);
+    std::memset(out, 0, sizeof *out);
+    const int T = 256;
+    CallAllocs A;
+    EdnParse P(st, A);
+    EdnRefusal r;
+    if (edn_parse(P, ev0, text, n, form, r, err) != 0) return -1;
+    if (r.reason) {
+        if (r.at >= 0) return input_error(err, "history.edn at byte %lld: %s", (long long)r.at, r.reason);
+        return input_error(err, "history.edn: %s", r.reason);
+    }
+    const auto t1 = P.t_h2d;
+    size_t& bytes = P.bytes;
+    const int64_t n_ops = P.n_ops, n_it = P.n_it;
+    EdnOp* op = P.op;
+    EdnItem* items = P.items;
+    int64_t* contrib = P.contrib;
+    unsigned long long* d_multi = P.err + 1;
 
     int64_t *ev_incl, *poff_incl, *it_incl, n_events = 0, n_payload = 0;
     JTB_OK(A.alloc(&ev_incl, (size_t)n_ops));
@@ -944,18 +1013,18 @@ inline int run_read_ledger_edn(cudaStream_t st, cudaEvent_t ev0, cudaEvent_t ev1
         auto keep = thrust::make_transform_iterator(oi, EdnKeep{op});
         auto plen = thrust::make_transform_iterator(oi, EdnPlen{op});
         JTB_OK(cub::DeviceScan::InclusiveSum(nullptr, bytes, keep, ev_incl, n_ops, st));
-        JTB_OK(need_tmp(bytes));
-        JTB_OK(cub::DeviceScan::InclusiveSum(tmp, bytes, keep, ev_incl, n_ops, st));
+        JTB_OK(P.need_tmp(bytes));
+        JTB_OK(cub::DeviceScan::InclusiveSum(P.tmp, bytes, keep, ev_incl, n_ops, st));
         JTB_OK(cub::DeviceScan::InclusiveSum(nullptr, bytes, plen, poff_incl, n_ops, st));
-        JTB_OK(need_tmp(bytes));
-        JTB_OK(cub::DeviceScan::InclusiveSum(tmp, bytes, plen, poff_incl, n_ops, st));
-        JTB_OK(fetch(&n_events, ev_incl + n_ops - 1));
-        JTB_OK(fetch(&n_payload, poff_incl + n_ops - 1));
+        JTB_OK(P.need_tmp(bytes));
+        JTB_OK(cub::DeviceScan::InclusiveSum(P.tmp, bytes, plen, poff_incl, n_ops, st));
+        JTB_OK(P.fetch(&n_events, ev_incl + n_ops - 1));
+        JTB_OK(P.fetch(&n_payload, poff_incl + n_ops - 1));
     }
     if (n_it) {
         JTB_OK(cub::DeviceScan::InclusiveSum(nullptr, bytes, contrib, it_incl, n_it, st));
-        JTB_OK(need_tmp(bytes));
-        JTB_OK(cub::DeviceScan::InclusiveSum(tmp, bytes, contrib, it_incl, n_it, st));
+        JTB_OK(P.need_tmp(bytes));
+        JTB_OK(cub::DeviceScan::InclusiveSum(P.tmp, bytes, contrib, it_incl, n_it, st));
     }
     EdnEvents e;
     int32_t* d_pl;

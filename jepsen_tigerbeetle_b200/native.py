@@ -21,7 +21,7 @@ _DEPS = _SOURCES + ["jtb_prep.h", "jtb_expand.h", "jtb_wgl.cuh", "jtb_scout.cuh"
                     "jtb_table_bench.cuh", "jtb_level.cuh", "jtb_partition.cuh", "jtb_monotonic.cuh",
                     "jtb_counter_bounds.cuh", "jtb_transfer_lookups.cuh", "jtb_read_explanations.cuh",
                     "jtb_read_gaps.cuh", "jtb_transfer_placement.cuh", "jtb_serial_witness.cuh", "jtb_repaired_witness.cuh",
-                    "jtb_lifted_witness.cuh", "jtb_class_witness.cuh", "jtb_lookup_witness.cuh", "jtb_edn.cuh", "jtb_call.cuh"]
+                    "jtb_lifted_witness.cuh", "jtb_class_witness.cuh", "jtb_lookup_witness.cuh", "jtb_edn.cuh", "jtb_edn_checks.cuh", "jtb_call.cuh"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared", "-ldl"]
 
@@ -31,6 +31,7 @@ EXPORTS = ["jtb_abi_version", "jtb_device_count", "jtb_create", "jtb_destroy", "
            "jtb_check_read_gaps", "jtb_check_transfer_placement", "jtb_check_serial_witness",
            "jtb_check_repaired_witness", "jtb_check_lifted_witness", "jtb_check_class_witness",
            "jtb_check_lookup_witness", "jtb_read_ledger_edn", "jtb_edn_history_free",
+           "jtb_ledger_edn_checks", "jtb_edn_checks_free",
            "jtb_table_bench", "jtb_get_stats", "jtb_struct_size", "jtb_prepare_seconds", "jtb_prepare_info",
            "jtb_final_configs", "jtb_gather_bench", "jtb_host_alloc", "jtb_host_free", "jtb_partition_by_key", "jtb_ledger_balances", "jtb_multi_create", "jtb_multi_create_error", "jtb_multi_destroy", "jtb_multi_n_gpus",
            "jtb_multi_last_error", "jtb_multi_check_linearizable", "jtb_multi_check_set_full"]
@@ -100,6 +101,8 @@ def lib() -> C.CDLL:
                                                    C.c_void_p]
             L.jtb_read_ledger_edn.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_void_p]
             L.jtb_edn_history_free.argtypes = [C.c_void_p]
+            L.jtb_ledger_edn_checks.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p]
+            L.jtb_edn_checks_free.argtypes = [C.c_void_p]
             L.jtb_table_bench.argtypes = [C.c_void_p, C.c_uint64, C.c_int, C.c_int, C.c_void_p,
                                           C.c_void_p, C.c_void_p]
             L.jtb_gather_bench.argtypes = [C.c_void_p, C.c_uint64, C.c_int, C.c_int, C.c_uint32, C.c_int, C.c_int,
@@ -436,6 +439,42 @@ class Context:
                            seconds_d2h=out.seconds_d2h, seconds_total=out.seconds_total, n_ops=out.n_ops)
         return _owned_flat(out, form)
 
+    # ---- K19: the host checks of a ledger compose on a stored history.edn -----------------------------------------
+    def ledger_edn_checks(self, data) -> dict:
+        """The bytes of a Jepsen history.edn (bytes, bytearray, memoryview, or a path) summarised on the device for the
+        checkers unexpected-ops, lookup-all-invoked-transfers, final-reads and stats (`jtb_ledger_edn_checks`):
+        {"refused": None, or {"at": byte or -1, "reason": str} when the device cannot answer exactly as those checkers
+        would; the counts of abi.EDN_CHECKS_COUNTS; "last": the last client op's record or None; "open", "fails",
+        "final_reads", "final_lookups": numpy arrays of abi.EDN_FLAG_DTYPE records in page-locked memory, released when
+        the last of them is gone; seconds_h2d, seconds_kernel, seconds_d2h, seconds_total}."""
+        import numpy as np
+        if isinstance(data, (str, os.PathLike)):
+            with open(data, "rb") as fh:
+                data = fh.read()
+        if not isinstance(data, bytes):
+            data = bytes(data)
+        keep = C.c_char_p(data)
+        out = abi.CEdnChecks()
+        rc = lib().jtb_ledger_edn_checks(self._h, C.cast(keep, C.c_void_p), len(data), 0, C.addressof(out))
+        if rc != 0:
+            raise NativeError(f"jtb_ledger_edn_checks rc={rc}: {self._err()}")
+        r = {name: int(getattr(out, name)) for name in abi.EDN_CHECKS_COUNTS}
+        r.update(seconds_h2d=out.seconds_h2d, seconds_kernel=out.seconds_kernel, seconds_d2h=out.seconds_d2h,
+                 seconds_total=out.seconds_total, refused=None, last=None)
+        dt = np.dtype(abi.EDN_FLAG_DTYPE)
+        if out.refused:
+            r["refused"] = {"at": int(out.refused_at), "reason": out.refused_reason.decode()}
+            empty = np.zeros(0, dt)
+            r.update(open=empty, fails=empty, final_reads=empty, final_lookups=empty)
+            return r
+        if out.last.op >= 0:
+            r["last"] = np.frombuffer(bytes(out.last), dt)[0]
+        owner = _EdnArrays(out, "jtb_edn_checks_free")
+        for name, n in (("open", out.n_open), ("fails", out.n_fail), ("final_reads", out.n_final_reads),
+                        ("final_lookups", out.n_final_lookups)):
+            r[name] = owner.view(getattr(out, name), dt, n)
+        return r
+
     def final_configs(self, h: FlatHistory, model: CModel, shard: int = 0, cap: int = 10) -> dict:
         """knossos' :configs of an INVALID shard (`jtb_final_configs`): call directly after `check_linearizable`
         on the same history.  Returns {"total": all such configurations, "configs": the first `cap` of them}."""
@@ -586,10 +625,11 @@ def prepare_info(h: FlatHistory, model: CModel) -> dict:
 
 
 class _EdnArrays:
-    """The page-locked arrays of one jtb_edn_history, released when the last numpy view of them is gone."""
+    """The page-locked arrays of one jtb_edn_history (or, with free="jtb_edn_checks_free", one jtb_edn_checks),
+    released when the last numpy view of them is gone."""
 
-    def __init__(self, out) -> None:
-        self.out, self.live = out, 0
+    def __init__(self, out, free: str = "jtb_edn_history_free") -> None:
+        self.out, self.live, self.free = out, 0, free
 
     def view(self, ptr, dtype, n):
         import weakref
@@ -605,7 +645,7 @@ class _EdnArrays:
     def _drop(self) -> None:
         self.live -= 1
         if self.live == 0 and _lib is not None:
-            _lib.jtb_edn_history_free(C.addressof(self.out))
+            getattr(_lib, self.free)(C.addressof(self.out))
 
 
 def _owned_flat(out, form: str) -> FlatHistory:
