@@ -342,19 +342,24 @@ class CSwResult(C.Structure):
                 ("seconds_total", C.c_double)]
 
 
-SW_SHARD_FIELDS = ("valid", "cause", "n_reads", "n_transfers", "n_committed", "n_committed_crashed", "n_after", "nodes",
-                   "rounds", "fail_index", "transfer_id")
-SW_RESULT_FIELDS = ("valid", "n_failures", "n_reads", "n_transfers", "n_committed", "n_committed_crashed", "n_after",
-                    "nodes", "rounds", "seconds_kernel", "seconds_total")
+def _names(struct) -> tuple:
+    return tuple(f for f, _ in struct._fields_)
 
 
-def sw_to_dict(res, shards, commit_read=None) -> dict:
-    """One result dict for the library and the oracle; "commit_read" (a numpy int32 array, one entry per transfer
-    micro-op in history order) when it was asked for."""
-    out = {f: getattr(res, f) for f in SW_RESULT_FIELDS}
-    out["shards"] = [{f: getattr(s, f) for f in SW_SHARD_FIELDS} for s in shards]
+SW_SHARD_FIELDS = _names(CSwShard)
+SW_RESULT_FIELDS = _names(CSwResult)
+
+
+def witness_to_dict(res, shards, commit_read=None, lookup_read=None) -> dict:
+    """One result dict of a witness check (jtb_sw_* .. jtb_lk_*, K13-K17) for the library and the oracle: the
+    result's fields and "shards" with each shard's; "commit_read" (a numpy int32 array, one entry per transfer micro-op
+    in history order) and "lookup_read" (one entry per :ok lookup in history order) when they were asked for."""
+    out = {f: getattr(res, f) for f, _ in res._fields_}
+    out["shards"] = [{f: getattr(s, f) for f, _ in s._fields_} for s in shards]
     if commit_read is not None:
         out["commit_read"] = commit_read
+    if lookup_read is not None:
+        out["lookup_read"] = lookup_read
     return out
 
 
@@ -370,17 +375,8 @@ class CRwResult(C.Structure):
     _fields_ = CSwResult._fields_[:9] + [("repairs", C.c_int64), ("n_bans", C.c_int64)] + CSwResult._fields_[9:]
 
 
-RW_SHARD_FIELDS = SW_SHARD_FIELDS + ("repairs", "n_bans")
-RW_RESULT_FIELDS = SW_RESULT_FIELDS[:9] + ("repairs", "n_bans") + SW_RESULT_FIELDS[9:]
-
-
-def rw_to_dict(res, shards, commit_read=None) -> dict:
-    """As sw_to_dict, for jtb_rw_result / jtb_rw_shard."""
-    out = {f: getattr(res, f) for f in RW_RESULT_FIELDS}
-    out["shards"] = [{f: getattr(s, f) for f in RW_SHARD_FIELDS} for s in shards]
-    if commit_read is not None:
-        out["commit_read"] = commit_read
-    return out
+RW_SHARD_FIELDS = _names(CRwShard)
+RW_RESULT_FIELDS = _names(CRwResult)
 
 
 LW_DEFAULT_MAX_LIFTS = 32
@@ -395,17 +391,8 @@ class CLwResult(C.Structure):
     _fields_ = CRwResult._fields_[:11] + [("lifts", C.c_int64), ("n_lifted", C.c_int64)] + CRwResult._fields_[11:]
 
 
-LW_SHARD_FIELDS = RW_SHARD_FIELDS + ("lifts", "n_lifted")
-LW_RESULT_FIELDS = RW_RESULT_FIELDS[:11] + ("lifts", "n_lifted") + RW_RESULT_FIELDS[11:]
-
-
-def lw_to_dict(res, shards, commit_read=None) -> dict:
-    """As sw_to_dict, for jtb_lw_result / jtb_lw_shard."""
-    out = {f: getattr(res, f) for f in LW_RESULT_FIELDS}
-    out["shards"] = [{f: getattr(s, f) for f in LW_SHARD_FIELDS} for s in shards]
-    if commit_read is not None:
-        out["commit_read"] = commit_read
-    return out
+LW_SHARD_FIELDS = _names(CLwShard)
+LW_RESULT_FIELDS = _names(CLwResult)
 
 
 class CCwShard(C.Structure):
@@ -418,17 +405,8 @@ class CCwResult(C.Structure):
         CLwResult._fields_[13:]
 
 
-CW_SHARD_FIELDS = LW_SHARD_FIELDS + ("class_cause", "class_rounds", "n_handed")
-CW_RESULT_FIELDS = LW_RESULT_FIELDS[:13] + ("class_rounds", "n_handed") + LW_RESULT_FIELDS[13:]
-
-
-def cw_to_dict(res, shards, commit_read=None) -> dict:
-    """As sw_to_dict, for jtb_cw_result / jtb_cw_shard."""
-    out = {f: getattr(res, f) for f in CW_RESULT_FIELDS}
-    out["shards"] = [{f: getattr(s, f) for f in CW_SHARD_FIELDS} for s in shards]
-    if commit_read is not None:
-        out["commit_read"] = commit_read
-    return out
+CW_SHARD_FIELDS = _names(CCwShard)
+CW_RESULT_FIELDS = _names(CCwResult)
 
 
 class CLkShard(C.Structure):
@@ -442,20 +420,8 @@ class CLkResult(C.Structure):
 
 
 CAUSE_LOOKUP = 9
-LK_SHARD_FIELDS = CW_SHARD_FIELDS + ("lookup_cause", "lookup_fail_index", "n_lookups_placed")
-LK_RESULT_FIELDS = CW_RESULT_FIELDS[:15] + ("n_lookups_placed",) + CW_RESULT_FIELDS[15:]
-
-
-def lk_to_dict(res, shards, commit_read=None, lookup_read=None) -> dict:
-    """As sw_to_dict, for jtb_lk_result / jtb_lk_shard; "lookup_read" (one entry per :ok lookup in history order) when
-    it was asked for."""
-    out = {f: getattr(res, f) for f in LK_RESULT_FIELDS}
-    out["shards"] = [{f: getattr(s, f) for f in LK_SHARD_FIELDS} for s in shards]
-    if commit_read is not None:
-        out["commit_read"] = commit_read
-    if lookup_read is not None:
-        out["lookup_read"] = lookup_read
-    return out
+LK_SHARD_FIELDS = _names(CLkShard)
+LK_RESULT_FIELDS = _names(CLkResult)
 
 
 def n_ok_lookups(h) -> int:
@@ -482,7 +448,6 @@ class CEdnHistory(C.Structure):
     _fields_ = [("history", CHistory), ("multi_transfer_txns", C.c_int64), ("n_ops", C.c_int64),
                 ("seconds_h2d", C.c_double), ("seconds_kernel", C.c_double), ("seconds_d2h", C.c_double),
                 ("seconds_total", C.c_double)]
-
 
 
 # ---- K19: the host checks of a ledger compose on a stored history.edn ----------------------------------------------

@@ -28,6 +28,7 @@
 #include "jtb_lifted_witness.cuh"
 #include "jtb_class_witness.cuh"
 #include "jtb_lookup_witness.cuh"
+#include "jtb_witness.cuh"
 #include "jtb_edn.cuh"
 #include "jtb_edn_checks.cuh"
 
@@ -1196,8 +1197,8 @@ int jtb_check_serial_witness(jtb_ctx* ctx, const jtb_history* h, int64_t max_nod
     std::lock_guard<std::mutex> lk(ctx->mu);
     if (cudaSetDevice(ctx->device) != cudaSuccess) { ctx->err = "cudaSetDevice failed"; return -1; }
     ctx->fc.valid = false;
-    return run_serial_witness(ctx->stream, ctx->ev0, ctx->ev1, h, max_nodes, max_rounds, flags, commit_read, shards,
-                              out, ctx->err);
+    return run_witness_as(ctx->stream, ctx->ev0, ctx->ev1, h, max_nodes, max_rounds, 0, 0, flags, commit_read, shards,
+                          out, ctx->err);
 }
 
 // K14: the repaired serial witness (csrc/jtb_repaired_witness.cuh)
@@ -1208,8 +1209,9 @@ int jtb_check_repaired_witness(jtb_ctx* ctx, const jtb_history* h, int64_t max_n
     std::lock_guard<std::mutex> lk(ctx->mu);
     if (cudaSetDevice(ctx->device) != cudaSuccess) { ctx->err = "cudaSetDevice failed"; return -1; }
     ctx->fc.valid = false;
-    return run_repaired_witness(ctx->stream, ctx->ev0, ctx->ev1, h, max_nodes, max_rounds, max_repairs, flags,
-                                commit_read, shards, out, ctx->err);
+    if (max_repairs <= 0) max_repairs = JTB_RW_DEFAULT_MAX_REPAIRS;
+    return run_witness_as(ctx->stream, ctx->ev0, ctx->ev1, h, max_nodes, max_rounds, max_repairs, 0, flags,
+                          commit_read, shards, out, ctx->err);
 }
 
 // K15: the lifted serial witness (csrc/jtb_lifted_witness.cuh)
@@ -1220,8 +1222,10 @@ int jtb_check_lifted_witness(jtb_ctx* ctx, const jtb_history* h, int64_t max_nod
     std::lock_guard<std::mutex> lk(ctx->mu);
     if (cudaSetDevice(ctx->device) != cudaSuccess) { ctx->err = "cudaSetDevice failed"; return -1; }
     ctx->fc.valid = false;
-    return run_lifted_witness(ctx->stream, ctx->ev0, ctx->ev1, h, max_nodes, max_rounds, max_repairs, max_lifts, flags,
-                              commit_read, shards, out, ctx->err);
+    if (max_repairs <= 0) max_repairs = JTB_RW_DEFAULT_MAX_REPAIRS;
+    if (max_lifts <= 0) max_lifts = JTB_LW_DEFAULT_MAX_LIFTS;
+    return run_witness_as(ctx->stream, ctx->ev0, ctx->ev1, h, max_nodes, max_rounds, max_repairs, max_lifts, flags,
+                          commit_read, shards, out, ctx->err);
 }
 
 // K16: the class witness (csrc/jtb_class_witness.cuh)
@@ -1232,8 +1236,10 @@ int jtb_check_class_witness(jtb_ctx* ctx, const jtb_history* h, int64_t max_node
     std::lock_guard<std::mutex> lk(ctx->mu);
     if (cudaSetDevice(ctx->device) != cudaSuccess) { ctx->err = "cudaSetDevice failed"; return -1; }
     ctx->fc.valid = false;
-    return run_class_witness(ctx->stream, ctx->ev0, ctx->ev1, h, max_nodes, max_rounds, max_repairs, max_lifts, flags,
-                             commit_read, shards, out, ctx->err);
+    if (max_repairs <= 0) max_repairs = JTB_RW_DEFAULT_MAX_REPAIRS;
+    if (max_lifts <= 0) max_lifts = JTB_LW_DEFAULT_MAX_LIFTS;
+    return run_witness_as(ctx->stream, ctx->ev0, ctx->ev1, h, max_nodes, max_rounds, max_repairs, max_lifts, flags,
+                          commit_read, shards, out, ctx->err, CwPass{});
 }
 
 // K17: the lookup witness (csrc/jtb_lookup_witness.cuh)
@@ -1244,8 +1250,12 @@ int jtb_check_lookup_witness(jtb_ctx* ctx, const jtb_history* h, int64_t max_nod
     std::lock_guard<std::mutex> lk(ctx->mu);
     if (cudaSetDevice(ctx->device) != cudaSuccess) { ctx->err = "cudaSetDevice failed"; return -1; }
     ctx->fc.valid = false;
-    return run_lookup_witness(ctx->stream, ctx->ev0, ctx->ev1, h, max_nodes, max_rounds, max_repairs, max_lifts, flags,
-                              commit_read, lookup_read, shards, out, ctx->err);
+    if (max_repairs <= 0) max_repairs = JTB_RW_DEFAULT_MAX_REPAIRS;
+    if (max_lifts <= 0) max_lifts = JTB_LW_DEFAULT_MAX_LIFTS;
+    LkPass pass;
+    pass.lookup_read = lookup_read;
+    return run_witness_as(ctx->stream, ctx->ev0, ctx->ev1, h, max_nodes, max_rounds, max_repairs, max_lifts, flags,
+                          commit_read, shards, out, ctx->err, pass);
 }
 
 // K18: a stored ledger history.edn read on the device (csrc/jtb_edn.cuh)

@@ -1,9 +1,9 @@
 // jtb_class_witness.cuh — K16: the class witness (K15's lifted serial witness, then a class pass on the shards it
 // leaves unproved, in which interchangeable crashed transfers are handed out earliest first) on the device.
 //
-// Semantics (include/jtb_check.h, DESIGN.md "K16 class witness").  K15 runs unchanged (run_repairs with CwPass as its
-// pass): pre snapshots K12's owners and owned counters after tp_finals; post runs the class pass on every shard K15
-// leaves UNKNOWN with cause UNDECIDED, NO_WITNESS or REAL_TIME, from the snapshot:
+// Semantics (include/jtb_check.h, DESIGN.md "K16 class witness").  K15 runs unchanged (run_witness, jtb_witness.cuh,
+// with CwPass as its pass): pre snapshots K12's owners and owned counters after tp_finals; post runs the class pass on
+// every shard K15 leaves UNKNOWN with cause UNDECIDED, NO_WITNESS or REAL_TIME, from the snapshot:
 //   - the classes, once: cw_keys, a thread per transfer, keys the crashed, windowed, unowned transfers of those shards
 //     by (shard, debit, credit, amount, M, A, invocation, id); one cub radix sort; cw_heads and a cub sum number the
 //     classes, and cw_classes gives each member its class and each class its first sorted position;
@@ -18,7 +18,7 @@
 //     failing gap of each class; cw_fix, a thread per gap, fixes the gaps before every failure of their classes;
 //     cw_own, a thread per record, gives the members to the gaps fixed.  The host reads one 8-byte pair per round (the
 //     gaps left, and the records of the next round, whose searches run before the read);
-//   - K13's real time, re-sum and commit_read (sw_tgap .. sw_commit) on the shards the rounds left live.
+//   - K13's real time, re-sum and commit_read (sw_real_time, sw_commit) on the shards the rounds left live.
 // The decision, node counts, rounds, class rounds, members handed out and commit_read equal the CW_SEARCH CPU test
 // oracle's.
 #pragma once
@@ -251,10 +251,11 @@ __global__ void cw_own(int32_t nrec, RgDev d, TpDev p, CwDev c, const unsigned l
 
 // ---- host ---------------------------------------------------------------------------------------------------------
 
-// K16's pass over K15's results (run_repairs' Pass)
+// K16's pass over K15's results (run_witness' Pass)
 struct CwPass {
     int32_t* owner0 = nullptr;   // K12's owners and owned counters, as tp_finals left them
     int64_t* own0 = nullptr;
+    std::vector<uint8_t> cok;    // per shard, after post: the class pass ran (K15 left it UNKNOWN, and not an anomaly)
 
     int pre(cudaStream_t st, TpStage& g, std::string& err) {
         JTB_OK(g.A.alloc(&owner0, g.nT)); JTB_OK(g.A.alloc(&own0, g.cells));
@@ -264,13 +265,13 @@ struct CwPass {
     }
 
     int post(cudaStream_t st, cudaEvent_t ev0, cudaEvent_t ev1, const jtb_history* h, TpStage& g, int32_t max_rounds,
-             jtb_cw_shard* shards, std::vector<int32_t>& cr_h, float& ms, std::string& err) {
+             jtb_lk_shard* shards, std::vector<int32_t>& cr_h, float& ms, std::string& err) {
         const int32_t S = g.S, nT = g.nT, m = g.m;
         const TlHost& T = g.T;
-        std::vector<uint8_t> cok(S, 0);
+        cok.assign(S, 0);
         bool any = false;
         for (int32_t s = 0; s < S; ++s) {
-            const jtb_cw_shard& o = shards[s];
+            const jtb_lk_shard& o = shards[s];
             any |= (cok[s] = g.dev[s] && o.valid == JTB_UNKNOWN &&
                              (o.cause == JTB_CAUSE_UNDECIDED || o.cause == JTB_CAUSE_NO_WITNESS ||
                               o.cause == JTB_CAUSE_REAL_TIME));
@@ -283,19 +284,13 @@ struct CwPass {
         JTB_OK(cudaMemcpyAsync(g.own, own0, (size_t)g.cells * 8, cudaMemcpyDeviceToDevice, st));
         SwDev w;
         CwDev c;
-        w.t_okcomp = g.d.t_okcomp;
-        std::vector<int32_t> rd_cidx(m);
-        for (int32_t i = 0; i < m; ++i) rd_cidx[i] = h->index[g.H.r_ev[g.d_of[i]]];
+        if (int rc = sw_alloc(st, g, cok, w, err)) return rc;
         const int32_t* d_cidx;
         int32_t *d_cr, *perm0, *perm, *head, *cno, *cls, *mcls, *chead, *un, *ur, *cmem, *cun, *roff, *words;
         CwKey *key0, *key;
         uint8_t* stmp;
-        JTB_OK(A.put(&w.sok, cok, st)); JTB_OK(A.put(&d_cidx, rd_cidx, st));
-        JTB_OK(A.alloc(&w.fixed, m)); JTB_OK(A.alloc(&w.cmin, nT)); JTB_OK(A.alloc(&w.sfail, S));
-        JTB_OK(A.alloc(&w.sunf, S)); JTB_OK(A.alloc(&w.unfixed, 1)); JTB_OK(A.alloc(&w.cnt, (size_t)S * SW_COUNTERS));
-        JTB_OK(A.alloc(&w.gmax, m)); JTB_OK(A.alloc(&w.gmin, m)); JTB_OK(A.alloc(&w.skey, m));
-        JTB_OK(A.alloc(&w.x, m)); JTB_OK(A.alloc(&w.P, m)); JTB_OK(A.alloc(&w.rtkey, S)); JTB_OK(A.alloc(&w.rtid, S));
-        JTB_OK(A.alloc(&w.bad, 1)); JTB_OK(A.alloc(&d_cr, nT));
+        const std::vector<int32_t> rd_cidx = sw_rd_cidx(h, g);
+        JTB_OK(A.put(&d_cidx, rd_cidx, st)); JTB_OK(A.alloc(&d_cr, nT));
         JTB_OK(A.alloc(&key0, nT)); JTB_OK(A.alloc(&key, nT)); JTB_OK(A.alloc(&perm0, nT)); JTB_OK(A.alloc(&perm, nT));
         JTB_OK(A.alloc(&head, nT)); JTB_OK(A.alloc(&cno, nT)); JTB_OK(A.alloc(&cls, nT)); JTB_OK(A.alloc(&mcls, nT));
         JTB_OK(A.alloc(&chead, nT)); JTB_OK(A.alloc(&un, nT)); JTB_OK(A.alloc(&ur, nT)); JTB_OK(A.alloc(&cmem, nT));
@@ -350,10 +345,6 @@ struct CwPass {
             JTB_OK(cudaStreamSynchronize(st));
             if (nm > 0) cw_classes<<<grid(nm, 256), 256, 0, st>>>(nm, perm, head, cno, cls, mcls, chead);
         }
-        JTB_OK(cudaMemsetAsync(w.sfail, 0x7f, (size_t)S * 4, st));   // RG_NONE
-        JTB_OK(cudaMemsetAsync(w.sunf, 0x7f, (size_t)S * 4, st));
-        JTB_OK(cudaMemsetAsync(w.cnt, 0, (size_t)S * SW_COUNTERS * 8, st));
-        JTB_OK(cudaMemsetAsync(w.unfixed, 0, 4, st));
         JTB_OK(cudaMemsetAsync(c.crounds, 0, (size_t)S * 4, st));
         JTB_OK(cudaMemsetAsync(c.handed, 0, (size_t)S * 4, st));
         sw_init<<<grid(m, 256), 256, 0, st>>>(x, p, w);
@@ -420,22 +411,8 @@ struct CwPass {
         }
         if (hw[0] > 0) sw_unfixed<<<grid(m, 256), 256, 0, st>>>(m, x, w);
         // real time and the counters, as K13
-        JTB_OK(cudaMemsetAsync(w.gmax, 0x80, (size_t)m * 4, st));   // INT_MIN
-        JTB_OK(cudaMemsetAsync(w.gmin, 0x7f, (size_t)m * 4, st));   // > every position
-        JTB_OK(cudaMemsetAsync(w.rtkey, 0xff, (size_t)S * 8, st));
-        JTB_OK(cudaMemsetAsync(w.rtid, 0xff, (size_t)S * 8, st));
-        JTB_OK(cudaMemsetAsync(w.bad, 0, 4, st));
-        JTB_OK(cudaMemsetAsync(g.own, 0, (size_t)g.cells * 8, st));
-        if (nT > 0) sw_tgap<<<grid(nT, 256), 256, 0, st>>>(x, p, w);
-        sw_scan_in<<<grid(m, 256), 256, 0, st>>>(x, w);
-        tb = stmp_bytes;
-        JTB_OK(cub::DeviceScan::InclusiveScanByKey(stmp, tb, w.skey, w.x, w.P, MaxOp{}, m, cuda::std::equal_to<>{}, st));
-        sw_rt<<<grid(m, 256), 256, 0, st>>>(x, p, w);
-        sw_sum<<<grid((int64_t)m * 32, 256), 256, 0, st>>>(x, p, w);
-        if (nT > 0) {
-            sw_after<<<grid(nT, 256), 256, 0, st>>>(x, p, w);
-            sw_commit<<<grid(nT, 256), 256, 0, st>>>(x, p, w, d_cidx, d_cr);
-        }
+        if (int rc = sw_real_time(st, g, w, stmp, stmp_bytes, err)) return rc;
+        if (nT > 0) sw_commit<<<grid(nT, 256), 256, 0, st>>>(x, p, w, d_cidx, d_cr);
         JTB_OK(cudaGetLastError());
         JTB_OK(cudaEventRecord(ev1, st));
         std::vector<unsigned long long> cnt_h((size_t)S * SW_COUNTERS), rtkey_h(S);
@@ -454,7 +431,7 @@ struct CwPass {
         if (bad) { err = "the counters of a serial witness do not add up"; return -1; }
         for (int32_t s = 0; s < S; ++s) {
             if (!cok[s]) continue;
-            jtb_cw_shard& o = shards[s];
+            jtb_lk_shard& o = shards[s];
             const unsigned long long* cc = &cnt_h[(size_t)s * SW_COUNTERS];
             o.nodes += (int64_t)cc[3];
             o.class_rounds = cr_rounds[s];
@@ -477,14 +454,5 @@ struct CwPass {
         return 0;
     }
 };
-
-inline int run_class_witness(cudaStream_t st, cudaEvent_t ev0, cudaEvent_t ev1, const jtb_history* h,
-                             int64_t max_nodes, int32_t max_rounds, int32_t max_repairs, int32_t max_lifts,
-                             int32_t flags, int32_t* commit_read, jtb_cw_shard* shards, jtb_cw_result* out,
-                             std::string& err) {
-    if (max_lifts <= 0) max_lifts = JTB_LW_DEFAULT_MAX_LIFTS;
-    return run_repairs(st, ev0, ev1, h, max_nodes, max_rounds, max_repairs, max_lifts, commit_read, shards, out, flags,
-                       err, CwPass{});
-}
 
 }  // namespace jtb

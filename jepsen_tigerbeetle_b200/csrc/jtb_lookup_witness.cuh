@@ -1,8 +1,10 @@
 // jtb_lookup_witness.cuh — K17: the lookup witness (K16's class witness, then every :ok lookup of a shard it proves is
 // placed in the shard's serial order and the merged order is checked) on the device.
 //
-// Semantics (include/jtb_check.h, DESIGN.md "K17 lookup witness").  K16 runs unchanged (run_repairs with LkPass, which
-// runs CwPass and then the lookup pass).  The lookup pass works on the shards K16 proves that have an :ok lookup:
+// Semantics (include/jtb_check.h, DESIGN.md "K17 lookup witness").  K16 runs unchanged (run_witness, jtb_witness.cuh,
+// with LkPass, which runs CwPass and then the lookup pass).  A shard K16 proves that has an :ok lookup but no read is
+// UNKNOWN with cause LOOKUP at its first lookup.  The lookup pass works on the shards K16 proves that have an :ok
+// lookup and reads on the device:
 //   - lk_shown, a thread per record: the transfers some lookup returns; lk_gap, a thread per transfer: the commit gap
 //     G(t) (a global position; rs_off[s + 1] is "after the last read") from K16's owners, a count per (shard, G) and
 //     D_g's largest invocation; a cub sum and K13's max-scan by shard give N(g) and the reads' points Q;
@@ -323,32 +325,30 @@ __global__ void lk_after(TpDev p, LkDev k, uint8_t* __restrict__ after) {
 
 // ---- host ---------------------------------------------------------------------------------------------------------
 
-// the per-shard lookup fields K17 adds to K16's
-struct LkOut {
-    std::vector<int32_t> cause, fail_index;
-    std::vector<int64_t> placed;
-    std::vector<int32_t> lread;   // per :ok lookup
-};
-
-// K17's pass over K16's results (run_repairs' Pass): CwPass, then the lookup pass
+// K17's pass over K16's results (run_witness' Pass): CwPass, then the lookup pass
 struct LkPass {
     CwPass cw;
-    LkOut* out = nullptr;
+    int32_t* lookup_read = nullptr;   // the caller's [n_l], or nullptr
 
     int pre(cudaStream_t st, TpStage& g, std::string& err) { return cw.pre(st, g, err); }
 
     int post(cudaStream_t st, cudaEvent_t ev0, cudaEvent_t ev1, const jtb_history* h, TpStage& g, int32_t max_rounds,
-             jtb_cw_shard* shards, std::vector<int32_t>& cr_h, float& ms, std::string& err) {
+             jtb_lk_shard* shards, std::vector<int32_t>& cr_h, float& ms, std::string& err) {
         const int32_t S = g.S, nT = g.nT, nL = g.nL, m = g.m;
         const int64_t nR = g.nR;
         const TlHost& T = g.T;
-        // the class pass runs on the shards K15 leaves so (CwPass::post's condition); K15's owners before it
-        std::vector<uint8_t> cls(S, 0);
+        if (lookup_read) std::fill(lookup_read, lookup_read + nL, JTB_SW_NEVER);
+        // a proved shard without reads has no serial order to place its lookups in
         for (int32_t s = 0; s < S; ++s) {
-            const jtb_cw_shard& o = shards[s];
-            cls[s] = g.dev[s] && o.valid == JTB_UNKNOWN &&
-                     (o.cause == JTB_CAUSE_UNDECIDED || o.cause == JTB_CAUSE_NO_WITNESS || o.cause == JTB_CAUSE_REAL_TIME);
+            jtb_lk_shard& o = shards[s];
+            if (o.valid == JTB_VALID && o.n_reads == 0 && T.lk_off[s + 1] > T.lk_off[s]) {
+                o.valid = JTB_UNKNOWN;
+                o.cause = o.lookup_cause = JTB_CAUSE_LOOKUP;
+                o.fail_index = o.lookup_fail_index = T.l_cidx[T.lk_off[s]];
+            }
         }
+        if (m == 0) return 0;
+        // K15's owners, before the class pass
         CallAllocs& A = g.A;
         int32_t* kowner;
         JTB_OK(A.alloc(&kowner, nT));
@@ -367,13 +367,11 @@ struct LkPass {
         k.kowner = kowner;
         const int64_t nE = (int64_t)m + nT + nL;
         const int32_t nH = m + S;
-        std::vector<int32_t> rd_cidx(m);
-        for (int32_t i = 0; i < m; ++i) rd_cidx[i] = h->index[g.H.r_ev[g.d_of[i]]];
         int32_t *hist, *gmax, *Q, *lperm0, *lperm, *head, *lcnt, *ccum, *oval0, *oval, *skey, *xin, *P;
         LkKey *lkey0, *lkey;
         LkOpKey *okey0, *okey;
         uint8_t *live, *stmp;
-        JTB_OK(A.put(&k.on, on, st)); JTB_OK(A.put(&k.cls, cls, st)); JTB_OK(A.put(&k.l_inv, T.l_inv, st));
+        JTB_OK(A.put(&k.on, on, st)); JTB_OK(A.put(&k.cls, cw.cok, st)); JTB_OK(A.put(&k.l_inv, T.l_inv, st));
         JTB_OK(A.alloc(&k.shown, nT)); JTB_OK(A.alloc(&k.G, nT)); JTB_OK(A.alloc(&k.layer, nT));
         JTB_OK(A.alloc(&hist, nH)); JTB_OK(A.alloc(&k.cum, nH)); JTB_OK(A.alloc(&gmax, m)); JTB_OK(A.alloc(&Q, m));
         JTB_OK(A.alloc(&k.lo, nL)); JTB_OK(A.alloc(&k.below, nL)); JTB_OK(A.alloc(&k.bad, nL));
@@ -386,6 +384,7 @@ struct LkPass {
         const int32_t *d_rcidx, *d_lcidx;
         int32_t *fidx, *lread;
         uint8_t* after;
+        const std::vector<int32_t> rd_cidx = sw_rd_cidx(h, g);
         JTB_OK(A.put(&d_rcidx, rd_cidx, st)); JTB_OK(A.put(&d_lcidx, T.l_cidx, st));
         JTB_OK(A.alloc(&fidx, S)); JTB_OK(A.alloc(&lread, nL)); JTB_OK(A.alloc(&after, nT));
         JTB_OK(A.alloc(&okey0, nE)); JTB_OK(A.alloc(&okey, nE)); JTB_OK(A.alloc(&oval0, nE)); JTB_OK(A.alloc(&oval, nE));
@@ -474,102 +473,28 @@ struct LkPass {
         JTB_OK(cudaEventRecord(ev1, st));
         std::vector<uint8_t> after_h(nT);
         JTB_OK(cudaMemcpyAsync(fidx_h.data(), fidx, (size_t)S * 4, cudaMemcpyDeviceToHost, st));
-        if (nL > 0) JTB_OK(cudaMemcpyAsync(out->lread.data(), lread, (size_t)nL * 4, cudaMemcpyDeviceToHost, st));
+        if (lookup_read && nL > 0)
+            JTB_OK(cudaMemcpyAsync(lookup_read, lread, (size_t)nL * 4, cudaMemcpyDeviceToHost, st));
         if (nT > 0) JTB_OK(cudaMemcpyAsync(after_h.data(), after, (size_t)nT, cudaMemcpyDeviceToHost, st));
         JTB_OK(cudaStreamSynchronize(st));
         JTB_OK(cudaEventElapsedTime(&ms, ev0, ev1));
         for (int32_t s = 0; s < S; ++s) {
             if (!on[s]) continue;
-            jtb_cw_shard& o = shards[s];
+            jtb_lk_shard& o = shards[s];
             if (fidx_h[s] != INT_MIN) {
                 o.valid = JTB_UNKNOWN;
-                o.cause = JTB_CAUSE_LOOKUP;
-                o.fail_index = fidx_h[s];
+                o.cause = o.lookup_cause = JTB_CAUSE_LOOKUP;
+                o.fail_index = o.lookup_fail_index = fidx_h[s];
                 o.transfer_id = -1;
                 o.n_committed = o.n_committed_crashed = o.n_after = 0;
-                out->cause[s] = JTB_CAUSE_LOOKUP;
-                out->fail_index[s] = fidx_h[s];
                 continue;
             }
             for (int32_t t = T.t_off[s]; t < T.t_off[s + 1]; ++t)
                 if (after_h[t]) cr_h[t] = JTB_SW_AFTER;
-            out->placed[s] = T.lk_off[s + 1] - T.lk_off[s];
+            o.n_lookups_placed = T.lk_off[s + 1] - T.lk_off[s];
         }
         return 0;
     }
 };
-
-inline int run_lookup_witness(cudaStream_t st, cudaEvent_t ev0, cudaEvent_t ev1, const jtb_history* h,
-                              int64_t max_nodes, int32_t max_rounds, int32_t max_repairs, int32_t max_lifts,
-                              int32_t flags, int32_t* commit_read, int32_t* lookup_read, jtb_lk_shard* shards,
-                              jtb_lk_result* out, std::string& err) {
-    const auto t0 = std::chrono::steady_clock::now();
-    if (!h || !shards || !out) { err = "null argument"; return -2; }
-    if (max_lifts <= 0) max_lifts = JTB_LW_DEFAULT_MAX_LIFTS;
-    const int32_t S = std::max(h->n_shards, 0);
-    // the :ok lookups of every shard (tl_host_pass's), and the first one's completion :index
-    std::vector<int64_t> nl(S, 0);
-    std::vector<int32_t> first(S, -1);
-    int64_t nL = 0;
-    for (int32_t s = 0; s < S; ++s)
-        for (int64_t e = h->shard_off[s]; e < h->shard_off[s + 1]; ++e)
-            if (h->process[e] >= 0 && h->type[e] == JTB_T_OK && h->f[e] == JTB_F_LOOKUP && h->payload_len[e] >= 0) {
-                if (nl[s]++ == 0) first[s] = h->index[e];
-                nL++;
-            }
-    std::vector<jtb_cw_shard> cw(std::max(S, 1));
-    jtb_cw_result cr;
-    LkOut lo;
-    lo.cause.assign(S, 0);
-    lo.fail_index.assign(S, -1);
-    lo.placed.assign(S, 0);
-    lo.lread.assign(nL, JTB_SW_NEVER);
-    LkPass pass;
-    pass.out = &lo;
-    if (int rc = run_repairs(st, ev0, ev1, h, max_nodes, max_rounds, max_repairs, max_lifts, commit_read, cw.data(),
-                             &cr, flags, err, pass))
-        return rc;
-    memset(out, 0, sizeof *out);
-    int64_t at = 0;
-    for (int32_t s = 0; s < S; ++s) {
-        const jtb_cw_shard& c = cw[s];
-        jtb_lk_shard& o = shards[s];
-        memset(&o, 0, sizeof o);
-        o.valid = c.valid; o.cause = c.cause; o.n_reads = c.n_reads; o.n_transfers = c.n_transfers;
-        o.n_committed = c.n_committed; o.n_committed_crashed = c.n_committed_crashed; o.n_after = c.n_after;
-        o.nodes = c.nodes; o.rounds = c.rounds; o.fail_index = c.fail_index; o.transfer_id = c.transfer_id;
-        o.repairs = c.repairs; o.n_bans = c.n_bans; o.lifts = c.lifts; o.n_lifted = c.n_lifted;
-        o.class_cause = c.class_cause; o.class_rounds = c.class_rounds; o.n_handed = c.n_handed;
-        o.lookup_cause = lo.cause[s];
-        o.lookup_fail_index = lo.fail_index[s];
-        o.n_lookups_placed = lo.placed[s];
-        // a proved shard without reads has no serial order to place its lookups in
-        if (o.valid == JTB_VALID && o.n_reads == 0 && nl[s] > 0) {
-            o.valid = JTB_UNKNOWN;
-            o.cause = o.lookup_cause = JTB_CAUSE_LOOKUP;
-            o.fail_index = o.lookup_fail_index = first[s];
-            if (commit_read)
-                for (int32_t t = 0; t < o.n_transfers; ++t) commit_read[at + t] = JTB_SW_NEVER;
-        }
-        at += o.n_transfers;
-        out->n_reads += o.n_reads;
-        out->n_transfers += o.n_transfers;
-        out->n_committed += o.n_committed;
-        out->n_committed_crashed += o.n_committed_crashed;
-        out->n_after += o.n_after;
-        out->nodes += o.nodes;
-        out->rounds = std::max(out->rounds, (int64_t)o.rounds);
-        out->repairs = std::max(out->repairs, (int64_t)o.repairs);
-        out->n_bans += o.n_bans;
-        out->lifts = std::max(out->lifts, (int64_t)o.lifts);
-        out->n_lifted += o.n_lifted;
-        out->class_rounds = std::max(out->class_rounds, (int64_t)o.class_rounds);
-        out->n_handed += o.n_handed;
-        out->n_lookups_placed += o.n_lookups_placed;
-    }
-    if (lookup_read && nL > 0) memcpy(lookup_read, lo.lread.data(), (size_t)nL * 4);
-    roll_up(out, shards, S, (float)(cr.seconds_kernel * 1e3), t0);
-    return 0;
-}
 
 }  // namespace jtb

@@ -261,6 +261,6 @@ __global__ void rw_count(int32_t m, SwDev w) {
 }
 
 // ---- host ---------------------------------------------------------------------------------------------------------
-// The repair loop on the host is run_repairs in jtb_lifted_witness.cuh, which K14 runs with no lift steps.
+// The repair loop on the host is run_witness in jtb_witness.cuh, which K14 runs with no lift steps.
 
 }  // namespace jtb

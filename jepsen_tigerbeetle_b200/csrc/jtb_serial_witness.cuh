@@ -17,6 +17,8 @@
 //     per :ok transfer in no gap, the smallest failure key per shard; sw_rt_id the smallest failing transfer id there;
 //   - sw_sum, a warp per gap: D_g's counters against V (a mismatch is an internal error);
 //   - sw_commit, a thread per transfer: commit_read.
+// The host runs these through run_witness (jtb_witness.cuh) with no repairs and no lifts: after the real time,
+// rw_verdict (K14's) turns each shard's failure into its cause and key, and sw_commit runs on the shards it proves.
 // The decision, the node counts and the rounds equal the SW_SEARCH CPU test oracle's, shard for shard, and commit_read
 // entry for entry.
 #pragma once
@@ -275,169 +277,51 @@ __global__ void sw_commit(RgDev d, TpDev p, SwDev w, const int32_t* __restrict__
 
 // ---- host ---------------------------------------------------------------------------------------------------------
 
-inline int run_serial_witness(cudaStream_t st, cudaEvent_t ev0, cudaEvent_t ev1, const jtb_history* h,
-                              int64_t max_nodes, int32_t max_rounds, int32_t flags, int32_t* commit_read,
-                              jtb_sw_shard* shards, jtb_sw_result* out, std::string& err) {
-    const auto t0 = std::chrono::steady_clock::now();
-    if (!h || !shards || !out) { err = "null argument"; return -2; }
-    if (max_rounds <= 0) max_rounds = JTB_TP_DEFAULT_MAX_ROUNDS;
-    TpStage g;
-    if (int rc = tp_stage(st, ev0, h, max_nodes, max_rounds, flags, g, err)) return rc;
+// the completion :index of the read at each sorted position
+inline std::vector<int32_t> sw_rd_cidx(const jtb_history* h, const TpStage& g) {
+    std::vector<int32_t> c(g.m);
+    for (int32_t i = 0; i < g.m; ++i) c[i] = h->index[g.H.r_ev[g.d_of[i]]];
+    return c;
+}
+
+// the witness state of the stage's gaps, transfers and shards, on the shards sok marks; failures, counters and the
+// unfixed count reset
+inline int sw_alloc(cudaStream_t st, TpStage& g, const std::vector<uint8_t>& sok, SwDev& w, std::string& err) {
+    CallAllocs& A = g.A;
     const int32_t S = g.S, nT = g.nT, m = g.m;
-    std::vector<jtb_tp_shard> tp(std::max(S, 1));
-    float ms = 0;
-    if (int rc = tp_finals(st, ev0, ev1, h, g, tp.data(), ms, err)) return rc;
-    const TlHost& T = g.T;
-    std::vector<uint8_t> sok(S, 0);
-    bool any = false;
-    for (int32_t s = 0; s < S; ++s) {
-        jtb_sw_shard& o = shards[s];
-        memset(&o, 0, sizeof o);
-        o.valid = JTB_VALID;
-        o.n_reads = tp[s].n_reads;
-        o.n_transfers = tp[s].n_transfers;
-        o.fail_index = -1;
-        o.transfer_id = -1;
-        if (tp[s].valid != JTB_VALID) {
-            o.valid = JTB_UNKNOWN;
-            o.cause = tp[s].cause ? tp[s].cause : tp[s].valid == JTB_INVALID ? JTB_CAUSE_ANOMALY : JTB_CAUSE_UNDECIDED;
-        }
-        any |= (sok[s] = g.dev[s] && o.valid == JTB_VALID);
-    }
-    std::vector<int32_t> cr_h(nT, JTB_SW_NEVER);
-    if (m > 0 && any) {
-        CallAllocs& A = g.A;
-        RgDev& x = g.x;
-        TpDev& p = g.p;
-        SwDev w;
-        w.t_okcomp = g.d.t_okcomp;
-        std::vector<int32_t> rd_cidx(m);
-        for (int32_t r = 0; r < m; ++r) rd_cidx[r] = h->index[g.H.r_ev[g.d_of[r]]];
-        const int32_t* d_cidx;
-        int32_t* d_cr;
-        uint8_t* stmp;
-        JTB_OK(A.put(&w.sok, sok, st)); JTB_OK(A.put(&d_cidx, rd_cidx, st));
-        JTB_OK(A.alloc(&w.fixed, m)); JTB_OK(A.alloc(&w.cmin, nT)); JTB_OK(A.alloc(&w.sfail, S));
-        JTB_OK(A.alloc(&w.sunf, S)); JTB_OK(A.alloc(&w.unfixed, 1)); JTB_OK(A.alloc(&w.cnt, (size_t)S * SW_COUNTERS));
-        JTB_OK(A.alloc(&w.gmax, m)); JTB_OK(A.alloc(&w.gmin, m)); JTB_OK(A.alloc(&w.skey, m));
-        JTB_OK(A.alloc(&w.x, m)); JTB_OK(A.alloc(&w.P, m)); JTB_OK(A.alloc(&w.rtkey, S)); JTB_OK(A.alloc(&w.rtid, S));
-        JTB_OK(A.alloc(&w.bad, 1)); JTB_OK(A.alloc(&d_cr, nT));
-        size_t stmp_bytes = 0;
-        JTB_OK(cub::DeviceScan::InclusiveScanByKey(nullptr, stmp_bytes, w.skey, w.x, w.P, MaxOp{}, m,
-                                                   cuda::std::equal_to<>{}, st));
-        JTB_OK(A.alloc(&stmp, stmp_bytes));
-        auto grid = [](int64_t n, int per) { return (unsigned)((n + per - 1) / per); };
-        JTB_OK(cudaMemsetAsync(w.sfail, 0x7f, (size_t)S * 4, st));   // RG_NONE
-        JTB_OK(cudaMemsetAsync(w.sunf, 0x7f, (size_t)S * 4, st));
-        JTB_OK(cudaMemsetAsync(w.cnt, 0, (size_t)S * SW_COUNTERS * 8, st));
-        JTB_OK(cudaMemsetAsync(w.unfixed, 0, 4, st));
-        JTB_OK(cudaMemsetAsync(p.srounds, 0, (size_t)S * 4, st));
-        sw_init<<<grid(m, 256), 256, 0, st>>>(x, p, w);
-        int32_t unfixed = 0;
-        JTB_OK(cudaMemcpyAsync(&unfixed, w.unfixed, 4, cudaMemcpyDeviceToHost, st));
-        JTB_OK(cudaStreamSynchronize(st));
-        // the witness rounds
-        for (int32_t r = 0; unfixed > 0 && r < max_rounds; ++r) {
-            JTB_OK(cudaMemsetAsync(w.cmin, 0x7f, (size_t)nT * 4, st));
-            JTB_OK(cudaMemsetAsync(w.unfixed, 0, 4, st));
-            w.round = r;
-            sw_gaps<<<grid(m, RG_WARPS), RG_WARPS * 32, 0, st>>>(x, p, w);
-            sw_fix<<<grid(m, 256), 256, 0, st>>>(m, x, p, w);
-            JTB_OK(cudaGetLastError());
-            JTB_OK(cudaMemcpyAsync(&unfixed, w.unfixed, 4, cudaMemcpyDeviceToHost, st));
-            JTB_OK(cudaStreamSynchronize(st));
-        }
-        if (unfixed > 0) sw_unfixed<<<grid(m, 256), 256, 0, st>>>(m, x, w);
-        // real time and the counters
-        JTB_OK(cudaMemsetAsync(w.gmax, 0x80, (size_t)m * 4, st));   // INT_MIN
-        JTB_OK(cudaMemsetAsync(w.gmin, 0x7f, (size_t)m * 4, st));   // > every position
-        JTB_OK(cudaMemsetAsync(w.rtkey, 0xff, (size_t)S * 8, st));
-        JTB_OK(cudaMemsetAsync(w.rtid, 0xff, (size_t)S * 8, st));
-        JTB_OK(cudaMemsetAsync(w.bad, 0, 4, st));
-        JTB_OK(cudaMemsetAsync(g.own, 0, (size_t)g.cells * 8, st));
-        if (nT > 0) sw_tgap<<<grid(nT, 256), 256, 0, st>>>(x, p, w);
-        sw_scan_in<<<grid(m, 256), 256, 0, st>>>(x, w);
-        size_t tb = stmp_bytes;
-        JTB_OK(cub::DeviceScan::InclusiveScanByKey(stmp, tb, w.skey, w.x, w.P, MaxOp{}, m, cuda::std::equal_to<>{}, st));
-        sw_rt<<<grid(m, 256), 256, 0, st>>>(x, p, w);
-        sw_sum<<<grid((int64_t)m * 32, 256), 256, 0, st>>>(x, p, w);
-        if (nT > 0) {
-            sw_after<<<grid(nT, 256), 256, 0, st>>>(x, p, w);
-            sw_rt_id<<<grid(nT, 256), 256, 0, st>>>(x, p, w);
-            sw_commit<<<grid(nT, 256), 256, 0, st>>>(x, p, w, d_cidx, d_cr);
-        }
-        JTB_OK(cudaGetLastError());
-        JTB_OK(cudaEventRecord(ev1, st));
-        std::vector<unsigned long long> cnt_h((size_t)S * SW_COUNTERS), rtkey_h(S), rtid_h(S);
-        std::vector<int32_t> sfail_h(S), sunf_h(S), sr_h(S);
-        unsigned int bad = 0;
-        JTB_OK(cudaMemcpyAsync(cnt_h.data(), w.cnt, cnt_h.size() * 8, cudaMemcpyDeviceToHost, st));
-        JTB_OK(cudaMemcpyAsync(rtkey_h.data(), w.rtkey, (size_t)S * 8, cudaMemcpyDeviceToHost, st));
-        JTB_OK(cudaMemcpyAsync(rtid_h.data(), w.rtid, (size_t)S * 8, cudaMemcpyDeviceToHost, st));
-        JTB_OK(cudaMemcpyAsync(sfail_h.data(), w.sfail, (size_t)S * 4, cudaMemcpyDeviceToHost, st));
-        JTB_OK(cudaMemcpyAsync(sunf_h.data(), w.sunf, (size_t)S * 4, cudaMemcpyDeviceToHost, st));
-        JTB_OK(cudaMemcpyAsync(sr_h.data(), p.srounds, (size_t)S * 4, cudaMemcpyDeviceToHost, st));
-        JTB_OK(cudaMemcpyAsync(&bad, w.bad, 4, cudaMemcpyDeviceToHost, st));
-        if (nT > 0) JTB_OK(cudaMemcpyAsync(cr_h.data(), d_cr, (size_t)nT * 4, cudaMemcpyDeviceToHost, st));
-        JTB_OK(cudaStreamSynchronize(st));
-        JTB_OK(cudaEventElapsedTime(&ms, ev0, ev1));
-        if (bad) { err = "the counters of a serial witness do not add up"; return -1; }
-        auto index_at = [&](int32_t at) -> int32_t {   // completion :index of the read at a sorted position
-            int32_t r;
-            if (cudaMemcpy(&r, x.ord + at, 4, cudaMemcpyDeviceToHost) != cudaSuccess) return INT_MIN;
-            return rd_cidx[r];
-        };
-        for (int32_t s = 0; s < S; ++s) {
-            if (!sok[s]) continue;
-            jtb_sw_shard& o = shards[s];
-            const unsigned long long* c = &cnt_h[(size_t)s * SW_COUNTERS];
-            o.nodes = (int64_t)c[3];
-            o.rounds = sr_h[s];
-            const int32_t fail = sfail_h[s] != RG_NONE ? sfail_h[s] : sunf_h[s];
-            if (fail != RG_NONE) {
-                o.valid = JTB_UNKNOWN;
-                o.cause = JTB_CAUSE_NO_WITNESS;
-                o.fail_index = index_at(fail);
-            } else if (rtkey_h[s] != ~0ull) {
-                o.valid = JTB_UNKNOWN;
-                o.cause = JTB_CAUSE_REAL_TIME;
-                const int32_t at = (int32_t)(rtkey_h[s] >> 1);
-                if (rtkey_h[s] & 1) {
-                    o.fail_index = index_at(at);
-                } else {
-                    o.transfer_id = (int64_t)(rtid_h[s] ^ 0x8000000000000000ull);
-                    int32_t t = T.t_off[s];
-                    while (T.t_id[t] != o.transfer_id) ++t;
-                    o.fail_index = T.t_cidx[t];
-                }
-            } else {
-                o.n_committed = (int64_t)c[0];
-                o.n_committed_crashed = (int64_t)c[1];
-                o.n_after = (int64_t)c[2];
-            }
-            if (o.fail_index == INT_MIN) { err = "cudaMemcpy of a failing read failed"; return -1; }
-        }
-    }
-    // commit_read: the shards with no reads commit their :ok transfers freely; a shard that is not VALID commits none
-    for (int32_t s = 0; s < S; ++s) {
-        const bool free_ = shards[s].valid == JTB_VALID && g.H.n_reads[s] == 0;
-        if (shards[s].valid == JTB_VALID && !free_) continue;
-        for (int32_t t = T.t_off[s]; t < T.t_off[s + 1]; ++t)
-            cr_h[t] = free_ && T.t_fate[t] == JTB_T_OK ? JTB_SW_FREE : JTB_SW_NEVER;
-    }
-    if (commit_read && nT > 0) memcpy(commit_read, cr_h.data(), (size_t)nT * 4);
-    memset(out, 0, sizeof *out);
-    for (int32_t s = 0; s < S; ++s) {
-        const jtb_sw_shard& o = shards[s];
-        out->n_reads += o.n_reads;
-        out->n_transfers += o.n_transfers;
-        out->n_committed += o.n_committed;
-        out->n_committed_crashed += o.n_committed_crashed;
-        out->n_after += o.n_after;
-        out->nodes += o.nodes;
-        out->rounds = std::max(out->rounds, (int64_t)o.rounds);
-    }
-    roll_up(out, shards, S, ms, t0);
+    w.t_okcomp = g.d.t_okcomp;
+    JTB_OK(A.put(&w.sok, sok, st));
+    JTB_OK(A.alloc(&w.fixed, m)); JTB_OK(A.alloc(&w.cmin, nT)); JTB_OK(A.alloc(&w.sfail, S));
+    JTB_OK(A.alloc(&w.sunf, S)); JTB_OK(A.alloc(&w.unfixed, 1)); JTB_OK(A.alloc(&w.cnt, (size_t)S * SW_COUNTERS));
+    JTB_OK(A.alloc(&w.gmax, m)); JTB_OK(A.alloc(&w.gmin, m)); JTB_OK(A.alloc(&w.skey, m));
+    JTB_OK(A.alloc(&w.x, m)); JTB_OK(A.alloc(&w.P, m)); JTB_OK(A.alloc(&w.rtkey, S)); JTB_OK(A.alloc(&w.rtid, S));
+    JTB_OK(A.alloc(&w.bad, 1));
+    JTB_OK(cudaMemsetAsync(w.sfail, 0x7f, (size_t)S * 4, st));   // RG_NONE
+    JTB_OK(cudaMemsetAsync(w.sunf, 0x7f, (size_t)S * 4, st));
+    JTB_OK(cudaMemsetAsync(w.cnt, 0, (size_t)S * SW_COUNTERS * 8, st));
+    JTB_OK(cudaMemsetAsync(w.unfixed, 0, 4, st));
+    return 0;
+}
+
+// the real time and the counters of the witness in p.owner: sw_tgap over owned counters cleared first, the max-scan
+// (cub's temporary storage stmp), sw_rt, sw_sum and sw_after; sw_rt_id and sw_commit are the caller's
+inline int sw_real_time(cudaStream_t st, TpStage& g, const SwDev& w, uint8_t* stmp, size_t stmp_bytes,
+                        std::string& err) {
+    const int32_t S = g.S, nT = g.nT, m = g.m;
+    auto grid = [](int64_t n, int per) { return (unsigned)((n + per - 1) / per); };
+    JTB_OK(cudaMemsetAsync(w.gmax, 0x80, (size_t)m * 4, st));   // INT_MIN
+    JTB_OK(cudaMemsetAsync(w.gmin, 0x7f, (size_t)m * 4, st));   // > every position
+    JTB_OK(cudaMemsetAsync(w.rtkey, 0xff, (size_t)S * 8, st));
+    JTB_OK(cudaMemsetAsync(w.rtid, 0xff, (size_t)S * 8, st));
+    JTB_OK(cudaMemsetAsync(w.bad, 0, 4, st));
+    JTB_OK(cudaMemsetAsync(g.own, 0, (size_t)g.cells * 8, st));
+    if (nT > 0) sw_tgap<<<grid(nT, 256), 256, 0, st>>>(g.x, g.p, w);
+    sw_scan_in<<<grid(m, 256), 256, 0, st>>>(g.x, w);
+    JTB_OK(cub::DeviceScan::InclusiveScanByKey(stmp, stmp_bytes, w.skey, w.x, w.P, MaxOp{}, m, cuda::std::equal_to<>{},
+                                               st));
+    sw_rt<<<grid(m, 256), 256, 0, st>>>(g.x, g.p, w);
+    sw_sum<<<grid((int64_t)m * 32, 256), 256, 0, st>>>(g.x, g.p, w);
+    if (nT > 0) sw_after<<<grid(nT, 256), 256, 0, st>>>(g.x, g.p, w);
     return 0;
 }
 

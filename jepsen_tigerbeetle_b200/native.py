@@ -21,7 +21,7 @@ _DEPS = _SOURCES + ["jtb_prep.h", "jtb_expand.h", "jtb_wgl.cuh", "jtb_scout.cuh"
                     "jtb_table_bench.cuh", "jtb_level.cuh", "jtb_partition.cuh", "jtb_monotonic.cuh",
                     "jtb_counter_bounds.cuh", "jtb_transfer_lookups.cuh", "jtb_read_explanations.cuh",
                     "jtb_read_gaps.cuh", "jtb_transfer_placement.cuh", "jtb_serial_witness.cuh", "jtb_repaired_witness.cuh",
-                    "jtb_lifted_witness.cuh", "jtb_class_witness.cuh", "jtb_lookup_witness.cuh", "jtb_edn.cuh", "jtb_edn_checks.cuh", "jtb_call.cuh"]
+                    "jtb_lifted_witness.cuh", "jtb_class_witness.cuh", "jtb_lookup_witness.cuh", "jtb_witness.cuh", "jtb_edn.cuh", "jtb_edn_checks.cuh", "jtb_call.cuh"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared", "-ldl"]
 
@@ -303,6 +303,24 @@ class Context:
             raise NativeError(f"jtb_check_transfer_placement rc={rc}: {self._err()}")
         return abi.tp_to_dict(res, shards[:h.n_shards])
 
+    def _witness(self, name, shard_t, result_t, h, witness, *args, lookups=False) -> dict:
+        """One call of the witness check `name` (K13-K17) with the arguments before commit_read; lookups: it also
+        returns lookup_read."""
+        import numpy as np
+        ch = as_c_history(h)
+        shards = (shard_t * max(1, h.n_shards))()
+        res = result_t()
+        cr = np.zeros(max(1, abi.n_transfer_records(h)), np.int32) if witness else None
+        nl = abi.n_ok_lookups(h) if lookups else 0
+        lr = np.zeros(max(1, nl), np.int32) if witness and lookups else None
+        rc = getattr(lib(), name)(self._h, C.addressof(ch), *args, cr.ctypes.data if witness else None,
+                                  *((lr.ctypes.data if witness else None,) if lookups else ()), C.addressof(shards),
+                                  C.addressof(res))
+        if rc != 0:
+            raise NativeError(f"{name} rc={rc}: {self._err()}")
+        return abi.witness_to_dict(res, shards[:h.n_shards], cr[:res.n_transfers].copy() if witness else None,
+                                   lr[:nl].copy() if witness and lookups else None)
+
     # ---- K13: serial-witness check --------------------------------------------------------------------------------
     def check_serial_witness(self, h: FlatHistory, max_nodes: int = 0, max_rounds: int = 0,
                              witness: bool = False) -> dict:
@@ -315,17 +333,8 @@ class Context:
         "cause", "n_reads", "n_transfers", "n_committed", "n_committed_crashed", "n_after", "nodes", "rounds",
         "fail_index", "transfer_id"}]}; witness=True adds "commit_read": per transfer micro-op in history order, the
         completion :index of the first read whose state holds it, abi.SW_NEVER, SW_AFTER or SW_FREE."""
-        import numpy as np
-        ch = as_c_history(h)
-        shards = (abi.CSwShard * max(1, h.n_shards))()
-        res = abi.CSwResult()
-        cr = np.zeros(max(1, abi.n_transfer_records(h)), np.int32) if witness else None
-        rc = lib().jtb_check_serial_witness(self._h, C.addressof(ch), max_nodes, max_rounds, 0,
-                                            cr.ctypes.data if witness else None, C.addressof(shards),
-                                            C.addressof(res))
-        if rc != 0:
-            raise NativeError(f"jtb_check_serial_witness rc={rc}: {self._err()}")
-        return abi.sw_to_dict(res, shards[:h.n_shards], cr[:res.n_transfers].copy() if witness else None)
+        return self._witness("jtb_check_serial_witness", abi.CSwShard, abi.CSwResult, h, witness, max_nodes, max_rounds,
+                             0)
 
     # ---- K14: repaired serial witness ----------------------------------------------------------------------------
     def check_repaired_witness(self, h: FlatHistory, max_nodes: int = 0, max_rounds: int = 0, max_repairs: int = 0,
@@ -335,17 +344,8 @@ class Context:
         witness rounds run again; every VALID is the same proof.  A shard check_serial_witness proves comes back as it
         returns it.  The dict of check_serial_witness with "repairs" (the most of any shard) and "n_bans" added, and
         per shard "repairs" and "n_bans"; flags must be 0."""
-        import numpy as np
-        ch = as_c_history(h)
-        shards = (abi.CRwShard * max(1, h.n_shards))()
-        res = abi.CRwResult()
-        cr = np.zeros(max(1, abi.n_transfer_records(h)), np.int32) if witness else None
-        rc = lib().jtb_check_repaired_witness(self._h, C.addressof(ch), max_nodes, max_rounds, max_repairs, flags,
-                                              cr.ctypes.data if witness else None, C.addressof(shards),
-                                              C.addressof(res))
-        if rc != 0:
-            raise NativeError(f"jtb_check_repaired_witness rc={rc}: {self._err()}")
-        return abi.rw_to_dict(res, shards[:h.n_shards], cr[:res.n_transfers].copy() if witness else None)
+        return self._witness("jtb_check_repaired_witness", abi.CRwShard, abi.CRwResult, h, witness, max_nodes,
+                             max_rounds, max_repairs, flags)
 
     # ---- K15: lifted serial witness ------------------------------------------------------------------------------
     def check_lifted_witness(self, h: FlatHistory, max_nodes: int = 0, max_rounds: int = 0, max_repairs: int = 0,
@@ -356,17 +356,8 @@ class Context:
         same proof.  A shard check_repaired_witness proves comes back as it returns it.  The dict of
         check_repaired_witness with "lifts" (the most of any shard) and "n_lifted" added, and per shard "lifts" and
         "n_lifted"; flags must be 0."""
-        import numpy as np
-        ch = as_c_history(h)
-        shards = (abi.CLwShard * max(1, h.n_shards))()
-        res = abi.CLwResult()
-        cr = np.zeros(max(1, abi.n_transfer_records(h)), np.int32) if witness else None
-        rc = lib().jtb_check_lifted_witness(self._h, C.addressof(ch), max_nodes, max_rounds, max_repairs, max_lifts,
-                                            flags, cr.ctypes.data if witness else None, C.addressof(shards),
-                                            C.addressof(res))
-        if rc != 0:
-            raise NativeError(f"jtb_check_lifted_witness rc={rc}: {self._err()}")
-        return abi.lw_to_dict(res, shards[:h.n_shards], cr[:res.n_transfers].copy() if witness else None)
+        return self._witness("jtb_check_lifted_witness", abi.CLwShard, abi.CLwResult, h, witness, max_nodes,
+                             max_rounds, max_repairs, max_lifts, flags)
 
     # ---- K16: class witness --------------------------------------------------------------------------------------
     def check_class_witness(self, h: FlatHistory, max_nodes: int = 0, max_rounds: int = 0, max_repairs: int = 0,
@@ -377,17 +368,8 @@ class Context:
         real-time pass and re-sum.  A shard check_lifted_witness proves comes back as it returns it.  The dict of
         check_lifted_witness with "class_rounds" (the most of any shard) and "n_handed" added, and per shard
         "class_cause", "class_rounds" and "n_handed"; flags must be 0."""
-        import numpy as np
-        ch = as_c_history(h)
-        shards = (abi.CCwShard * max(1, h.n_shards))()
-        res = abi.CCwResult()
-        cr = np.zeros(max(1, abi.n_transfer_records(h)), np.int32) if witness else None
-        rc = lib().jtb_check_class_witness(self._h, C.addressof(ch), max_nodes, max_rounds, max_repairs, max_lifts,
-                                           flags, cr.ctypes.data if witness else None, C.addressof(shards),
-                                           C.addressof(res))
-        if rc != 0:
-            raise NativeError(f"jtb_check_class_witness rc={rc}: {self._err()}")
-        return abi.cw_to_dict(res, shards[:h.n_shards], cr[:res.n_transfers].copy() if witness else None)
+        return self._witness("jtb_check_class_witness", abi.CCwShard, abi.CCwResult, h, witness, max_nodes,
+                             max_rounds, max_repairs, max_lifts, flags)
 
     # ---- K17: lookup witness -------------------------------------------------------------------------------------
     def check_lookup_witness(self, h: FlatHistory, max_nodes: int = 0, max_rounds: int = 0, max_repairs: int = 0,
@@ -398,21 +380,8 @@ class Context:
         be placed is UNKNOWN with cause "lookup".  The dict of check_class_witness with "n_lookups_placed" added, and
         per shard "lookup_cause", "lookup_fail_index" and "n_lookups_placed"; with witness=True also "lookup_read" (one
         entry per :ok lookup in history order).  flags must be 0."""
-        import numpy as np
-        ch = as_c_history(h)
-        shards = (abi.CLkShard * max(1, h.n_shards))()
-        res = abi.CLkResult()
-        cr = np.zeros(max(1, abi.n_transfer_records(h)), np.int32) if witness else None
-        nl = abi.n_ok_lookups(h)
-        lr = np.zeros(max(1, nl), np.int32) if witness else None
-        rc = lib().jtb_check_lookup_witness(self._h, C.addressof(ch), max_nodes, max_rounds, max_repairs, max_lifts,
-                                            flags, cr.ctypes.data if witness else None,
-                                            lr.ctypes.data if witness else None, C.addressof(shards),
-                                            C.addressof(res))
-        if rc != 0:
-            raise NativeError(f"jtb_check_lookup_witness rc={rc}: {self._err()}")
-        return abi.lk_to_dict(res, shards[:h.n_shards], cr[:res.n_transfers].copy() if witness else None,
-                              lr[:nl].copy() if witness else None)
+        return self._witness("jtb_check_lookup_witness", abi.CLkShard, abi.CLkResult, h, witness, max_nodes,
+                             max_rounds, max_repairs, max_lifts, flags, lookups=True)
 
     # ---- K18: a stored ledger history.edn read on the device ------------------------------------------------------
     def read_ledger_edn(self, data, form: str, timings: dict | None = None) -> FlatHistory:

@@ -201,7 +201,7 @@ def check_serial_witness(h: FlatHistory, algo: int = SW_SEARCH, max_nodes: int =
                                          cr.ctypes.data if witness else None, C.addressof(shards), C.addressof(res))
     if rc != 0:
         raise RuntimeError(lib().jtbm_sw_last_error().decode())
-    return abi.sw_to_dict(res, shards[:h.n_shards], cr[:res.n_transfers].copy() if witness else None)
+    return abi.witness_to_dict(res, shards[:h.n_shards], cr[:res.n_transfers].copy() if witness else None)
 
 
 def check_repaired_witness(h: FlatHistory, algo: int = RW_SEARCH, max_nodes: int = 0, max_rounds: int = 0,
@@ -217,7 +217,7 @@ def check_repaired_witness(h: FlatHistory, algo: int = RW_SEARCH, max_nodes: int
                                            C.addressof(res))
     if rc != 0:
         raise RuntimeError(lib().jtbm_rw_last_error().decode())
-    return abi.rw_to_dict(res, shards[:h.n_shards], cr[:res.n_transfers].copy() if witness else None)
+    return abi.witness_to_dict(res, shards[:h.n_shards], cr[:res.n_transfers].copy() if witness else None)
 
 
 def check_lifted_witness(h: FlatHistory, algo: int = LW_SEARCH, max_nodes: int = 0, max_rounds: int = 0,
@@ -232,7 +232,7 @@ def check_lifted_witness(h: FlatHistory, algo: int = LW_SEARCH, max_nodes: int =
                                          cr.ctypes.data if witness else None, C.addressof(shards), C.addressof(res))
     if rc != 0:
         raise RuntimeError(lib().jtbm_lw_last_error().decode())
-    return abi.lw_to_dict(res, shards[:h.n_shards], cr[:res.n_transfers].copy() if witness else None)
+    return abi.witness_to_dict(res, shards[:h.n_shards], cr[:res.n_transfers].copy() if witness else None)
 
 
 def check_class_witness(h: FlatHistory, algo: int = CW_SEARCH, max_nodes: int = 0, max_rounds: int = 0,
@@ -247,7 +247,7 @@ def check_class_witness(h: FlatHistory, algo: int = CW_SEARCH, max_nodes: int = 
                                         cr.ctypes.data if witness else None, C.addressof(shards), C.addressof(res))
     if rc != 0:
         raise RuntimeError(lib().jtbm_cw_last_error().decode())
-    return abi.cw_to_dict(res, shards[:h.n_shards], cr[:res.n_transfers].copy() if witness else None)
+    return abi.witness_to_dict(res, shards[:h.n_shards], cr[:res.n_transfers].copy() if witness else None)
 
 
 def check_lookup_witness(h: FlatHistory, algo: int = LK_SEARCH, max_nodes: int = 0, max_rounds: int = 0,
@@ -266,5 +266,5 @@ def check_lookup_witness(h: FlatHistory, algo: int = LK_SEARCH, max_nodes: int =
                                          C.addressof(shards), C.addressof(res))
     if rc != 0:
         raise RuntimeError(lib().jtbm_lk_last_error().decode())
-    return abi.lk_to_dict(res, shards[:h.n_shards], cr[:res.n_transfers].copy() if witness else None,
-                          lr[:nl].copy() if witness else None)
+    return abi.witness_to_dict(res, shards[:h.n_shards], cr[:res.n_transfers].copy() if witness else None,
+                               lr[:nl].copy() if witness else None)
