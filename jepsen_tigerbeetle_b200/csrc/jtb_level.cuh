@@ -15,9 +15,10 @@
 //
 //   Inside a level, a warp takes 32 configurations: phase 1, one lane per configuration, finds the candidate ops
 //   (bit masks from the frontier row); phase 2 hands EVERY child of the 32 configurations to its own lane (prefix sum
-//   + k-th-set-bit select), so all probes of the warp are in flight at once and no lane idles on a configuration with
-//   fewer children; new children are compacted in shared memory and appended to the next level 32 at a time
-//   (one atomic per 32 entries, fully coalesced stores).
+//   + k-th-set-bit select), so no lane idles on a configuration with fewer children, and each lane builds its next
+//   child and loads that child's window slot before it resolves the current one (LV_INFLIGHT probes in flight); new
+//   children are compacted in shared memory and appended to the next level 32 at a time (one atomic per 32 entries,
+//   fully coalesced stores).
 //
 //   Levels are separated by one grid barrier (monotone counter in HBM).  Narrow levels (<= narrow_max
 //   configurations: the start of every search, eager-read searches) are run by CTA 0 alone with __syncthreads()
@@ -41,6 +42,7 @@ namespace jtb {
 constexpr int LV_WARPS = JTB_LV_WARPS;
 constexpr int LV_THREADS = LV_WARPS * 32;
 constexpr int LV_STAGE = 64;        // staged new entries per warp (ring; flushed 32 at a time)
+constexpr int LV_INFLIGHT = 2;      // phase 2: window loads per lane in flight (measured on the H100: 3 is 8 % slower)
 constexpr int LV_MAX_PROBE = 128;
 constexpr int LV_CLS_WORDS = 8;     // beam mode: 64-bit words of the per-configuration class mask (512 crashed-op classes
                                     // per key); the exhaustive sweep keeps one word (64 classes, else the work list runs)
@@ -87,6 +89,7 @@ struct LvRelease {
 struct LvCtrl {
     alignas(128) LvSeg seg[3][LV_NSEG];      // append counters, three sets in rotation (input / output / spare)
     alignas(128) unsigned flags[3][32];      // result flags of the attempt whose output set is [i] (word 0 used)
+    alignas(128) unsigned next_chunk[3][32]; // chunks handed out beyond the fixed first ones, same rotation (word 0 used)
     alignas(128) LvState pub;                // state after a run of narrow levels (CTA 0 -> everyone)
     alignas(128) int n_undecided;
     int abort;                               // a grid barrier timed out (internal error)
@@ -158,13 +161,17 @@ __device__ __forceinline__ void lv_load_state(LvState& dst, const LvState* src) 
 
 // Probe + insert into the level window.  1 = inserted (new this level), 0 = already present, -1 = window exhausted.
 // A slot is free when it is empty or carries another epoch's tag (dead: every level only ever looks for its own keys).
+// idx = the key's home slot (hash_key & mask) and home = what an earlier ldcg128 of it returned: the caller issues the
+// home loads of several children before it resolves any of them.  A home value that is stale by now is harmless: a
+// free slot is only ever taken by a CAS against the value read, and a slot of this epoch is never overwritten, so a
+// stale "free" fails its CAS and goes on with what the slot holds, and a stale "taken" is still taken.
 template <int KW>
-__device__ __forceinline__ int lv_insert(uint64_t* table, uint64_t mask, const uint64_t (&k)[KW], uint64_t tag, int* plen) {
-    uint64_t idx = hash_key<KW>(k) & mask;
+__device__ __forceinline__ int lv_insert(uint64_t* table, uint64_t mask, const uint64_t (&k)[KW], uint64_t tag,
+                                         uint64_t idx, K128 home, int* plen) {
     const uint64_t mine0 = k[0] | tag;
     for (int i = 0; i < LV_MAX_PROBE; ++i) {
         uint64_t* slot = table + idx * KW;
-        K128 cur = ldcg128(slot);
+        K128 cur = i == 0 ? home : ldcg128(slot);
         for (int round = 0; round < 2; ++round) {
             const bool free_slot = !(cur.lo >> 63) || (cur.lo & LV_TAG_MASK) != tag;
             if (!free_slot) break;
@@ -405,7 +412,17 @@ __global__ void __launch_bounds__(LV_THREADS, JTB_LV_CTAS) level_search_kernel(c
         long long tp = clock64();
         if (blockIdx.x == 0 && threadIdx.x == 0) ctrl->prof[8]++;
 #endif
-        for (unsigned chunk = first_chunk; chunk < n_chunks; chunk += chunk_stride) {
+        // A warp's first chunk is fixed (first_chunk < chunk_stride covers [0, chunk_stride) once).  On a level of at least
+        // two chunks per warp the others are handed out one at a time from a counter: a warp whose chunks had few children
+        // takes more of them, so the grid reaches the barrier together instead of waiting for the warp with the most work.
+        const bool dyn = n_chunks >= 2u * chunk_stride;
+        auto next_chunk = [&](unsigned chunk) -> unsigned {
+            if (!dyn) return chunk + chunk_stride;
+            unsigned c = 0;
+            if (lane == 0) c = atomicAdd(&ctrl->next_chunk[a.s_out][0], 1u);
+            return chunk_stride + __shfl_sync(FULL, c, 0);
+        };
+        for (unsigned chunk = first_chunk; chunk < n_chunks; chunk = next_chunk(chunk)) {
             // ---------------- phase 1: lane = configuration ------------------------------------------------
             const unsigned long long idx = (unsigned long long)chunk * G + lane;
             const bool have = (unsigned)lane < G && idx < a.n_in;
@@ -482,103 +499,144 @@ __global__ void __launch_bounds__(LV_THREADS, JTB_LV_CTAS) level_search_kernel(c
             const unsigned total = __shfl_sync(FULL, incl, 31);
             if (lane == 0) S.start[32] = total;
             __syncwarp();
-            // ---------------- phase 2: lane = child ------------------------------------------------------------
-            for (unsigned g0 = 0; g0 < total; g0 += 32) {
-                const unsigned g = g0 + lane;
-                const bool act = g < total;
-                Child<KW> ch;
-                bool is_new = false;
-                int owner = 0;
-                unsigned child_crashed = 0;
-                if (act) {
+            // ---------------- phase 2: lane = child, LV_INFLIGHT rounds in flight -----------------------------------
+            // Round r hands child 32 r + lane to the lane.  Iteration r builds the key of round r's child and issues the
+            // load of its home slot, and only then resolves the child of round r - (LV_INFLIGHT - 1) (CAS, bookkeeping,
+            // staging) from the home slot loaded that many iterations earlier: a lane has LV_INFLIGHT window loads in
+            // flight instead of one.  Two children with equal keys, of one round or of two, still make one insert: the
+            // later one's CAS fails against the earlier one's write and finds its key there (lv_insert).
+            constexpr int NB = LV_INFLIGHT, NEW = NB - 1;   // [NEW] = the child being built, [0] = the one being resolved
+            Child<KW> ch[NB];
+            K128 home[NB];          // the child's home slot, as loaded
+            unsigned src[NB];       // owner | 32 (a crashed-op class) | slot or class << 6
+            unsigned crashed[NB];   // beam mode: crashed ops the child has consumed
+            bool probe[NB];         // the child goes into the window (its home slot was loaded)
+#pragma unroll
+            for (int q = 0; q < NB; ++q) { src[q] = 0; crashed[q] = 0; probe[q] = false; }
+            for (unsigned g0 = 0; g0 < total + 32 * NEW; g0 += 32) {
+#pragma unroll
+                for (int q = 0; q < NEW; ++q) {
+                    ch[q] = ch[q + 1]; home[q] = home[q + 1]; src[q] = src[q + 1]; crashed[q] = crashed[q + 1]; probe[q] = probe[q + 1];
+                }
+                probe[NEW] = false; src[NEW] = 0; crashed[NEW] = 0;
+                do {   // build round g0 / 32's child and load its home slot
+                    const unsigned g = g0 + lane;
+                    if (g >= total) break;
                     int lo = 0, hi = 32;       // largest o with start[o] <= g
                     while (hi - lo > 1) {
                         const int mid = (lo + hi) >> 1;
                         if (S.start[mid] <= g) lo = mid; else hi = mid;
                     }
-                    owner = lo;
-                    const int k = (int)(g - S.start[owner]);
+                    const int k = (int)(g - S.start[lo]);
                     Expander<MODEL, KW, EAGER> Y;
 #pragma unroll
-                    for (int i = 0; i < KW; ++i) Y.w[i] = S.w[owner][i];
+                    for (int i = 0; i < KW; ++i) Y.w[i] = S.w[lo][i];
                     if constexpr (BAL && !NEGOK) {
 #pragma unroll
-                        for (int i = 0; i < 8; ++i) Y.bal[i] = S.bal[owner][i];
+                        for (int i = 0; i < 8; ++i) Y.bal[i] = S.bal[lo][i];
                     }
-                    Y.rd_ok = S.rd_ok[owner];
+                    Y.rd_ok = S.rd_ok[lo];
                     Y.gj = (int)((Y.w[0] >> 32) & XRANK_MASK);
                     Y.reg = (int32_t)(uint32_t)Y.w[0];
                     Y.row = T.rows + (size_t)Y.gj * T.row_words;
-                    Y.fr_pos = S.hdr[owner][0]; Y.shard = S.hdr[owner][1]; Y.gj_end = S.hdr[owner][2];
-                    Y.cls_base = S.hdr[owner][3]; Y.rslot = S.hdr[owner][4]; Y.ncls = S.hdr[owner][5];
-                    const uint64_t otodo = S.todo[owner];
+                    Y.fr_pos = S.hdr[lo][0]; Y.shard = S.hdr[lo][1]; Y.gj_end = S.hdr[lo][2];
+                    Y.cls_base = S.hdr[lo][3]; Y.rslot = S.hdr[lo][4]; Y.ncls = S.hdr[lo][5];
+                    const uint64_t otodo = S.todo[lo];
                     const int ns = __popcll(otodo);
                     bool ok;
-                    int t_slot = 0;
-                    if constexpr (BEAM) child_crashed = S.crashed[owner] + (k >= ns ? 1u : 0u);
-                    if (k < ns) { t_slot = select64(otodo, k); ok = Y.child_slot(T, t_slot, neg_ok, ch, true); }
-                    else {   // (k - ns)-th candidate class: find its word, then the bit
+                    if constexpr (BEAM) crashed[NEW] = S.crashed[lo] + (k >= ns ? 1u : 0u);
+                    if (k < ns) {
+                        const int t = select64(otodo, k);
+                        src[NEW] = (unsigned)lo | (unsigned)t << 6;
+                        ok = Y.child_slot(T, t, neg_ok, ch[NEW], true);
+                    } else {   // (k - ns)-th candidate class: find its word, then the bit
                         int kk = k - ns, cw = 0;
                         for (; cw < CLS_WORDS - 1; ++cw) {
-                            const int pc = __popcll(S.cls_todo[owner][cw]);
+                            const int pc = __popcll(S.cls_todo[lo][cw]);
                             if (kk < pc) break;
                             kk -= pc;
                         }
-                        ok = Y.child_class(T, cw * 64 + select64(S.cls_todo[owner][cw], kk), neg_ok, ch);
+                        const int ci = cw * 64 + select64(S.cls_todo[lo][cw], kk);
+                        src[NEW] = (unsigned)lo | 32u | (unsigned)ci << 6;
+                        ok = Y.child_class(T, ci, neg_ok, ch[NEW]);
                     }
-                    if (ok) {
-                        if (ch.done) {
-                            // every :ok op of the shard is linearized -> VALID
-                            if (atomicExch(&p.shard_found[Y.shard], 1) == 0) {
-                                if (atomicSub(&ctrl->n_undecided, 1) == 1) atomicOr(res_flags, LV_F_DECIDED);
-                            }
-                        } else {
-                            int plen;
-                            const int r = lv_insert<KW>(p.table, wmask, ch.w, tag, &plen);
-                            my_probes++;
-                            my_max_probe = max(my_max_probe, plen);
-                            if (r < 0) atomicOr(res_flags, LV_F_RETRY);
-                            is_new = r == 1;
-                            if constexpr (BAL) {
-                                if (is_new && ch.d < 0) Y.load_transfer(t_slot, ch);   // only NEW children need the transfer
-                            }
-                            if (is_new && ch.cgj > Y.gj && (wit_shard != Y.shard || wit_rank < ch.cgj)) {
-                                wit_shard = Y.shard; wit_rank = ch.cgj;   // furthest frontier reached: the witness
-                                atomicMax(&p.shard_max_rank[Y.shard], ch.cgj);
-                            }
-                            if (BEAM && is_new) {
-                                // priority of the child RELATIVE TO THE INPUT LEVEL's best of its shard (the output level's
-                                // own best is only known when the level is complete), and the trackers of the output level
-                                LvBeam* bm = p.beam;
-                                const int key = lv_beam_key((int)child_crashed, __ldcg(&bm->min_crashed[a.s_in][Y.shard]), ch.cgj,
-                                                            __ldcg(&bm->max_rank[a.s_in][Y.shard]));
-                                atomicAdd(&bm->hist[a.s_out][key], 1u);
-                                child_crashed = min(child_crashed, 0xffffu) | ((unsigned)key << 16);
-                                if (bt_shard != Y.shard) { bt_shard = Y.shard; bt_min = 0x7fffffff; bt_max = -1; }
-                                const int cc = (int)(child_crashed & 0xffffu);
-                                if (cc < bt_min) { bt_min = cc; atomicMin(&bm->min_crashed[a.s_out][Y.shard], bt_min); }
-                                if (ch.cgj > bt_max) { bt_max = ch.cgj; atomicMax(&bm->max_rank[a.s_out][Y.shard], bt_max); }
-                            }
+                    if (!ok) break;
+                    if (ch[NEW].done) {
+                        // every :ok op of the shard is linearized -> VALID
+                        if (atomicExch(&p.shard_found[Y.shard], 1) == 0) {
+                            if (atomicSub(&ctrl->n_undecided, 1) == 1) atomicOr(res_flags, LV_F_DECIDED);
                         }
+                    } else {
+                        probe[NEW] = true;
+                        home[NEW] = ldcg128(p.table + (hash_key<KW>(ch[NEW].w) & wmask) * KW);
                     }
-                }
-                // ---- stage the new children; append 32 at a time ----
-                const unsigned newm = __ballot_sync(FULL, is_new);
-                if (newm) {
-                    if (is_new) {
-                        const unsigned r = (stg_tail + __popc(newm & lt_mask)) % LV_STAGE;
-                        uint64_t* e = S.stage[r];
-                        if constexpr (BEAM) S.stage_aux[r] = child_crashed;
-#pragma unroll
-                        for (int i = 0; i < KW; ++i) e[i] = ch.w[i];
+                } while (0);
+                if (g0 >= 32 * NEW) {   // round g0 / 32 - NEW, warp-uniform
+                    bool is_new = false;
+                    const int o = (int)(src[0] & 31);
+                    int32_t amt = 0, d = 0, c = 0;   // bank: the transfer the child applies to its parent's balances
+                    if (probe[0]) {
+                        const int shard = S.hdr[o][1];
+                        const int gj = (int)((S.w[o][0] >> 32) & XRANK_MASK);
+                        const int cgj = (int)((ch[0].w[0] >> 32) & XRANK_MASK);   // = ch[0].cgj
+                        int plen;
+                        // the home index is hashed again rather than held from the load: it saves two registers
+                        const int r = lv_insert<KW>(p.table, wmask, ch[0].w, tag, hash_key<KW>(ch[0].w) & wmask, home[0], &plen);
+                        my_probes++;
+                        my_max_probe = max(my_max_probe, plen);
+                        if (r < 0) atomicOr(res_flags, LV_F_RETRY);
+                        is_new = r == 1;
                         if constexpr (BAL) {
-                            S.stage_mv[r] = (unsigned)owner | ((unsigned)(ch.d & 7) << 5) | ((unsigned)(ch.c & 7) << 8);
-                            S.stage_amt[r] = ch.amt;
+                            // only NEW children need the transfer; it is read again from the record child_slot /
+                            // child_class took it from rather than held from one iteration to the next (a read applies
+                            // none)
+                            const int t = (int)(src[0] >> 6);
+                            if (is_new && (src[0] & 32)) {
+                                const I4 op = ld_i4(reinterpret_cast<const int32_t*>(T.classes + S.hdr[o][3] + t));
+                                amt = op.y; d = op.z; c = op.w;
+                            } else if (is_new && !((S.rd_ok[o] >> t) & 1ull)) {
+                                Expander<MODEL, KW, EAGER> Y;
+                                Y.row = T.rows + (size_t)gj * T.row_words;
+                                Y.load_transfer(t, ch[0]);
+                                amt = ch[0].amt; d = ch[0].d; c = ch[0].c;
+                            }
+                        }
+                        if (is_new && cgj > gj && (wit_shard != shard || wit_rank < cgj)) {
+                            wit_shard = shard; wit_rank = cgj;   // furthest frontier reached: the witness
+                            atomicMax(&p.shard_max_rank[shard], cgj);
+                        }
+                        if (BEAM && is_new) {
+                            // priority of the child RELATIVE TO THE INPUT LEVEL's best of its shard (the output level's
+                            // own best is only known when the level is complete), and the trackers of the output level
+                            LvBeam* bm = p.beam;
+                            const int key = lv_beam_key((int)crashed[0], __ldcg(&bm->min_crashed[a.s_in][shard]),
+                                                        cgj, __ldcg(&bm->max_rank[a.s_in][shard]));
+                            atomicAdd(&bm->hist[a.s_out][key], 1u);
+                            crashed[0] = min(crashed[0], 0xffffu) | ((unsigned)key << 16);
+                            if (bt_shard != shard) { bt_shard = shard; bt_min = 0x7fffffff; bt_max = -1; }
+                            const int cc = (int)(crashed[0] & 0xffffu);
+                            if (cc < bt_min) { bt_min = cc; atomicMin(&bm->min_crashed[a.s_out][shard], bt_min); }
+                            if (cgj > bt_max) { bt_max = cgj; atomicMax(&bm->max_rank[a.s_out][shard], bt_max); }
                         }
                     }
-                    stg_tail += __popc(newm);
-                    __syncwarp();
-                    if (stg_tail - stg_head >= 32) flush(32);
+                    // ---- stage the new children; append 32 at a time ----
+                    const unsigned newm = __ballot_sync(FULL, is_new);
+                    if (newm) {
+                        if (is_new) {
+                            const unsigned r = (stg_tail + __popc(newm & lt_mask)) % LV_STAGE;
+                            uint64_t* e = S.stage[r];
+                            if constexpr (BEAM) S.stage_aux[r] = crashed[0];
+#pragma unroll
+                            for (int i = 0; i < KW; ++i) e[i] = ch[0].w[i];
+                            if constexpr (BAL) {
+                                S.stage_mv[r] = (unsigned)o | ((unsigned)(d & 7) << 5) | ((unsigned)(c & 7) << 8);
+                                S.stage_amt[r] = amt;
+                            }
+                        }
+                        stg_tail += __popc(newm);
+                        __syncwarp();
+                        if (stg_tail - stg_head >= 32) flush(32);
+                    }
                 }
             }
             // the staged balances are built from this chunk's S.bal: flush before the next chunk overwrites it
@@ -681,7 +739,7 @@ __global__ void __launch_bounds__(LV_THREADS, JTB_LV_CTAS) level_search_kernel(c
     auto reset_spare = [&](const LvState& a) {   // by ONE warp, during the attempt: the set nobody reads or writes now
         ctrl->seg[a.s_spare][lane].n = 0;
         ctrl->seg[a.s_spare][lane + 32].n = 0;
-        if (lane == 0) ctrl->flags[a.s_spare][0] = 0;
+        if (lane == 0) { ctrl->flags[a.s_spare][0] = 0; ctrl->next_chunk[a.s_spare][0] = 0; }
         if constexpr (BEAM) {
             for (int i = lane; i < LV_BEAM_BINS; i += 32) p.beam->hist[a.s_spare][i] = 0;
             if (lane < LV_BEAM_SHARDS) { p.beam->min_crashed[a.s_spare][lane] = 0x7fffffff; p.beam->max_rank[a.s_spare][lane] = -1; }
