@@ -1051,6 +1051,20 @@ typedef struct jtb_edn_checks {
 int  jtb_ledger_edn_checks(jtb_ctx* ctx, const char* text, int64_t n_bytes, int32_t flags, jtb_edn_checks* out);
 void jtb_edn_checks_free(jtb_edn_checks* out);
 
+/* ---- K20: a stored set-full history.edn read on the device ----------------------------------------------------- *
+ * The bytes of a set-full history.edn (set_full.clj:29-45, 107-134; the EDN subset and op fields of K18) flattened into
+ * the keyed set form: exactly the arrays of edn.read_history(text, independent=True) + history.flatten_ops(ops, "set").
+ * A 2-element vector or list :value is a jepsen.independent tuple [key value]; each integer key is one shard, in
+ * ascending key order, and the events whose key is nil or whose :value is not a tuple form the last shard, key id -1
+ * (even when a real key -1 exists).  An :add of a nil value is dropped; a :read of nil has payload_len -1, of a set
+ * literal its members sorted ascending, of a vector or list its members in order.  multi_transfer_txns is 0.  Refused
+ * (rc < 0, jtb_last_error naming the first offending byte): whatever K18 refuses about the EDN and the op fields, :f
+ * other than :add or :read on a client op, a key that is not an integer or nil or lies outside int64, an add value or
+ * member that is not an integer or lies outside int32, a read value that is not nil or a collection, a set literal with
+ * a repeated member, and more than 2^31 - 3 members.  Release the arrays with jtb_edn_history_free.  flags is reserved
+ * and must be 0. */
+int  jtb_read_set_edn(jtb_ctx* ctx, const char* text, int64_t n_bytes, int32_t flags, jtb_edn_history* out);
+
 /* ---- multi-GPU fan-out inside the library (SURVEY §8(b) `n_gpus`, §8(e)) ----------------------------------- *
  * What `independent/checker` (set_full.clj:155) does over JVM threads, done over the GPUs of one box for a host
  * that is a single process (a JVM through JNI): the shards (independent keys) of the history are partitioned over

@@ -91,15 +91,12 @@ class StoredOp(Mapping):
         return repr(self._op) if self._op is not None else f"StoredOp(bytes {self._begin}..{self._end})"
 
 
-class StoredLedgerHistory:
-    """A stored ledger history.edn (a path or its bytes) that the ledger checks read on the GPU (K18, K19).
+class _StoredHistory:
+    """The bytes of a stored history.edn (a path or its bytes), the native.Context the device reads them on (None opens
+    one on device 0 when the device is first needed), and the op maps of `edn.read_history` for the checkers that
+    iterate it (parsed once, on first use, and cached)."""
 
-    `_flat` asks it for the "bank", "ledger-counters" or "ledger-lookups" form and gets the device reader's FlatHistory,
-    read once per form and cached, instead of flattening op maps in Python.  The host checkers of a `ledger_checker()`
-    compose (unexpected-ops, final-reads, lookup-transfers) and stats build their results from one device summary
-    (`checks()`, K19), whose flagged ops are `StoredOp`s parsed only when read.  When the device refuses the file they
-    iterate it instead: iterating yields the op maps of `edn.read_history` (parsed once, on first use, and cached).
-    ctx: the native.Context to read on; None opens one on device 0 when the device is first needed."""
+    _independent = False   # read_history(..., independent=): whether 2-vector :values are [key value] tuples
 
     def __init__(self, path_or_bytes, ctx=None) -> None:
         if isinstance(path_or_bytes, (bytes, bytearray, memoryview)):
@@ -110,13 +107,42 @@ class StoredLedgerHistory:
         self._ctx = ctx
         self._forms: dict[str, FlatHistory] = {}
         self._ops: list | None = None
-        self._checks: dict | None = None
 
     def _context(self):
         if self._ctx is None:
             from .native import Context
             self._ctx = Context(device=0)
         return self._ctx
+
+    def ops(self) -> list:
+        if self._ops is None:
+            from .edn import read_history
+            self._ops = read_history(self.data.decode(), independent=self._independent)
+        return self._ops
+
+    def __iter__(self):
+        return iter(self.ops())
+
+    def __len__(self) -> int:
+        return len(self.ops())
+
+    def __getitem__(self, i):
+        return self.ops()[i]
+
+
+class StoredLedgerHistory(_StoredHistory):
+    """A stored ledger history.edn (a path or its bytes) that the ledger checks read on the GPU (K18, K19).
+
+    `_flat` asks it for the "bank", "ledger-counters" or "ledger-lookups" form and gets the device reader's FlatHistory,
+    read once per form and cached, instead of flattening op maps in Python.  The host checkers of a `ledger_checker()`
+    compose (unexpected-ops, final-reads, lookup-transfers) and stats build their results from one device summary
+    (`checks()`, K19), whose flagged ops are `StoredOp`s parsed only when read.  When the device refuses the file they
+    iterate it instead: iterating yields the op maps of `edn.read_history` (parsed once, on first use, and cached).
+    ctx: the native.Context to read on; None opens one on device 0 when the device is first needed."""
+
+    def __init__(self, path_or_bytes, ctx=None) -> None:
+        super().__init__(path_or_bytes, ctx)
+        self._checks: dict | None = None
 
     def flat(self, form: str) -> FlatHistory:
         if form not in self._forms:
@@ -130,20 +156,31 @@ class StoredLedgerHistory:
             self._checks = self._context().ledger_edn_checks(self.data)
         return None if self._checks["refused"] else self._checks
 
-    def ops(self) -> list:
-        if self._ops is None:
-            from .edn import read_history
-            self._ops = read_history(self.data.decode())
-        return self._ops
 
-    def __iter__(self):
-        return iter(self.ops())
+class StoredSetHistory(_StoredHistory):
+    """A stored set-full history.edn (a path or its bytes) that the set checks read on the GPU (K20).
 
-    def __len__(self) -> int:
-        return len(self.ops())
+    `_flat` asks it for the "set" form, which SetFull, ReadAllInvokedAdds, `independent_checker` and
+    `linearizable({"model": "set"})` read, and gets the device reader's keyed FlatHistory (`Context.read_set_edn`), read
+    once and cached, instead of flattening op maps in Python.  When the device refuses the file (`refused` then holds
+    its reason), and for any other model, the op maps are flattened instead; iterating yields them: those of
+    `edn.read_history(text, independent=True)`, so a 2-element :value is a (key, value) tuple.
+    ctx: the native.Context to read on; None opens one on device 0 when the device is first needed."""
 
-    def __getitem__(self, i):
-        return self.ops()[i]
+    _independent = True
+    refused: str | None = None
+
+    def flat(self, form: str = "set") -> FlatHistory:
+        if form != "set":
+            raise ValueError(f"a stored set history is read on the device in the set form only, not {form!r}")
+        if form not in self._forms:
+            from .native import EdnRefused
+            try:
+                self._forms[form] = self._context().read_set_edn(self.data)
+            except EdnRefused as e:
+                self.refused = str(e)
+                self._forms[form] = flatten_ops(self.ops(), "set")
+        return self._forms[form]
 
 
 def _summary(history) -> dict | None:
@@ -161,6 +198,8 @@ def _flat(history, model: str) -> FlatHistory:
         if model in ("bank", "ledger-counters", "ledger-lookups"):
             return history.flat(model)
         return flatten_ops(history.ops(), model)
+    if isinstance(history, StoredSetHistory):
+        return history.flat(model) if model == "set" else flatten_ops(history.ops(), model)
     return flatten_ops(history, model)
 
 
@@ -1268,3 +1307,15 @@ def ledger_checker(checker_opts: Mapping[str, Any] | None = None, ctx: Context |
     if lookup_witness:
         cs["lookup-witness"] = lookup_witness_checker(ctx=ctx)
     return compose(cs)
+
+
+def set_full_workload_checker(ctx: Context | None = None) -> Independent:
+    """The set-full workload's checker (workloads/set_full.clj:155-158) on one context:
+        (independent/checker (checker/compose {:set-full (checker/set-full {:linearizable? true})
+                                               :read-all-invoked-adds (read-all-invoked-adds)}))
+    It is the set-full counterpart of `ledger_checker()`; given a `StoredSetHistory`, it reads the file on the device.
+    ctx: the context both checkers run on; None opens one on device 0 now."""
+    if ctx is None:
+        ctx = Context(device=0)
+    return independent_checker(compose({"set-full": set_full({"linearizable?": True}, ctx=ctx),
+                                        "read-all-invoked-adds": read_all_invoked_adds(ctx=ctx)}))

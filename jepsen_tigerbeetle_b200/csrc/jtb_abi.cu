@@ -31,6 +31,7 @@
 #include "jtb_witness.cuh"
 #include "jtb_edn.cuh"
 #include "jtb_edn_checks.cuh"
+#include "jtb_set_edn.cuh"
 
 using namespace jtb;
 
@@ -1283,6 +1284,15 @@ int jtb_ledger_edn_checks(jtb_ctx* ctx, const char* text, int64_t n_bytes, int32
 
 void jtb_edn_checks_free(jtb_edn_checks* out) {
     if (out) jtb_edn_checks_release(out);
+}
+
+// K20: a stored set-full history.edn read on the device (csrc/jtb_set_edn.cuh)
+int jtb_read_set_edn(jtb_ctx* ctx, const char* text, int64_t n_bytes, int32_t flags, jtb_edn_history* out) {
+    if (!ctx) return -1;
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    if (cudaSetDevice(ctx->device) != cudaSuccess) { ctx->err = "cudaSetDevice failed"; return -1; }
+    ctx->fc.valid = false;
+    return run_read_set_edn(ctx->stream, ctx->ev0, ctx->ev1, text, n_bytes, flags, out, ctx->err);
 }
 
 // SURVEY 8(f) N2: the step before the checkers (independent/subhistory, ledger->bank) on the device

@@ -11,7 +11,8 @@
 //      gives, per byte, whether it lies inside a string.
 //   2. depth: an inclusive sum of +1 per open ([ { ( and the { of #{) and -1 per close outside strings.  Bracket
 //      pairing is checked by a stable radix sort of the brackets by level: each level then alternates open, close.
-//   3. form starts (opens, strings, tokens that are not tags) at depth <= 3 are compacted; the top-level count decides
+//   3. form starts (opens, strings, tokens that are not tags) at depth <= 3 (K20, jtb_set_edn.cuh, reads one level
+//      deeper) are compacted; the top-level count decides
 //      between one-op-per-form and one-vector files (base depth 0 or 1).  Ops are the form starts at the base depth,
 //      their keys and values those at base + 1, micro-ops those at base + 2.
 //   4. one thread per map entry records where each of the seven op keys' value is; a thread per op then reads those
@@ -267,18 +268,19 @@ __device__ __forceinline__ int edn_depth_before(const char* t, const int* depth,
     return depth[i] - (edn_open(t[i]) ? 1 : 0);
 }
 
-struct EdnFormStart {   // an open, an opening quote or a token that is not a tag, at depth <= 3
+struct EdnFormStart {   // an open, an opening quote or a token that is not a tag, at depth <= max_depth
     const char* t;
     const uint8_t* par;
     const int* depth;
+    int max_depth;      // 3 for the ledger forms; the set form's members sit one level deeper
     __device__ bool operator()(int64_t i) const {
         const char c = t[i];
-        if (par[i]) return c == '"' && (i == 0 || !par[i - 1]) && depth[i] <= 3;
+        if (par[i]) return c == '"' && (i == 0 || !par[i - 1]) && depth[i] <= max_depth;
         if (c == '"') return false;
-        if (edn_open(c)) return depth[i] - 1 <= 3;
+        if (edn_open(c)) return depth[i] - 1 <= max_depth;
         if (edn_delim(c) || c == '#') return false;
         if (i > 0 && !edn_delim(t[i - 1])) return false;
-        return depth[i] <= 3;
+        return depth[i] <= max_depth;
     }
 };
 
@@ -339,22 +341,16 @@ __global__ void edn_key_kernel(const char* t, const int64_t* ch, int64_t n_ch, c
     if (k >= 0) atomicMax(&field[(int64_t)o * EK_N + k], (int32_t)j + 2);   // the value's index + 1; the last key wins
 }
 
-__global__ void edn_op_kernel(const char* t, int64_t n, const int64_t* ops, int64_t n_ops, const int64_t* ch,
-                              const int32_t* n_child, const int32_t* field, EdnOp* out, unsigned long long* err) {
-    const int64_t o = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-    if (o >= n_ops) return;
-    const int64_t pos = ops[o];
-    EdnOp op{};
-    op.value_child = -1;
-    op.first_item = INT_MAX;
-    op.plen = -1;
-    const int32_t* fo = field + o * EK_N;
+// The fields every form reads from op o's map: :type, :time, :process and, for a client op, :index and :final?.  False
+// when the map has an odd number of forms (refused; the op stays a non-client op, so no later pass reads its fields).
+__device__ __forceinline__ bool edn_op_fields(const char* t, int64_t n, int64_t o, int64_t pos, const int64_t* ch,
+                                              const int32_t* n_child, const int32_t* fo, EdnOp& op,
+                                              unsigned long long* err) {
     int64_t v = 0;
     if (t[pos] != '{' || (pos > 0 && t[pos - 1] == '#')) edn_fail(err, pos, EE_NOT_MAP);
-    if (n_child[o] & 1) {   // refused; the op stays a non-client op, so no later pass reads its fields
+    if (n_child[o] & 1) {
         edn_fail(err, pos, EE_ODD_MAP);
-        out[o] = op;
-        return;
+        return false;
     }
     // :type (every op)
     if (!fo[EK_TYPE]) {
@@ -401,6 +397,26 @@ __global__ void edn_op_kernel(const char* t, int64_t n, const int64_t* ops, int6
             if (truthy < 0) edn_fail(err, p, EE_NUMBER);
             else if (truthy) op.flags = JTB_FLAG_FINAL;
         }
+    }
+    return true;
+}
+
+__global__ void edn_op_kernel(const char* t, int64_t n, const int64_t* ops, int64_t n_ops, const int64_t* ch,
+                              const int32_t* n_child, const int32_t* field, EdnOp* out, unsigned long long* err) {
+    const int64_t o = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    if (o >= n_ops) return;
+    const int64_t pos = ops[o];
+    EdnOp op{};
+    op.value_child = -1;
+    op.first_item = INT_MAX;
+    op.plen = -1;
+    const int32_t* fo = field + o * EK_N;
+    int64_t v = 0;
+    if (!edn_op_fields(t, n, o, pos, ch, n_child, fo, op, err)) {
+        out[o] = op;
+        return;
+    }
+    if (op.client) {
         if (!fo[EK_F] || !edn_is(t, ch[fo[EK_F] - 1], ":txn", 4)) edn_fail(err, fo[EK_F] ? ch[fo[EK_F] - 1] : pos, EE_F);
         op.vkind = VK_NIL;
         if (fo[EK_VALUE]) {
@@ -737,12 +753,15 @@ struct EdnParse {
     size_t tmp_cap = 0, bytes = 0;
     int64_t* d_cnt = nullptr;           // 4 counters for reductions and selections
     char* text = nullptr;               // the text, padded with 64 spaces
+    int* depth = nullptr;               // per byte: the bracket depth (an open counts itself)
     int64_t N = 0;                      // max(n, 1)
     unsigned long long* err = nullptr;  // [0] the first error (byte << 8 | EdnErr), [1] multi-transfer txns
     int base = 0;                       // the depth of the op maps (1: one vector of ops)
     uint32_t* lv2 = nullptr;            // the brackets sorted by (level, position): levels ...
     int64_t *br2 = nullptr, nb = 0;     // ... and positions; pairs (2k, 2k + 1) match
+    int64_t *forms = nullptr, nf = 0;   // every form start at depth <= the reader's limit
     int64_t *ops = nullptr, n_ops = 0, *ch = nullptr, n_ch = 0, *it_pos = nullptr, n_it = 0;
+    int32_t* n_child = nullptr;         // per op: its map's forms
     int32_t* field = nullptr;           // per op and EK_*: the child index of the key's value + 1, 0 absent
     EdnOp* op = nullptr;
     EdnItem* items = nullptr;
@@ -800,12 +819,12 @@ struct EdnRefusal {
     void set(unsigned long long w) { at = (int64_t)(w >> 8); reason = edn_err_text((uint32_t)(w & 0xff)); }
 };
 
-// Passes 1–5 on text[0, n) read as `form`: the text copied to the device (P.t_h2d, then ev0 recorded), string state,
-// depth, bracket pairing, form starts, op keys and fields, micro-ops, tags, the per-process sort (ledger-lookups), and
-// the events' and payload's checks.  Returns 0 (r.reason set when the input is refused: the first error in the file) or
+// Passes 1–4 on text[0, n), shared by every reader: the text copied to the device (P.t_h2d, then ev0 recorded), string
+// state, depth, bracket pairing, the form starts at depth <= max_depth, ops, their map entries and the forms one level
+// below those, and where each op's keys are (P.n_child, P.field).  Returns 0 (r.reason set when the input is refused) or
 // -1 with err on a CUDA or allocation error.
-inline int edn_parse(EdnParse& P, cudaEvent_t ev0, const char* text, int64_t n, int32_t form, EdnRefusal& r,
-                     std::string& err) {
+inline int edn_parse_forms(EdnParse& P, cudaEvent_t ev0, const char* text, int64_t n, int max_depth, EdnRefusal& r,
+                           std::string& err) {
     cudaStream_t st = P.st;
     CallAllocs& A = P.A;
     const int T = 256;
@@ -828,6 +847,7 @@ inline int edn_parse(EdnParse& P, cudaEvent_t ev0, const char* text, int64_t n, 
     int* depth;
     JTB_OK(A.alloc(&par, (size_t)N));
     JTB_OK(A.alloc(&depth, (size_t)N));
+    P.depth = depth;
     JTB_OK(A.alloc(&P.d_cnt, 4));
     int64_t* d_cnt = P.d_cnt;
     auto cnt = thrust::counting_iterator<int64_t>(0);
@@ -880,8 +900,9 @@ inline int edn_parse(EdnParse& P, cudaEvent_t ev0, const char* text, int64_t n, 
     }
 
     // ---- 3: form starts, the base depth, ops, their children and micro-ops ------------------------------------------
-    int64_t *forms, nf = 0;
-    JTB_OK(P.select(cnt, N, EdnFormStart{d_text, par, depth}, &forms, &nf));
+    JTB_OK(P.select(cnt, N, EdnFormStart{d_text, par, depth, max_depth}, &P.forms, &P.nf));
+    const int64_t* forms = P.forms;
+    const int64_t nf = P.nf;
     int base = 0;
     if (nf) {
         int* d_top = (int*)d_cnt;
@@ -903,33 +924,57 @@ inline int edn_parse(EdnParse& P, cudaEvent_t ev0, const char* text, int64_t n, 
     JTB_OK(P.select(forms, nf, EdnAtDepth{d_text, depth, base}, &P.ops, &P.n_ops));
     JTB_OK(P.select(forms, nf, EdnAtDepth{d_text, depth, base + 1}, &P.ch, &P.n_ch));
     JTB_OK(P.select(forms, nf, EdnAtDepth{d_text, depth, base + 2}, &P.it_pos, &P.n_it));
-    const int64_t *ops = P.ops, *ch = P.ch, *it_pos = P.it_pos;
+    const int64_t *ops = P.ops, *ch = P.ch;
     const int64_t n_ops = P.n_ops, n_ch = P.n_ch, n_it = P.n_it;
     if (n_ops >= INT_MAX || n_ch >= INT_MAX - 2 || n_it >= INT_MAX) {
         r.reason = "more than 2^31 - 3 ops, map entries or micro-ops";
         return 0;
     }
 
-    // ---- 4: op keys and fields ----------------------------------------------------------------------------------------
-    int32_t *ch_op, *first_child, *n_child;
+    // ---- 4: op keys ---------------------------------------------------------------------------------------------------
+    int32_t *ch_op, *first_child;
     JTB_OK(A.alloc(&ch_op, (size_t)n_ch));
     JTB_OK(A.alloc(&first_child, (size_t)n_ops));
-    JTB_OK(A.alloc(&n_child, (size_t)n_ops));
+    JTB_OK(A.alloc(&P.n_child, (size_t)n_ops));
     JTB_OK(A.alloc(&P.field, (size_t)n_ops * EK_N));
     JTB_OK(A.alloc(&P.op, (size_t)n_ops));
+    JTB_OK(cudaMemsetAsync(first_child, 0x7f, (size_t)n_ops * 4, st));
+    JTB_OK(cudaMemsetAsync(P.n_child, 0, (size_t)n_ops * 4, st));
+    JTB_OK(cudaMemsetAsync(P.field, 0, (size_t)n_ops * EK_N * 4, st));
+    if (n_ops && n_ch) {
+        edn_child_kernel<<<edn_blocks(n_ch), T, 0, st>>>(ops, n_ops, ch, n_ch, ch_op, first_child, P.n_child);
+        edn_key_kernel<<<edn_blocks(n_ch), T, 0, st>>>(d_text, ch, n_ch, ch_op, first_child, P.field);
+        JTB_OK(cudaGetLastError());
+    }
+    return 0;
+}
+
+// Passes 1–5 on text[0, n) read as `form`: edn_parse_forms (form starts at depth <= 3), then the op fields, micro-ops,
+// tags, the per-process sort (ledger-lookups), and the events' and payload's checks.  Returns 0 (r.reason set when the
+// input is refused: the first error in the file) or -1 with err on a CUDA or allocation error.
+inline int edn_parse(EdnParse& P, cudaEvent_t ev0, const char* text, int64_t n, int32_t form, EdnRefusal& r,
+                     std::string& err) {
+    if (edn_parse_forms(P, ev0, text, n, 3, r, err) != 0) return -1;
+    if (r.reason) return 0;
+    cudaStream_t st = P.st;
+    CallAllocs& A = P.A;
+    const int T = 256;
+    const int64_t N = P.N;
+    char* d_text = P.text;
+    unsigned long long* d_err = P.err;
+    int64_t* d_cnt = P.d_cnt;
+    size_t& bytes = P.bytes;
+    unsigned long long w = ~0ull;
+    const int64_t *ops = P.ops, *ch = P.ch, *it_pos = P.it_pos;
+    const int64_t n_ops = P.n_ops, n_ch = P.n_ch, n_it = P.n_it;
     int32_t* field = P.field;
     EdnOp* op = P.op;
-    JTB_OK(cudaMemsetAsync(first_child, 0x7f, (size_t)n_ops * 4, st));
-    JTB_OK(cudaMemsetAsync(n_child, 0, (size_t)n_ops * 4, st));
-    JTB_OK(cudaMemsetAsync(field, 0, (size_t)n_ops * EK_N * 4, st));
+
+    // ---- 4: op fields ---------------------------------------------------------------------------------------------
     unsigned long long* d_multi = d_err + 1;
     JTB_OK(cudaMemsetAsync(d_multi, 0, 8, st));
     if (n_ops) {
-        if (n_ch) {
-            edn_child_kernel<<<edn_blocks(n_ch), T, 0, st>>>(ops, n_ops, ch, n_ch, ch_op, first_child, n_child);
-            edn_key_kernel<<<edn_blocks(n_ch), T, 0, st>>>(d_text, ch, n_ch, ch_op, first_child, field);
-        }
-        edn_op_kernel<<<edn_blocks(n_ops), T, 0, st>>>(d_text, N, ops, n_ops, ch, n_child, field, op, d_err);
+        edn_op_kernel<<<edn_blocks(n_ops), T, 0, st>>>(d_text, N, ops, n_ops, ch, P.n_child, field, op, d_err);
         JTB_OK(cudaGetLastError());
     }
 

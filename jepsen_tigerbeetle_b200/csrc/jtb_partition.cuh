@@ -38,21 +38,17 @@ __global__ void pt_balances(const int64_t* __restrict__ credits, const int64_t* 
     if (i < n) out[i] = (int32_t)(credits[i] - debits[i]);
 }
 
-inline int run_partition_by_key(cudaStream_t st, int64_t n, const int64_t* event_key, int32_t* order, int64_t* shard_off,
-                                int64_t* key_ids, int32_t key_cap, int32_t* n_keys, std::string& err) {
-    *n_keys = 0;
-    if (n <= 0) { if (key_cap >= 0) shard_off[0] = 0; return 0; }
-    if (n >= (1ll << 31)) { err = "too many events"; return -2; }
+// The device half of the partition, on keys already on the device: d_key[0, n) (0 < n < 2^31) -> *d_order (the event
+// indices in partition order), d_off / d_ids (the first event and key of each run, up to key_cap of them) and *n_runs.
+// Everything it allocates lives on A.
+inline int partition_by_key_device(cudaStream_t st, CallAllocs& A, int64_t n, const int64_t* d_key, int32_t** d_order,
+                                   int64_t* d_off, int64_t* d_ids, int32_t key_cap, int32_t* n_runs, std::string& err) {
     const unsigned grid = (unsigned)((n + 255) / 256);
-    CallAllocs A;
-    const int64_t* d_key;
     uint64_t *d_k0, *d_k1;
     int32_t *d_i0, *d_i1, *d_head, *d_run;
-    int64_t *d_off, *d_ids;
     uint8_t* d_tmp;
-    JTB_OK(A.put(&d_key, event_key, (size_t)n, st)); JTB_OK(A.alloc(&d_k0, n)); JTB_OK(A.alloc(&d_k1, n));
+    JTB_OK(A.alloc(&d_k0, n)); JTB_OK(A.alloc(&d_k1, n));
     JTB_OK(A.alloc(&d_i0, n)); JTB_OK(A.alloc(&d_i1, n)); JTB_OK(A.alloc(&d_head, n)); JTB_OK(A.alloc(&d_run, n));
-    JTB_OK(A.alloc(&d_off, (size_t)key_cap + 1)); JTB_OK(A.alloc(&d_ids, (size_t)key_cap + 1));
     pt_init<<<grid, 256, 0, st>>>(d_key, n, d_k0, d_i0);
     size_t tmp_sort = 0, tmp_scan = 0;
     JTB_OK(cub::DeviceRadixSort::SortPairs(nullptr, tmp_sort, (const uint64_t*)d_k0, d_k1, (const int32_t*)d_i0, d_i1, (int)n, 0, 64, st));
@@ -65,9 +61,25 @@ inline int run_partition_by_key(cudaStream_t st, int64_t n, const int64_t* event
     JTB_OK(cub::DeviceScan::InclusiveSum(d_tmp, tb, (const int32_t*)d_head, d_run, (int)n, st));
     pt_emit<<<grid, 256, 0, st>>>(d_k1, d_head, d_run, n, d_off, d_ids, key_cap);
     JTB_OK(cudaGetLastError());
+    JTB_OK(cudaMemcpyAsync(n_runs, d_run + (n - 1), 4, cudaMemcpyDeviceToHost, st));
+    *d_order = d_i1;
+    return 0;
+}
+
+inline int run_partition_by_key(cudaStream_t st, int64_t n, const int64_t* event_key, int32_t* order, int64_t* shard_off,
+                                int64_t* key_ids, int32_t key_cap, int32_t* n_keys, std::string& err) {
+    *n_keys = 0;
+    if (n <= 0) { if (key_cap >= 0) shard_off[0] = 0; return 0; }
+    if (n >= (1ll << 31)) { err = "too many events"; return -2; }
+    CallAllocs A;
+    const int64_t* d_key;
+    int32_t* d_order;
+    int64_t *d_off, *d_ids;
+    JTB_OK(A.put(&d_key, event_key, (size_t)n, st));
+    JTB_OK(A.alloc(&d_off, (size_t)key_cap + 1)); JTB_OK(A.alloc(&d_ids, (size_t)key_cap + 1));
     int32_t total = 0;
-    JTB_OK(cudaMemcpyAsync(&total, d_run + (n - 1), 4, cudaMemcpyDeviceToHost, st));
-    JTB_OK(cudaMemcpyAsync(order, d_i1, n * 4, cudaMemcpyDeviceToHost, st));
+    if (partition_by_key_device(st, A, n, d_key, &d_order, d_off, d_ids, key_cap, &total, err) != 0) return -1;
+    JTB_OK(cudaMemcpyAsync(order, d_order, n * 4, cudaMemcpyDeviceToHost, st));
     JTB_OK(cudaStreamSynchronize(st));
     if (total > key_cap) { err = "key_cap too small"; return -4; }
     JTB_OK(cudaMemcpy(shard_off, d_off, (size_t)total * 8, cudaMemcpyDeviceToHost));

@@ -198,3 +198,13 @@ def read_ledger_flat(path, form: str, ctx=None):
     with native.Context(device=0) as c:
         return c.read_ledger_edn(path, form)
 
+
+def read_set_flat(path, ctx=None):
+    """history.edn (a path or its bytes) of a set-full test -> the FlatHistory
+    flatten_ops(read_history(text, independent=True), "set") makes, one shard per key, read on the GPU (K20,
+    `Context.read_set_edn`).  ctx: a native.Context to use; None opens one on device 0 for this call."""
+    from . import native
+    if ctx is not None:
+        return ctx.read_set_edn(path)
+    with native.Context(device=0) as c:
+        return c.read_set_edn(path)

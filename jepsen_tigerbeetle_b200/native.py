@@ -21,7 +21,8 @@ _DEPS = _SOURCES + ["jtb_prep.h", "jtb_expand.h", "jtb_wgl.cuh", "jtb_scout.cuh"
                     "jtb_table_bench.cuh", "jtb_level.cuh", "jtb_partition.cuh", "jtb_monotonic.cuh",
                     "jtb_counter_bounds.cuh", "jtb_transfer_lookups.cuh", "jtb_read_explanations.cuh",
                     "jtb_read_gaps.cuh", "jtb_transfer_placement.cuh", "jtb_serial_witness.cuh", "jtb_repaired_witness.cuh",
-                    "jtb_lifted_witness.cuh", "jtb_class_witness.cuh", "jtb_lookup_witness.cuh", "jtb_witness.cuh", "jtb_edn.cuh", "jtb_edn_checks.cuh", "jtb_call.cuh"]
+                    "jtb_lifted_witness.cuh", "jtb_class_witness.cuh", "jtb_lookup_witness.cuh", "jtb_witness.cuh", "jtb_edn.cuh", "jtb_edn_checks.cuh", "jtb_set_edn.cuh",
+                    "jtb_call.cuh"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared", "-ldl"]
 
@@ -31,7 +32,7 @@ EXPORTS = ["jtb_abi_version", "jtb_device_count", "jtb_create", "jtb_destroy", "
            "jtb_check_read_gaps", "jtb_check_transfer_placement", "jtb_check_serial_witness",
            "jtb_check_repaired_witness", "jtb_check_lifted_witness", "jtb_check_class_witness",
            "jtb_check_lookup_witness", "jtb_read_ledger_edn", "jtb_edn_history_free",
-           "jtb_ledger_edn_checks", "jtb_edn_checks_free",
+           "jtb_ledger_edn_checks", "jtb_edn_checks_free", "jtb_read_set_edn",
            "jtb_table_bench", "jtb_get_stats", "jtb_struct_size", "jtb_prepare_seconds", "jtb_prepare_info",
            "jtb_final_configs", "jtb_gather_bench", "jtb_host_alloc", "jtb_host_free", "jtb_partition_by_key", "jtb_ledger_balances", "jtb_multi_create", "jtb_multi_create_error", "jtb_multi_destroy", "jtb_multi_n_gpus",
            "jtb_multi_last_error", "jtb_multi_check_linearizable", "jtb_multi_check_set_full"]
@@ -42,6 +43,11 @@ _lock = threading.Lock()
 
 class NativeError(RuntimeError):
     pass
+
+
+class EdnRefused(NativeError):
+    """A stored-history reader refused its input (rc -2): the EDN, or a value in it, is one the Python path raises on
+    or one the device cannot read exactly; the message names the byte and the reason."""
 
 
 def build(force: bool = False) -> str:
@@ -103,6 +109,7 @@ def lib() -> C.CDLL:
             L.jtb_edn_history_free.argtypes = [C.c_void_p]
             L.jtb_ledger_edn_checks.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p]
             L.jtb_edn_checks_free.argtypes = [C.c_void_p]
+            L.jtb_read_set_edn.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p]
             L.jtb_table_bench.argtypes = [C.c_void_p, C.c_uint64, C.c_int, C.c_int, C.c_void_p,
                                           C.c_void_p, C.c_void_p]
             L.jtb_gather_bench.argtypes = [C.c_void_p, C.c_uint64, C.c_int, C.c_int, C.c_uint32, C.c_int, C.c_int,
@@ -392,6 +399,18 @@ class Context:
         seconds_kernel, seconds_d2h, seconds_total and n_ops."""
         if form not in abi.FORMS:
             raise ValueError(f"unknown ledger form {form!r}")
+        return self._read_edn("jtb_read_ledger_edn", data, form, timings, abi.FORMS[form])
+
+    # ---- K20: a stored set-full history.edn read on the device ----------------------------------------------------
+    def read_set_edn(self, data, timings: dict | None = None) -> FlatHistory:
+        """The bytes of a set-full history.edn (bytes, bytearray, memoryview, or a path) flattened on the device into the
+        keyed "set" form: the arrays flatten_ops(edn.read_history(text, independent=True), "set") makes, one shard per
+        key and the unkeyed events last (key id -1), in page-locked memory the returned FlatHistory owns.  Raises
+        NativeError where the Python path raises or the EDN is outside the subset Jepsen's store writes.  `timings`, when
+        given, receives the call's seconds_h2d, seconds_kernel, seconds_d2h, seconds_total and n_ops."""
+        return self._read_edn("jtb_read_set_edn", data, "set", timings)
+
+    def _read_edn(self, fn: str, data, form: str, timings: dict | None, *args) -> FlatHistory:
         if isinstance(data, (str, os.PathLike)):
             with open(data, "rb") as fh:
                 data = fh.read()
@@ -400,9 +419,9 @@ class Context:
         n = len(data)
         keep = C.c_char_p(data)   # the bytes object's own buffer, no copy
         out = abi.CEdnHistory()
-        rc = lib().jtb_read_ledger_edn(self._h, C.cast(keep, C.c_void_p), n, abi.FORMS[form], 0, C.addressof(out))
+        rc = getattr(lib(), fn)(self._h, C.cast(keep, C.c_void_p), n, *args, 0, C.addressof(out))
         if rc != 0:
-            raise NativeError(f"jtb_read_ledger_edn rc={rc}: {self._err()}")
+            raise (EdnRefused if rc == -2 else NativeError)(f"{fn} rc={rc}: {self._err()}")
         if timings is not None:
             timings.update(seconds_h2d=out.seconds_h2d, seconds_kernel=out.seconds_kernel,
                            seconds_d2h=out.seconds_d2h, seconds_total=out.seconds_total, n_ops=out.n_ops)
@@ -625,11 +644,11 @@ def _owned_flat(out, form: str) -> FlatHistory:
         ("time_ns", np.int64), ("a", np.int32), ("b", np.int32), ("c", np.int32), ("payload_off", np.int64),
         ("payload_len", np.int32))}
     meta = {"model": form}
-    if form != "bank":
+    if form in ("ledger-counters", "ledger-lookups"):
         meta["multi_transfer_txns"] = int(out.multi_transfer_txns)
     return FlatHistory(payload=owner.view(h.payload, np.int32, h.n_payload),
-                       shard_off=owner.view(h.shard_off, np.int64, 2), key_ids=owner.view(h.key_ids, np.int64, 1),
-                       meta=meta, **arr)
+                       shard_off=owner.view(h.shard_off, np.int64, h.n_shards + 1),
+                       key_ids=owner.view(h.key_ids, np.int64, h.n_shards), meta=meta, **arr)
 
 
 def device_count() -> int:

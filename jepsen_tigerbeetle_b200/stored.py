@@ -1,4 +1,4 @@
-"""Stored ledger histories: seeded ledger op maps, and the EDN text Jepsen's store writes for them.
+"""Stored ledger and set-full histories: seeded op maps, and the EDN text Jepsen's store writes for them.
 
 `ledger_ops` turns a ledger-lookups FlatHistory (`synth.generate_ledger_lookups`) back into the op maps a ledger test
 records (tests/ledger.clj:27-87): transfers as [[:t id {:debit-acct d :credit-acct c :amount a}]], reads as
@@ -7,6 +7,9 @@ records (tests/ledger.clj:27-87): transfers as [[:t id {:debit-acct d :credit-ac
 `#jepsen.history.Op{...}` per line (or one vector of op maps), keywords for keyword-like strings, EDN strings for the
 rest.  Tests and `scripts/edn_read_bench.py` use both to feed the device reader (`Context.read_ledger_edn`) and the
 Python path (`edn.read_history` + `history.flatten_ops`) the same bytes.
+
+`set_ops` does the same for a keyed set history (`synth.config_c4` and friends): the op maps a set-full test records
+(workloads/set_full.clj:29-45, 107-134), for `Context.read_set_edn` and `edn.read_history(text, independent=True)`.
 """
 from __future__ import annotations
 
@@ -16,8 +19,8 @@ from typing import Any, Iterable, Mapping
 import numpy as np
 
 from . import synth
-from .history import (F_LOOKUP, F_READ, F_TRANSFER, FLAG_FINAL, T_INVOKE, T_OK, TRANSFER_RECORD, FlatHistory,
-                      transfer_id)
+from .history import (F_ADD, F_LOOKUP, F_READ, F_TRANSFER, FLAG_FINAL, T_INFO, T_INVOKE, T_OK, TRANSFER_RECORD,
+                      FlatHistory, transfer_id)
 
 TYPE_NAME = {0: "invoke", 1: "ok", 2: "fail", 3: "info"}
 _KEYWORD = re.compile(r"[A-Za-z*+!_?<>=-][A-Za-z0-9*+!_?<>=./-]*\Z")
@@ -106,6 +109,43 @@ def generate_ledger_ops(spec: synth.SynthSpec, p_lookup: float = 0.0, nemesis_ev
     transfers from spec.p_info, mid-run lookups from p_lookup, and the final phase (one :final? read, then one :final?
     lookup per client returning every committed transfer) when spec.final_reads."""
     return ledger_ops(synth.generate_ledger_lookups(spec, p_lookup=p_lookup, **mutations), nemesis_every)
+
+
+def set_ops(h: FlatHistory, nemesis_every: int = 0) -> list[dict]:
+    """The op maps of a keyed set history, in history order across keys (by :index): `flatten_ops(
+    edn.read_history(write_edn(set_ops(h)), independent=True), "set")` has h's events, keys and read payloads.  An add is
+    [k id] on its invoke and completion; a read invoke is [k nil] and an :ok read [k #{ids}]; an :info completion
+    repeats its invoke's value with :error :timeout; the final reads carry :final? true.  nemesis_every > 0 inserts a
+    nemesis op before every nemesis_every-th client op, as `ledger_ops` does."""
+    key = np.repeat(h.key_ids, np.diff(h.shard_off))
+    ops: list[dict] = []
+    for c, e in enumerate(np.argsort(h.index, kind="stable")):
+        t, k = int(h.type[e]), int(key[e])
+        if h.f[e] == F_ADD:
+            f, value = "add", (k, int(h.a[e]))
+        elif h.f[e] == F_READ:
+            pl = h.payload[h.payload_off[e]:h.payload_off[e] + max(int(h.payload_len[e]), 0)]
+            f, value = "read", (k, frozenset(int(x) for x in pl) if t == T_OK else None)
+        else:
+            raise ValueError(f"event {e}: not a set-full :add or :read")
+        op = {"index": int(h.index[e]), "time": int(h.time_ns[e]), "type": TYPE_NAME[t], "process": int(h.process[e]),
+              "f": f, "value": value}
+        if t == T_INFO:
+            op["error"] = "timeout"
+        if h.flags[e] & FLAG_FINAL:
+            op["final?"] = True
+        if nemesis_every > 0 and c % nemesis_every == nemesis_every - 1:
+            ops.append(_nemesis_op(len(ops), int(h.time_ns[e])))
+        ops.append(op)
+    return ops
+
+
+def generate_set_ops(spec: synth.SynthSpec, nemesis_every: int = 0) -> list[dict]:
+    """Seeded set-full op maps: `set_ops(synth.generate(spec))` for a spec of model "set" (e.g. the shapes of
+    synth.config_c1 and config_c4)."""
+    if spec.model != "set":
+        raise ValueError(f"a set-full history needs a spec of model 'set', not {spec.model!r}")
+    return set_ops(synth.generate(spec), nemesis_every)
 
 
 def _value(v: Any, memo: dict | None = None) -> str:
